@@ -508,6 +508,92 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t matcher, b200_lba_t opt,
  * 4 edge build, 5 pose optimisation + scatter, 6 whole chain (CUDA events on the stream). */
 int b200_track_stage_ms(b200_matcher_t matcher, int stage, float* ms);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * New landmarks of the mapping module: module::two_view_triangulator (src/stella_vslam/module/two_view_triangulator.{h,cc}, with
+ * solve::triangulator::triangulate, solve/triangulator.h:77-90, and data::triangulate_stereo, data/common.cc:192-260) and the
+ * numeric chain of mapping_module::create_new_landmarks after the baseline test (mapping_module.cc, triangulate_with_two_keyframes).
+ * Linear triangulation takes the null vector of the 4x4 system by a two-sided Jacobi SVD in the manner of Eigen::JacobiSVD; all
+ * arithmetic follows the CPU restatement's evaluation order (fp64 / fp32 where the reference uses each, no contraction).  atan2 /
+ * cos / asin are CUDA's libm (within 1-2 ulp of glibc); they feed accept / reject comparisons only (DESIGN.md section 4).
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* One keyframe as the triangulator reads it.  b200_camera_t lacks the fields below and keeps its layout. */
+typedef struct b200_tri_keyframe {
+    double pose_cw[16];             /* keyframe::get_pose_cw(), row-major 4x4 */
+    double pose_wc[16];             /* keyframe::get_pose_wc() as the keyframe stores it (camera centre = column 3) */
+    int32_t model;                  /* 0: perspective family (perspective / fisheye / radial division), 1: equirectangular */
+    double fx, fy, cx, cy, fx_inv, fy_inv; /* camera::perspective (fisheye, radial_division) members */
+    double focal_x_baseline, true_baseline; /* camera::base */
+    double cols, rows;              /* equirectangular */
+    float scale_factor;             /* orb_params_->scale_factor_ */
+    int32_t num_levels;             /* entries of the two tables below */
+    const float* scale_factors;     /* orb_params_->scale_factors_ */
+    const float* level_sigma_sq;    /* orb_params_->level_sigma_sq_ */
+    int32_t n_keypoints;
+    const float* x;                 /* frm_obs_.undist_keypts_[i].pt.x */
+    const float* y;
+    const int32_t* octave;          /* undist_keypts_[i].octave */
+    const float* x_right;           /* frm_obs_.stereo_x_right_, NULL when empty (monocular) */
+    const float* depth;             /* frm_obs_.depths_, NULL when empty */
+    const double* bearings;         /* frm_obs_.bearings_, n x 3 */
+} b200_tri_keyframe_t;
+
+/* two_view_triangulator(keyfrm_1, keyfrm_2, rays_parallax_deg_thr).triangulate(idx_1, idx_2, pos_w) for every match of every problem,
+ * in one upload, one launch and one download.  cos(deg * pi / 180) and ratio_factor_ are taken on the host as the constructor does.
+ * Out per match: pos_w (3 doubles; the point computed before the depth / reprojection / scale tests, zeros when neither triangulation
+ * branch applied) and ok (1 = the reference returns true); n_ok.  B200_ERR_INVALID (nothing written) for an index or octave out of
+ * range and for a stereo keypoint (x_right >= 0) on an equirectangular camera, which the reference does not implement (it throws). */
+typedef struct b200_triangulate_problem {
+    const b200_tri_keyframe_t* keyfrm_1;
+    const b200_tri_keyframe_t* keyfrm_2;
+    float rays_parallax_deg_thr;    /* the mapping module passes 1.0 */
+    int32_t n_matches;
+    const int32_t* matches;         /* n_matches x (idx_1, idx_2) */
+    double* pos_w;                  /* out, n_matches x 3 */
+    uint8_t* ok;                    /* out, n_matches */
+    int32_t n_ok;                   /* out */
+} b200_triangulate_problem_t;
+int b200_triangulate_pairs(b200_matcher_t h, int n_problems, b200_triangulate_problem_t* problems);
+
+/* mapping_module::create_new_landmarks after the baseline test, for `n_keyframes` current keyframes (several maps / streams, or a
+ * backlog) in ONE launch sequence: one upload, one candidate pass of match_for_triangulation (variant B200_PAIRS_TRIANGULATION of
+ * b200_match_pairs, check_orientation = false as the mapping module builds it) over every (keyframe, neighbour) problem, then per
+ * neighbour rank the sequential resolve and the triangulation of that rank's matches, one download and one synchronisation.
+ * Neighbours are processed in the caller's order (get_top_n_covisibilities); every created landmark attaches to its row of the current
+ * keyframe, so the later neighbours no longer match that row (robust.cc:44-48) -- the dependency that makes the reference loop
+ * sequential, kept on the device.  The caller builds E_12 and the epiplane with the reference's own code, as for b200_match_pairs.
+ * Output per keyframe: the landmarks in creation order (neighbour rank, then ascending idx_1), i.e. the order of next_landmark_id_.
+ * Deviation: the reference polls abort_create_new_landmarks between neighbours (from the second one on); this chain is not
+ * interruptible, so the caller tests the flag before the call and the result is the reference's outcome without an abort (which
+ * in the reference depends on timing).  B200_ERR_CAPACITY as b200_match_pairs (max_candidates 0 = 64 gated candidates per row;
+ * on-chip occupancy table bounds the neighbours' keypoint counts); B200_ERR_INVALID as b200_triangulate_pairs, checked over every
+ * keypoint of the views. */
+typedef struct b200_new_landmarks_neighbour {
+    const b200_tri_keyframe_t* keyfrm;
+    const uint8_t* desc;            /* n_keypoints x 32 */
+    const uint8_t* valid;           /* keypoint has no landmark (robust.cc:66-69); NULL = all */
+    const int32_t* node;            /* BoW node per keypoint (bow_tree::match_for_triangulation); NULL iff the current keyframe's is NULL */
+    double E_12[9];                 /* row-major, essential_solver::create_E_21(keyfrm_1, keyfrm_2) */
+    double epiplane_in_keyfrm_2[3];
+    int32_t valid_epiplane;
+    int32_t* match_out;             /* optional out, current keyframe's n_keypoints: the matcher's result for this neighbour */
+    int32_t n_matches;              /* out: the return value of match_for_triangulation */
+    int32_t n_created;              /* out: landmarks created with this neighbour */
+} b200_new_landmarks_neighbour_t;
+typedef struct b200_new_landmarks_problem {
+    const b200_tri_keyframe_t* keyfrm; /* the current keyframe (side 1 of every match) */
+    const uint8_t* desc;
+    const uint8_t* valid;           /* keypoint has no landmark at entry; NULL = all */
+    const int32_t* node;
+    int32_t n_neighbours;
+    b200_new_landmarks_neighbour_t* neighbours; /* ordered */
+    int32_t* created_rank;          /* out, capacity n_keypoints: neighbour rank of each created landmark */
+    int32_t* created_idx;           /* out, capacity n_keypoints x (idx_1, idx_2) */
+    double* created_pos_w;          /* out, capacity n_keypoints x 3 */
+    int32_t n_created;              /* out */
+} b200_new_landmarks_problem_t;
+int b200_create_new_landmarks(b200_matcher_t h, int n_keyframes, b200_new_landmarks_problem_t* problems, float lowe_ratio, float residual_rad_thr,
+                              float rays_parallax_deg_thr, int max_candidates);
+
 /* Profiling mode: an event after every launch of the following solves (adds a few microseconds per launch; off by default).
  * b200_lba_kernel_ms reports, for the LAST batch, the summed device time and the number of intervals of
  *   kernel 0 plan (5 launches, one interval), 1 landmark pass / build, 2 keyframe rows, 3 Schur rows, 4 reduced-system Cholesky,

@@ -425,4 +425,57 @@ private:
     optimize::pose_optimizer opt_;
 };
 }  // namespace tracking
+
+namespace mapping {
+// module::two_view_triangulator (module/two_view_triangulator.h): triangulate(matches) over (idx_1, idx_2) pairs (b200_triangulate_pairs)
+class two_view_triangulator {
+public:
+    two_view_triangulator(const b200_tri_keyframe_t& keyfrm_1, const b200_tri_keyframe_t& keyfrm_2, float rays_parallax_deg_thr = 1.0f,
+                          int device = 0)
+        : k1_(keyfrm_1), k2_(keyfrm_2), deg_(rays_parallax_deg_thr), m_(device) {}
+    // pos_w: 3 per match, ok: 1 per match; returns the number accepted
+    int triangulate(const std::vector<std::pair<int32_t, int32_t>>& matches, std::vector<double>& pos_w, std::vector<uint8_t>& ok) {
+        std::vector<int32_t> flat(2 * matches.size());
+        for (size_t k = 0; k < matches.size(); ++k) {
+            flat[2 * k] = matches[k].first;
+            flat[2 * k + 1] = matches[k].second;
+        }
+        pos_w.assign(3 * matches.size(), 0.0);
+        ok.assign(matches.size(), 0);
+        b200_triangulate_problem_t P{};
+        P.keyfrm_1 = &k1_;
+        P.keyfrm_2 = &k2_;
+        P.rays_parallax_deg_thr = deg_;
+        P.n_matches = static_cast<int32_t>(matches.size());
+        P.matches = flat.data();
+        P.pos_w = pos_w.data();
+        P.ok = ok.data();
+        check(b200_triangulate_pairs(m_.get(), 1, &P), "b200_triangulate_pairs");
+        return P.n_ok;
+    }
+
+private:
+    b200_tri_keyframe_t k1_, k2_;
+    float deg_;
+    match::device_matcher m_;
+};
+
+// mapping_module::create_new_landmarks after the baseline test, for a batch of current keyframes (b200_create_new_landmarks); the
+// problems' created_* / per-neighbour outputs are filled in place.  Defaults: the mapping module's matchers (lowe_ratio 0.95,
+// residual 0.2 degrees) and triangulator (1 degree).
+class new_landmark_creator {
+public:
+    explicit new_landmark_creator(int device = 0, float lowe_ratio = 0.95f, float residual_rad_thr = 0.2f * 3.14159265358979f / 180.0f,
+                                  float rays_parallax_deg_thr = 1.0f)
+        : m_(device), lowe_(lowe_ratio), residual_(residual_rad_thr), deg_(rays_parallax_deg_thr) {}
+    void create(std::vector<b200_new_landmarks_problem_t>& problems, int max_candidates = 0) {
+        check(b200_create_new_landmarks(m_.get(), static_cast<int>(problems.size()), problems.data(), lowe_, residual_, deg_, max_candidates),
+              "b200_create_new_landmarks");
+    }
+
+private:
+    match::device_matcher m_;
+    float lowe_, residual_, deg_;
+};
+}  // namespace mapping
 }  // namespace b200

@@ -22,6 +22,7 @@
 
 #include "common.cuh"
 #include "track_chain.cuh"
+#include "triangulate.cuh"
 
 namespace b200 {
 namespace match {
@@ -2471,3 +2472,531 @@ int b200_hamming_matrix(b200_matcher_t h, const uint8_t* desc1, int n1, const ui
 }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------
+// New landmarks of the mapping module (mapping_module::create_new_landmarks, src/stella_vslam/mapping_module.cc, and
+// module::two_view_triangulator): the triangulation device function lives in triangulate.cuh.
+//   b200_triangulate_pairs    : one thread per match over every problem of the call (flattened offsets)
+//   b200_create_new_landmarks : pairs_candidates_kernel over every (keyframe, neighbour) problem, then per neighbour rank the
+//                               resolve (guided_resolve_kernel, mode 6) and landmark_claim_kernel, which triangulates that rank's
+//                               matches, appends the landmarks in idx_1 order and closes the rows it created a landmark on to the
+//                               later ranks (list_len = 0: match_for_triangulation skips a keypoint with a landmark, robust.cc:44-48)
+// ---------------------------------------------------------------------------------------------------------------
+namespace b200 {
+namespace mapping {
+
+using match::PairsDev;
+using tri::TriKfDev;
+
+struct TriProblemDev {
+    int k1, k2;  // rows of the keyframe table
+    float cos_thr, ratio_factor;
+    int begin;   // first match of the problem in the flattened arrays
+};
+
+__global__ void __launch_bounds__(256) triangulate_pairs_kernel(const TriKfDev* __restrict__ kfs, const TriProblemDev* __restrict__ ps, int n_problems,
+                                                                int total, const int2* __restrict__ matches, double* __restrict__ pos_w,
+                                                                unsigned char* __restrict__ ok, int* __restrict__ unconverged) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= total) return;
+    int lo = 0, hi = n_problems - 1;  // last problem that starts at or before t
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (ps[mid].begin <= t) lo = mid;
+        else hi = mid - 1;
+    }
+    const TriProblemDev& P = ps[lo];
+    const int2 m = matches[t];
+    double p[3];
+    const int r = tri::two_view_triangulate(kfs[P.k1], kfs[P.k2], m.x, m.y, P.cos_thr, P.ratio_factor, p);
+    if (r < 0) atomicAdd(unconverged, 1);
+    pos_w[3 * (size_t)t] = p[0];
+    pos_w[3 * (size_t)t + 1] = p[1];
+    pos_w[3 * (size_t)t + 2] = p[2];
+    ok[t] = r == 1;
+}
+
+struct ChainKfDev {
+    int cur;       // row of the current keyframe in the keyframe table
+    int n_nb;      // neighbours (ranks)
+    int nb_begin;  // row of its rank-0 neighbour in the keyframe table and in nb_consts (the ranks follow)
+    int* n_created_rank;  // [n_nb]
+    int* n_created;       // [1], running count
+    int* created_rank;
+    int2* created_idx;
+    double* created_pos;
+};
+
+constexpr int kClaimThreads = 256;
+
+__global__ void __launch_bounds__(kClaimThreads) landmark_claim_kernel(const TriKfDev* __restrict__ kfs, const float2* __restrict__ nb_consts, const ChainKfDev* __restrict__ ks,
+                                                                       const PairsDev* __restrict__ pairs, int n_kf, int rank,
+                                                                       int* __restrict__ unconverged) {
+    __shared__ int warp_total[kClaimThreads / 32];
+    const ChainKfDev K = ks[blockIdx.x];
+    if (rank >= K.n_nb) return;
+    const PairsDev& g = pairs[(size_t)rank * n_kf + blockIdx.x];
+    const TriKfDev& k1 = kfs[K.cur];
+    const TriKfDev& k2 = kfs[K.nb_begin + rank];
+    const float2 c = nb_consts[K.nb_begin + rank];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int base = *K.n_created;  // written by this keyframe's block of the previous rank (stream order)
+    int made = 0;
+    for (int c0 = 0; c0 < g.n_queries; c0 += kClaimThreads) {
+        const int i = c0 + threadIdx.x;
+        const int j = i < g.n_queries ? g.match_out[i] : -1;
+        double p[3];
+        bool ok = false;
+        if (j >= 0) {
+            const int r = tri::two_view_triangulate(k1, k2, i, j, c.x, c.y, p);
+            if (r < 0) atomicAdd(unconverged, 1);
+            ok = r == 1;
+        }
+        // ordered compaction: rows in ascending idx_1 (the order of matched_idx_pairs, robust.cc:135-143)
+        const unsigned bal = __ballot_sync(0xFFFFFFFFu, ok);
+        if (lane == 0) warp_total[warp] = __popc(bal);
+        __syncthreads();
+        int off = 0, chunk = 0;
+#pragma unroll
+        for (int w = 0; w < kClaimThreads / 32; ++w) {
+            off += w < warp ? warp_total[w] : 0;
+            chunk += warp_total[w];
+        }
+        if (ok) {
+            const int at = base + off + __popc(bal & ((1u << lane) - 1u));
+            K.created_rank[at] = rank;
+            K.created_idx[at] = make_int2(i, j);
+            K.created_pos[3 * (size_t)at] = p[0];
+            K.created_pos[3 * (size_t)at + 1] = p[1];
+            K.created_pos[3 * (size_t)at + 2] = p[2];
+            for (int r2 = rank + 1; r2 < K.n_nb; ++r2) pairs[(size_t)r2 * n_kf + blockIdx.x].list_len[i] = 0;
+        }
+        base += chunk;
+        made += chunk;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        *K.n_created = base;
+        K.n_created_rank[rank] = made;
+    }
+}
+
+// host-side staging: caller arrays are packed into one pinned buffer and go up in one copy
+struct Stage {
+    struct Item {
+        size_t off;
+        const void* src;
+        size_t bytes;
+    };
+    std::vector<Item> items;
+    size_t o = 0;
+    static size_t al(size_t v) { return round_up(v, (size_t)256); }
+    size_t add(const void* src, size_t bytes) {
+        const size_t at = o;
+        items.push_back({at, src, src ? bytes : 0});
+        o += al(std::max(bytes, (size_t)1));
+        return at;
+    }
+    size_t reserve(size_t bytes) {
+        const size_t at = o;
+        o += al(std::max(bytes, (size_t)1));
+        return at;
+    }
+};
+
+struct KfLay {
+    size_t x, y, oct, xr, dep, b, sf, ls;
+};
+
+bool kf_valid(const b200_tri_keyframe_t* K) {
+    if (!K || K->n_keypoints < 0 || (K->model != 0 && K->model != 1) || K->num_levels < 1 || K->num_levels > 64 || !K->scale_factors
+        || !K->level_sigma_sq)
+        return false;
+    return K->n_keypoints == 0 || (K->x && K->y && K->octave && K->bearings);
+}
+
+// octave of keypoint i in range, and no stereo keypoint on an equirectangular camera (data/common.cc:240-242 throws there)
+bool kp_valid(const b200_tri_keyframe_t* K, int i) {
+    return i >= 0 && i < K->n_keypoints && K->octave[i] >= 0 && K->octave[i] < K->num_levels
+           && !(K->model == 1 && K->x_right && K->x_right[i] >= 0.0f);
+}
+
+KfLay stage_kf(Stage& s, const b200_tri_keyframe_t* K) {
+    const size_t n = (size_t)K->n_keypoints, nl = (size_t)K->num_levels;
+    KfLay L;
+    L.x = s.add(K->x, 4 * n);
+    L.y = s.add(K->y, 4 * n);
+    L.oct = s.add(K->octave, 4 * n);
+    L.xr = s.add(K->x_right, 4 * n);
+    L.dep = s.add(K->depth, 4 * n);
+    L.b = s.add(K->bearings, 24 * n);
+    L.sf = s.add(K->scale_factors, 4 * nl);
+    L.ls = s.add(K->level_sigma_sq, 4 * nl);
+    return L;
+}
+
+TriKfDev make_kf(const b200_tri_keyframe_t* K, const KfLay& L, unsigned char* db) {
+    TriKfDev d{};
+    std::memcpy(d.pose_cw, K->pose_cw, sizeof(d.pose_cw));
+    std::memcpy(d.pose_wc, K->pose_wc, sizeof(d.pose_wc));
+    d.model = K->model;
+    d.fx = K->fx;
+    d.fy = K->fy;
+    d.cx = K->cx;
+    d.cy = K->cy;
+    d.fx_inv = K->fx_inv;
+    d.fy_inv = K->fy_inv;
+    d.fxb = K->focal_x_baseline;
+    d.true_baseline = K->true_baseline;
+    d.cols = K->cols;
+    d.rows = K->rows;
+    d.x = (const float*)(db + L.x);
+    d.y = (const float*)(db + L.y);
+    d.octave = (const int*)(db + L.oct);
+    d.x_right = K->x_right ? (const float*)(db + L.xr) : nullptr;
+    d.depth = K->depth ? (const float*)(db + L.dep) : nullptr;
+    d.bearings = (const double*)(db + L.b);
+    d.scale_factors = (const float*)(db + L.sf);
+    d.level_sigma_sq = (const float*)(db + L.ls);
+    return d;
+}
+
+// the triangulator's constructor (two_view_triangulator.cc:15-16): ratio_factor_ and cos_rays_parallax_thr_ are floats
+float2 tri_constants(const b200_tri_keyframe_t* k1, const b200_tri_keyframe_t* k2, float rays_parallax_deg_thr) {
+    const float cos_thr = (float)std::cos(rays_parallax_deg_thr * M_PI / 180.0);
+    const float ratio_factor = 2.0f * std::max(k1->scale_factor, k2->scale_factor);
+    return make_float2(cos_thr, ratio_factor);
+}
+
+}  // namespace mapping
+}  // namespace b200
+
+int b200_triangulate_pairs(b200_matcher_t h, int n_problems, b200_triangulate_problem_t* problems) {
+    B200_RANGE("b200:mapping:triangulate");
+    using namespace b200::mapping;
+    if (!h || n_problems < 0) return B200_ERR_INVALID;
+    if (n_problems == 0) return B200_OK;
+    if (!problems) return B200_ERR_INVALID;
+    auto& m = h->m;
+    B200_CUDA(cudaSetDevice(m.device));
+    // keyframe table: each distinct keyframe view goes up once
+    std::vector<const b200_tri_keyframe_t*> kf_list;
+    auto kf_row = [&](const b200_tri_keyframe_t* K) {
+        for (size_t r = 0; r < kf_list.size(); ++r)
+            if (kf_list[r] == K) return (int)r;
+        kf_list.push_back(K);
+        return (int)kf_list.size() - 1;
+    };
+    std::vector<TriProblemDev> tp(n_problems);
+    int total = 0;
+    for (int p = 0; p < n_problems; ++p) {
+        const b200_triangulate_problem_t& P = problems[p];
+        if (!kf_valid(P.keyfrm_1) || !kf_valid(P.keyfrm_2) || P.n_matches < 0 || (P.n_matches > 0 && (!P.matches || !P.pos_w || !P.ok))) {
+            b200::set_error("b200_triangulate_pairs: bad keyframe view, size or null buffer in problem %d", p);
+            return B200_ERR_INVALID;
+        }
+        for (int k = 0; k < P.n_matches; ++k)
+            if (!kp_valid(P.keyfrm_1, P.matches[2 * k]) || !kp_valid(P.keyfrm_2, P.matches[2 * k + 1])) {
+                b200::set_error("b200_triangulate_pairs: problem %d match %d: index or octave out of range, or a stereo keypoint on an "
+                                "equirectangular camera", p, k);
+                return B200_ERR_INVALID;
+            }
+        if (total > INT_MAX - P.n_matches) return B200_ERR_INVALID;
+        const float2 c = tri_constants(P.keyfrm_1, P.keyfrm_2, P.rays_parallax_deg_thr);
+        tp[p] = TriProblemDev{kf_row(P.keyfrm_1), kf_row(P.keyfrm_2), c.x, c.y, total};
+        total += P.n_matches;
+    }
+    Stage s;
+    const size_t o_kfs = s.reserve(sizeof(TriKfDev) * kf_list.size());
+    const size_t o_ps = s.reserve(sizeof(TriProblemDev) * (size_t)n_problems);
+    std::vector<KfLay> kl;
+    for (const b200_tri_keyframe_t* K : kf_list) kl.push_back(stage_kf(s, K));
+    // every problem's (idx_1, idx_2) rows, consecutive in problem order
+    const size_t o_matches = s.reserve(8 * (size_t)std::max(total, 1));
+    const size_t in_bytes = s.o, out_begin = s.o;
+    const size_t o_pos = s.reserve(24 * (size_t)std::max(total, 1));
+    const size_t o_ok = s.reserve((size_t)std::max(total, 1));
+    const size_t o_unconv = s.reserve(4);
+    const size_t out_end = s.o;
+    int rc;
+    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, s.o))) return rc;
+    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, s.o))) return rc;
+    unsigned char *hb = m.h_guided, *db = m.d_guided;
+    for (const Stage::Item& it : s.items)
+        if (it.bytes) std::memcpy(hb + it.off, it.src, it.bytes);
+    for (int p = 0; p < n_problems; ++p)
+        if (problems[p].n_matches) std::memcpy(hb + o_matches + 8 * (size_t)tp[p].begin, problems[p].matches, 8 * (size_t)problems[p].n_matches);
+    TriKfDev* hk = reinterpret_cast<TriKfDev*>(hb + o_kfs);
+    for (size_t r = 0; r < kf_list.size(); ++r) hk[r] = make_kf(kf_list[r], kl[r], db);
+    std::memcpy(hb + o_ps, tp.data(), sizeof(TriProblemDev) * (size_t)n_problems);
+    cudaStream_t st = m.stream;
+    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaMemsetAsync(db + o_unconv, 0, 4, st));
+    if (total > 0) {
+        triangulate_pairs_kernel<<<b200::ceil_div(total, 256), 256, 0, st>>>(
+            (const TriKfDev*)(db + o_kfs), (const TriProblemDev*)(db + o_ps), n_problems, total, (const int2*)(db + o_matches),
+            (double*)(db + o_pos), db + o_ok, (int*)(db + o_unconv));
+        B200_CUDA(cudaGetLastError());
+    }
+    B200_CUDA(cudaMemcpyAsync(hb + out_begin, db + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    m.last_h2d = in_bytes;
+    m.last_d2h = out_end - out_begin;
+    const int unconverged = *reinterpret_cast<const int*>(hb + o_unconv);
+    if (unconverged > 0) {
+        b200::set_error("b200_triangulate_pairs: the 4x4 Jacobi SVD did not converge within %d sweeps for %d matches", b200::tri::kMaxSweeps,
+                        unconverged);
+        return B200_ERR_INVALID;
+    }
+    for (int p = 0; p < n_problems; ++p) {
+        b200_triangulate_problem_t& P = problems[p];
+        const size_t b = (size_t)tp[p].begin, n = (size_t)P.n_matches;
+        int n_ok = 0;
+        if (n) {
+            std::memcpy(P.pos_w, hb + o_pos + 24 * b, 24 * n);
+            std::memcpy(P.ok, hb + o_ok + b, n);
+            for (size_t k = 0; k < n; ++k) n_ok += P.ok[k];
+        }
+        P.n_ok = n_ok;
+    }
+    return B200_OK;
+}
+
+int b200_create_new_landmarks(b200_matcher_t h, int n_keyframes, b200_new_landmarks_problem_t* problems, float lowe_ratio, float residual_rad_thr,
+                              float rays_parallax_deg_thr, int max_candidates) {
+    B200_RANGE("b200:mapping:new_landmarks");
+    using namespace b200::mapping;
+    if (!h || n_keyframes < 0 || max_candidates < 0) return B200_ERR_INVALID;
+    if (n_keyframes == 0) return B200_OK;
+    if (!problems) return B200_ERR_INVALID;
+    auto& m = h->m;
+    B200_CUDA(cudaSetDevice(m.device));
+    const int cap = max_candidates ? max_candidates : 64;
+    const int n_kf = n_keyframes;
+    int n_ranks = 0, max_n1 = 0, max_n2 = 0;
+    for (int k = 0; k < n_kf; ++k) {
+        const b200_new_landmarks_problem_t& P = problems[k];
+        const b200_tri_keyframe_t* C = P.keyfrm;
+        bool bad = !kf_valid(C) || P.n_neighbours < 0 || (P.n_neighbours > 0 && !P.neighbours)
+                   || (C->n_keypoints > 0 && (!P.desc || !P.created_rank || !P.created_idx || !P.created_pos_w));
+        for (int i = 0; !bad && i < C->n_keypoints; ++i) bad = !kp_valid(C, i);
+        for (int r = 0; !bad && r < P.n_neighbours; ++r) {
+            const b200_new_landmarks_neighbour_t& N = P.neighbours[r];
+            bad = !kf_valid(N.keyfrm) || (N.keyfrm->n_keypoints > 0 && !N.desc) || ((P.node == nullptr) != (N.node == nullptr));
+            for (int i = 0; !bad && i < N.keyfrm->n_keypoints; ++i) bad = !kp_valid(N.keyfrm, i);
+            if (!bad) max_n2 = std::max(max_n2, N.keyfrm->n_keypoints);
+        }
+        if (bad) {
+            b200::set_error("b200_create_new_landmarks: keyframe %d: bad keyframe view, size, null buffer, octave out of range or a stereo "
+                            "keypoint on an equirectangular camera", k);
+            return B200_ERR_INVALID;
+        }
+        n_ranks = std::max(n_ranks, P.n_neighbours);
+        max_n1 = std::max(max_n1, C->n_keypoints);
+    }
+    if (n_ranks == 0) {
+        for (int k = 0; k < n_kf; ++k) problems[k].n_created = 0;
+        return B200_OK;
+    }
+    const size_t rs_bytes = (size_t)std::max(max_n2, 1) * 6 + 16;
+    if (rs_bytes > 200 * 1024) {
+        b200::set_error("b200_create_new_landmarks: %d keypoints per neighbour exceed the on-chip occupancy table", max_n2);
+        return B200_ERR_CAPACITY;
+    }
+    // host-derived per-keypoint inputs of the matcher: scale_factors_[octave] of the rows, stereo flags of both sides
+    std::vector<std::vector<float>> scale1(n_kf);
+    std::vector<std::vector<unsigned char>> stereo_cur(n_kf);
+    std::vector<std::vector<std::vector<unsigned char>>> stereo_nb(n_kf);
+    auto stereo_of = [](const b200_tri_keyframe_t* K, std::vector<unsigned char>& out) {
+        if (!K->x_right) return;
+        out.resize(K->n_keypoints);
+        for (int i = 0; i < K->n_keypoints; ++i) out[i] = K->x_right[i] >= 0.0f;
+    };
+    Stage s;
+    const size_t P_total = (size_t)n_ranks * n_kf;
+    const size_t o_pairs = s.reserve(sizeof(PairsDev) * P_total);
+    const size_t o_chain = s.reserve(sizeof(ChainKfDev) * n_kf);
+    int n_views = 0;
+    for (int k = 0; k < n_kf; ++k) n_views += 1 + problems[k].n_neighbours;
+    const size_t o_kfs = s.reserve(sizeof(TriKfDev) * n_views);
+    const size_t o_consts = s.reserve(8 * (size_t)n_views);
+    struct CurLay {
+        KfLay kf;
+        size_t desc, valid, node, scale, stereo;
+    };
+    struct NbLay {
+        KfLay kf;
+        size_t desc, valid, node, stereo;
+    };
+    std::vector<CurLay> cl(n_kf);
+    std::vector<std::vector<NbLay>> nl(n_kf);
+    for (int k = 0; k < n_kf; ++k) {
+        const b200_new_landmarks_problem_t& P = problems[k];
+        const b200_tri_keyframe_t* C = P.keyfrm;
+        const size_t n1 = (size_t)C->n_keypoints;
+        scale1[k].resize(n1);
+        for (size_t i = 0; i < n1; ++i) scale1[k][i] = C->scale_factors[C->octave[i]];
+        stereo_of(C, stereo_cur[k]);
+        CurLay& L = cl[k];
+        L.kf = stage_kf(s, C);
+        L.desc = s.add(P.desc, 32 * n1);
+        L.valid = s.add(P.valid, n1);
+        L.node = s.add(P.node, 4 * n1);
+        L.scale = s.add(scale1[k].data(), 4 * n1);
+        L.stereo = s.add(C->x_right ? stereo_cur[k].data() : nullptr, n1);
+        stereo_nb[k].resize(P.n_neighbours);
+        nl[k].resize(P.n_neighbours);
+        for (int r = 0; r < P.n_neighbours; ++r) {
+            const b200_new_landmarks_neighbour_t& N = P.neighbours[r];
+            const size_t n2 = (size_t)N.keyfrm->n_keypoints;
+            stereo_of(N.keyfrm, stereo_nb[k][r]);
+            NbLay& M = nl[k][r];
+            M.kf = stage_kf(s, N.keyfrm);
+            M.desc = s.add(N.desc, 32 * n2);
+            M.valid = s.add(N.valid, n2);
+            M.node = s.add(N.node, 4 * n2);
+            M.stereo = s.add(N.keyfrm->x_right ? stereo_nb[k][r].data() : nullptr, n2);
+        }
+    }
+    const size_t in_bytes = s.o, out_begin = s.o;
+    // outputs (one download): per problem match_out + n_matches, per keyframe the created list and counts, the two flags
+    std::vector<size_t> o_mout(P_total), o_nm(P_total);
+    for (int r = 0; r < n_ranks; ++r)
+        for (int k = 0; k < n_kf; ++k) {
+            const size_t q = (size_t)r * n_kf + k;
+            o_mout[q] = s.reserve(4 * (size_t)(r < problems[k].n_neighbours ? problems[k].keyfrm->n_keypoints : 0));
+            o_nm[q] = s.reserve(4);
+        }
+    struct OutLay {
+        size_t n_rank, n_created, rank, idx, pos;
+    };
+    std::vector<OutLay> ol(n_kf);
+    for (int k = 0; k < n_kf; ++k) {
+        const size_t n1 = (size_t)problems[k].keyfrm->n_keypoints;
+        ol[k].n_rank = s.reserve(4 * (size_t)std::max(problems[k].n_neighbours, 1));
+        ol[k].n_created = s.reserve(4);
+        ol[k].rank = s.reserve(4 * n1);
+        ol[k].idx = s.reserve(8 * n1);
+        ol[k].pos = s.reserve(24 * n1);
+    }
+    const size_t o_overflow = s.reserve(4), o_unconv = s.reserve(4);
+    const size_t out_end = s.o;
+    std::vector<size_t> o_lists(P_total), o_llen(P_total);
+    for (int r = 0; r < n_ranks; ++r)
+        for (int k = 0; k < n_kf; ++k) {
+            const size_t q = (size_t)r * n_kf + k;
+            const size_t n1 = r < problems[k].n_neighbours ? (size_t)problems[k].keyfrm->n_keypoints : 0;
+            o_lists[q] = s.reserve(8 * (size_t)cap * n1);
+            o_llen[q] = s.reserve(4 * n1);
+        }
+    int rc;
+    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, s.o))) return rc;
+    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, out_end))) return rc;
+    unsigned char *hb = m.h_guided, *db = m.d_guided;
+    for (const Stage::Item& it : s.items)
+        if (it.bytes) std::memcpy(hb + it.off, it.src, it.bytes);
+    TriKfDev* hk = reinterpret_cast<TriKfDev*>(hb + o_kfs);
+    float2* hc = reinterpret_cast<float2*>(hb + o_consts);
+    ChainKfDev* hch = reinterpret_cast<ChainKfDev*>(hb + o_chain);
+    PairsDev* hg = reinterpret_cast<PairsDev*>(hb + o_pairs);
+    int view = 0;
+    for (int k = 0; k < n_kf; ++k) {
+        const b200_new_landmarks_problem_t& P = problems[k];
+        const b200_tri_keyframe_t* C = P.keyfrm;
+        const int cur = view++;
+        hk[cur] = make_kf(C, cl[k].kf, db);
+        ChainKfDev K{};
+        K.cur = cur;
+        K.n_nb = P.n_neighbours;
+        K.nb_begin = view;
+        K.n_created_rank = (int*)(db + ol[k].n_rank);
+        K.n_created = (int*)(db + ol[k].n_created);
+        K.created_rank = (int*)(db + ol[k].rank);
+        K.created_idx = (int2*)(db + ol[k].idx);
+        K.created_pos = (double*)(db + ol[k].pos);
+        for (int r = 0; r < n_ranks; ++r) {
+            const size_t q = (size_t)r * n_kf + k;
+            PairsDev g{};
+            g.cap = cap;
+            g.lists = (uint2*)(db + o_lists[q]);
+            g.list_len = (int*)(db + o_llen[q]);
+            g.match_out = (int*)(db + o_mout[q]);
+            g.n_matches = (int*)(db + o_nm[q]);
+            if (r < P.n_neighbours) {
+                const b200_new_landmarks_neighbour_t& N = P.neighbours[r];
+                const NbLay& M = nl[k][r];
+                hk[view] = make_kf(N.keyfrm, M.kf, db);
+                hc[view] = tri_constants(C, N.keyfrm, rays_parallax_deg_thr);
+                ++view;
+                g.n_queries = C->n_keypoints;
+                g.n_train = N.keyfrm->n_keypoints;
+                g.desc1 = (const uint4*)(db + cl[k].desc);
+                g.desc2 = (const uint4*)(db + M.desc);
+                g.valid1 = P.valid ? db + cl[k].valid : nullptr;
+                g.valid2 = N.valid ? db + M.valid : nullptr;
+                g.stereo1 = C->x_right ? db + cl[k].stereo : nullptr;
+                g.stereo2 = N.keyfrm->x_right ? db + M.stereo : nullptr;
+                g.node1 = P.node ? (const int*)(db + cl[k].node) : nullptr;
+                g.node2 = N.node ? (const int*)(db + M.node) : nullptr;
+                g.bearing1 = hk[cur].bearings;
+                g.bearing2 = (const double*)(db + M.kf.b);
+                g.scale1 = (const float*)(db + cl[k].scale);
+                for (int e = 0; e < 9; ++e) g.E[e] = N.E_12[e];
+                for (int e = 0; e < 3; ++e) g.epi[e] = N.epiplane_in_keyfrm_2[e];
+                g.valid_epiplane = N.valid_epiplane;
+                g.residual_rad_thr = residual_rad_thr;
+            }
+            hg[q] = g;
+        }
+        hch[k] = K;
+    }
+    cudaStream_t st = m.stream;
+    const PairsDev* dg = reinterpret_cast<const PairsDev*>(db + o_pairs);
+    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaMemsetAsync(db + out_begin, 0, out_end - out_begin, st));
+    b200::match::pairs_candidates_kernel<<<dim3(std::max(1, b200::ceil_div(max_n1, b200::match::kPairRows)), (unsigned)P_total),
+                                           b200::match::kPairRows, 0, st>>>(dg, B200_PAIRS_TRIANGULATION, (unsigned)b200::match::kThrLow, 0,
+                                                                            (int*)(db + o_overflow));
+    if (rs_bytes > 48 * 1024)
+        B200_CUDA(cudaFuncSetAttribute(b200::match::guided_resolve_kernel<PairsDev>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rs_bytes));
+    for (int r = 0; r < n_ranks; ++r) {
+        b200::match::guided_resolve_kernel<PairsDev><<<n_kf, 32, rs_bytes, st>>>(dg + (size_t)r * n_kf, 6, (unsigned)b200::match::kThrLow, lowe_ratio);
+        landmark_claim_kernel<<<n_kf, kClaimThreads, 0, st>>>((const TriKfDev*)(db + o_kfs), (const float2*)(db + o_consts), (const ChainKfDev*)(db + o_chain), dg, n_kf, r,
+                                                              (int*)(db + o_unconv));
+    }
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaMemcpyAsync(hb + out_begin, db + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    m.last_h2d = in_bytes;
+    m.last_d2h = out_end - out_begin;
+    const int overflow = *reinterpret_cast<const int*>(hb + o_overflow);
+    if (overflow > 0) {
+        b200::set_error("b200_create_new_landmarks: a row kept %d gated candidates, max_candidates is %d", overflow, cap);
+        return B200_ERR_CAPACITY;
+    }
+    const int unconverged = *reinterpret_cast<const int*>(hb + o_unconv);
+    if (unconverged > 0) {
+        b200::set_error("b200_create_new_landmarks: the 4x4 Jacobi SVD did not converge within %d sweeps for %d matches",
+                        b200::tri::kMaxSweeps, unconverged);
+        return B200_ERR_INVALID;
+    }
+    for (int k = 0; k < n_kf; ++k) {
+        b200_new_landmarks_problem_t& P = problems[k];
+        const size_t n1 = (size_t)P.keyfrm->n_keypoints;
+        for (int r = 0; r < P.n_neighbours; ++r) {
+            b200_new_landmarks_neighbour_t& N = P.neighbours[r];
+            const size_t q = (size_t)r * n_kf + k;
+            N.n_matches = *reinterpret_cast<const int*>(hb + o_nm[q]);
+            N.n_created = reinterpret_cast<const int*>(hb + ol[k].n_rank)[r];
+            if (N.match_out && n1) std::memcpy(N.match_out, hb + o_mout[q], 4 * n1);
+        }
+        const int nc = *reinterpret_cast<const int*>(hb + ol[k].n_created);
+        P.n_created = nc;
+        if (nc) {
+            std::memcpy(P.created_rank, hb + ol[k].rank, 4 * (size_t)nc);
+            std::memcpy(P.created_idx, hb + ol[k].idx, 8 * (size_t)nc);
+            std::memcpy(P.created_pos_w, hb + ol[k].pos, 24 * (size_t)nc);
+        }
+    }
+    return B200_OK;
+}

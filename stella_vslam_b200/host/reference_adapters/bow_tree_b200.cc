@@ -18,6 +18,7 @@
 #include "stella_vslam/match/robust.h"
 
 #include "b200vslam.h"
+#include "pairs_gather_b200.h"
 
 namespace stella_vslam {
 namespace match {
@@ -29,30 +30,8 @@ b200_matcher_t pairs_matcher() {
     return h;
 }
 
-// node id per keypoint (-1: the keypoint is in no node and is never visited)
-std::vector<int32_t> node_of(const data::bow_feature_vector& fv, size_t n) {
-    std::vector<int32_t> node(n, -1);
-    for (const auto& kv : fv)
-        for (const auto idx : kv.second) node.at(idx) = static_cast<int32_t>(kv.first);
-    return node;
-}
-
-struct side {
-    std::vector<float> angle, scale;
-    std::vector<uint8_t> valid, stereo;
-    std::vector<double> bearing;
-    void fill(const data::frame_observation& obs, const feature::orb_params* prm) {
-        const size_t n = obs.undist_keypts_.size();
-        angle.resize(n); scale.resize(n); valid.assign(n, 0); stereo.assign(n, 0); bearing.resize(3 * n);
-        for (size_t i = 0; i < n; ++i) {
-            angle[i] = obs.undist_keypts_[i].angle;
-            scale[i] = prm->scale_factors_.at(obs.undist_keypts_[i].octave);
-            stereo[i] = !obs.stereo_x_right_.empty() && 0 <= obs.stereo_x_right_.at(i);
-            if (i < obs.bearings_.size())
-                for (int k = 0; k < 3; ++k) bearing[3 * i + k] = obs.bearings_[i](k);
-        }
-    }
-};
+using b200_gather::node_of;
+using b200_gather::side;
 
 // shared body of the two match_for_triangulation (robust.cc:14-146, bow_tree.cc:11-167)
 unsigned int triangulation(const std::shared_ptr<data::keyframe>& keyfrm_1, const std::shared_ptr<data::keyframe>& keyfrm_2, const Mat33_t& E_12,

@@ -491,3 +491,124 @@ def make_tracking_frame(kps, desc, camera, scale_factors, seed=0, stereo=False, 
     return dict(pose_cw=pose, gt_pose_cw=gt, kp_landmark=kp_landmark, kp_x_right=kp_x_right,
                 landmarks=dict(pos_w=pw, mean_normal=normal, min_valid_dist=min_valid, max_valid_dist=max_valid, desc=ldesc, skip=skip,
                                has_observation=has_obs))
+
+
+def make_mapping_problem(seed, n_neighbours=10, n_keypoints=2000, model="perspective", stereo=False, num_levels=8, scale_factor=1.2):
+    """A current keyframe and `n_neighbours` ordered covisibilities for the mapping module's landmark creation
+    (mapping_module::create_new_landmarks, two_view_triangulator).  Returns (cur, neighbours): keyframe dicts in the shape of
+    stella_vslam_b200.mapping (poses, camera, undistorted keypoints, octaves, bearings, descriptors, BoW nodes, no_landmark and, with
+    `stereo`, x_right / depth).  model: "perspective" (640 x 480, f = 500) or "equirectangular" (1920 x 960; stereo is not defined there).
+    Built in: points seen by the current keyframe and by several neighbours (so the row claims between ranks decide outcomes), far
+    points with near-parallel rays, correspondences shifted along the epipolar line (points behind a camera, depth tests), perturbed
+    x_right and pixel noise of varied strength (chi-square tests), inconsistent octaves (scale-ratio test) and keypoints that already
+    carry a landmark."""
+    rng = np.random.default_rng(seed)
+    equirect = model == "equirectangular"
+    assert not (equirect and stereo)
+    sf = np.cumprod(np.concatenate([[np.float32(1.0)], np.full(num_levels - 1, np.float32(scale_factor))])).astype(np.float32)
+    sigma_sq = (sf * sf).astype(np.float32)
+    fx = fy = 500.0
+    cx, cy, cols, rows = 320.0, 240.0, 1920.0, 960.0
+    true_baseline = 0.1
+    n_pts = int(1.2 * n_keypoints)
+    depth = rng.uniform(2.0, 25.0, n_pts)
+    far = rng.random(n_pts) < 0.05
+    depth[far] = rng.uniform(200.0, 2000.0, far.sum())                    # near-parallel rays
+    if equirect:
+        d = rng.normal(0, 1, (n_pts, 3))
+        d /= np.linalg.norm(d, axis=1, keepdims=True)
+    else:
+        d = np.stack([rng.uniform(-0.6, 0.6, n_pts), rng.uniform(-0.45, 0.45, n_pts), np.ones(n_pts)], 1)
+        d /= np.linalg.norm(d, axis=1, keepdims=True)
+    pts = d * depth[:, None]
+    pdesc = rng.integers(0, 256, (n_pts, 32), dtype=np.uint8)
+    pnode = rng.integers(0, 120, n_pts).astype(np.int32)
+    octave_pt = rng.choice(num_levels, n_pts, p=np.array([.3, .22, .16, .12, .08, .06, .04, .02])).astype(np.int32)
+
+    def pose(R, c):
+        P, W = np.eye(4), np.eye(4)
+        P[:3, :3], P[:3, 3] = R, -R @ c
+        W[:3, :3], W[:3, 3] = R.T, c
+        return P, W
+
+    def flip(desc, n_bits):
+        out = desc.copy()
+        for k in range(len(out)):
+            for b in rng.choice(256, n_bits[k], replace=False):
+                out[k, b // 8] ^= np.uint8(1 << (b % 8))
+        return out
+
+    def view(R, c, n_kp, vis_frac, shifted_frac):
+        P, W = pose(R, c)
+        pc = pts @ R.T + P[:3, 3]
+        if equirect:
+            visible = np.ones(n_pts, bool)
+        else:
+            with np.errstate(divide="ignore", invalid="ignore"):
+                u, v = fx * pc[:, 0] / pc[:, 2] + cx, fy * pc[:, 1] / pc[:, 2] + cy
+            visible = (pc[:, 2] > 0.5) & (u > 0) & (u < 640) & (v > 0) & (v < 480)
+        cand = np.flatnonzero(visible)
+        n_obs = min(len(cand), int(vis_frac * n_kp))
+        obs = np.sort(rng.choice(cand, n_obs, replace=False))
+        n_cl = n_kp - n_obs
+        pt_idx = np.concatenate([obs, np.full(n_cl, -1)])
+        perm = rng.permutation(n_kp)
+        pt_idx = pt_idx[perm]
+        # camera-frame direction per keypoint: observed points (some shifted along the ray of the current keyframe), clutter at random
+        X = np.where(pt_idx[:, None] >= 0, pts[np.maximum(pt_idx, 0)], 0.0)
+        shifted = (pt_idx >= 0) & (rng.random(n_kp) < shifted_frac)
+        s = rng.uniform(-1.5, 3.0, n_kp)
+        X = np.where(shifted[:, None], X * s[:, None], X)                # the current keyframe sits at the origin
+        Xc = X @ R.T + P[:3, 3]
+        clutter = pt_idx < 0
+        rnd = np.stack([rng.uniform(-0.6, 0.6, n_kp), rng.uniform(-0.45, 0.45, n_kp), np.ones(n_kp)], 1) * rng.uniform(2, 30, (n_kp, 1))
+        if equirect:
+            rnd = rng.normal(0, 1, (n_kp, 3)) * rng.uniform(2, 30, (n_kp, 1))
+        Xc = np.where(clutter[:, None], rnd, Xc)
+        bad = np.zeros(n_kp, bool) if equirect else (Xc[:, 2] <= 0.1)                              # shifted behind this camera: not observable, make it clutter
+        Xc[bad] = rnd[bad]
+        clutter |= bad
+        noise_px = rng.choice([0.2, 0.7, 1.5, 2.5], n_kp, p=[.4, .3, .2, .1])
+        oct_ = np.where(clutter, rng.integers(0, num_levels, n_kp), octave_pt[np.maximum(pt_idx, 0)]).astype(np.int32)
+        wrong_oct = ~clutter & (rng.random(n_kp) < 0.04)
+        oct_[wrong_oct] = np.where(oct_[wrong_oct] < 4, num_levels - 1, 0)
+        if equirect:
+            b = Xc / np.linalg.norm(Xc, axis=1, keepdims=True)
+            lat, lon = -np.arcsin(b[:, 1]), np.arctan2(b[:, 0], b[:, 2])
+            x = cols * (0.5 + lon / (2 * np.pi)) + rng.normal(0, 1, n_kp) * noise_px
+            y = rows * (0.5 - lat / np.pi) + rng.normal(0, 1, n_kp) * noise_px
+            x, y = x.astype(np.float32), y.astype(np.float32)
+            lon2, lat2 = (x.astype(np.float64) / cols - 0.5) * 2 * np.pi, -(y.astype(np.float64) / rows - 0.5) * np.pi
+            bearings = np.stack([np.cos(lat2) * np.sin(lon2), -np.sin(lat2), np.cos(lat2) * np.cos(lon2)], 1)
+        else:
+            x = (fx * Xc[:, 0] / Xc[:, 2] + cx + rng.normal(0, 1, n_kp) * noise_px).astype(np.float32)
+            y = (fy * Xc[:, 1] / Xc[:, 2] + cy + rng.normal(0, 1, n_kp) * noise_px).astype(np.float32)
+            bearings = np.stack([(x - cx) / fx, (y - cy) / fy, np.ones(n_kp)], 1)
+            bearings /= np.linalg.norm(bearings, axis=1, keepdims=True)
+        desc = np.where(clutter[:, None], rng.integers(0, 256, (n_kp, 32), dtype=np.uint8), pdesc[np.maximum(pt_idx, 0)])
+        desc = flip(desc, rng.integers(0, 14, n_kp))
+        node = np.where(clutter, rng.integers(0, 120, n_kp), pnode[np.maximum(pt_idx, 0)]).astype(np.int32)
+        kf = dict(pose_cw=P, pose_wc=W, model=1 if equirect else 0, fx=fx, fy=fy, cx=cx, cy=cy, fx_inv=1.0 / fx, fy_inv=1.0 / fy,
+                  focal_x_baseline=fx * true_baseline if stereo else 0.0, true_baseline=true_baseline if stereo else 0.0, cols=cols, rows=rows,
+                  img_bounds=(0.0, 640.0, 0.0, 480.0),
+                  scale_factor=np.float32(scale_factor), scale_factors=sf, level_sigma_sq=sigma_sq, x=x, y=y, octave=oct_,
+                  bearings=np.ascontiguousarray(bearings), desc=np.ascontiguousarray(desc), node=node,
+                  no_landmark=(rng.random(n_kp) >= 0.25).astype(np.uint8), x_right=None, depth=None, angle=np.zeros(n_kp, np.float32))
+        if stereo:
+            has = (rng.random(n_kp) < 0.5) & (Xc[:, 2] > 0.5) & (Xc[:, 2] < 60.0)
+            z = Xc[:, 2].astype(np.float32)
+            xr = (x - np.float32(fx * true_baseline) / z + rng.normal(0, 0.3, n_kp).astype(np.float32)).astype(np.float32)
+            off = has & (rng.random(n_kp) < 0.08)
+            xr[off] += rng.uniform(-6, 6, off.sum()).astype(np.float32)    # x_right off: 3-dof chi-square
+            kf["x_right"] = np.where(has & (xr >= 0), xr, np.float32(-1)).astype(np.float32)
+            kf["depth"] = np.where(kf["x_right"] >= 0, z, np.float32(-1)).astype(np.float32)
+        return kf
+
+    cur = view(np.eye(3), np.zeros(3), n_keypoints, 0.8, 0.0)
+    neighbours = []
+    for r in range(n_neighbours):
+        c = rng.normal(0, 1, 3) * np.array([0.6, 0.2, 0.6])
+        c *= rng.uniform(0.3, 1.2) / max(np.linalg.norm(c), 1e-9)
+        R = _rodrigues(rng.normal(0, 0.06, 3))
+        neighbours.append(view(R, c, n_keypoints, 0.7, 0.05))
+    return cur, neighbours
