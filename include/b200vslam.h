@@ -147,6 +147,45 @@ int b200_convert_to_grayscale(b200_orb_t h, const uint8_t* src, int width, int h
 int b200_convert_to_grayscale_device(b200_orb_t h, const void* d_src, int width, int height, size_t src_pitch, size_t src_frame_stride,
                                      int channels, int rgb_order, void* d_gray, size_t gray_pitch, size_t gray_frame_stride, int batch);
 
+/* util::stereo_rectifier (src/stella_vslam/util/stereo_rectifier.cc:12-66): the undistort-and-rectify step in front of the grayscale
+ * conversion and the extractor for a stereo rig whose frames are not rectified yet (system::feed_stereo_frame requires rectified input).
+ * b200_rectifier_create builds both eyes' maps once, on the host in double with the host libm, as
+ *   model 0: cv::initUndistortRectifyMap(K, D, R, K_rect, size, CV_32F)           (D: 4, 5 or 8 coefficients k1 k2 p1 p2 [k3 [k4 k5 k6]])
+ *   model 1: cv::fisheye::initUndistortRectifyMap(K, D, R, K_rect, size, CV_32F)  (D: 4 coefficients k1..k4; rays behind the camera map
+ *            to an infinity of the sign opposite to the ray's x / y, as OpenCV 4.13 writes them)
+ * and converts them once to the fixed-point form cv::remap derives from float maps (source corner + 5-bit fractions).  Every
+ * rectify is then cv::remap(..., INTER_LINEAR) with BORDER_CONSTANT 0 in integer arithmetic only, bit-exact by construction.
+ * Deviations: the 12- and 14-coefficient models (thin prism, tilt) and model values other than 0 / 1 are B200_ERR_INVALID (the reference
+ * throws for equirectangular, stereo_rectifier.cc:52-54); cols and rows are limited to 32766 (the fixed-point corner is a short). */
+typedef struct {
+    int32_t model;         /* 0 perspective, 1 fisheye (StereoRectifier.model) */
+    int32_t cols, rows;    /* Camera.cols / rows: source, map and output size */
+    double K_rect[9];      /* camera::perspective::cv_cam_matrix_ of the rectified camera, row-major (CV_32F there: its float values) */
+    double K[2][9];        /* StereoRectifier.K_left / K_right, row-major */
+    double R[2][9];        /* StereoRectifier.R_left / R_right, row-major */
+    double D[2][8];        /* StereoRectifier.D_left / D_right; the first n_dist[eye] entries are read */
+    int32_t n_dist[2];
+    int32_t device;        /* CUDA device ordinal */
+} b200_rectifier_params_t;
+typedef struct b200_rectifier_s* b200_rectifier_t;
+int b200_rectifier_create(const b200_rectifier_params_t* p, b200_rectifier_t* out);
+int b200_rectifier_destroy(b200_rectifier_t h);
+/* Same contract as b200_orb_set_stream: run on the caller's stream (NULL = legacy default), use_own != 0 restores the own stream. */
+int b200_rectifier_set_stream(b200_rectifier_t h, void* stream, int use_own);
+/* The CV_32F maps as built (the reference's undist_map_{x,y}_{l,r}_): eye 0 left, 1 right; rows x cols floats each, tightly packed. */
+int b200_rectifier_maps(b200_rectifier_t h, int eye, float* map_x, float* map_y);
+/* stereo_rectifier::rectify for one pair of 8-bit frames with `channels` (1, 3 or 4) interleaved channels in HOST memory, rows `*_pitch`
+ * bytes apart (pitch >= cols * channels).  Includes the uploads and downloads; returns when the outputs are written. */
+int b200_stereo_rectify(b200_rectifier_t h, int channels, const uint8_t* left, size_t left_pitch, const uint8_t* right, size_t right_pitch,
+                        uint8_t* out_left, size_t out_left_pitch, uint8_t* out_right, size_t out_right_pitch);
+/* Same for `batch` pairs in DEVICE memory, enqueued on the rectifier's stream without synchronising: pair f reads d_left / d_right +
+ * f * src_frame_stride and writes d_out_left / d_out_right + f * out_frame_stride.  Interleaving the eyes (d_out_right = d_out_left +
+ * one frame, out_frame_stride = two frames) lets ONE b200_orb_extract_device over 2 * batch frames follow on the same stream and feed
+ * b200_stereo_compute(h, 2p, h, 2p + 1).  Outputs must not overlap inputs.  Word-wide stores when the output pointers, pitch and frame
+ * stride are multiples of 4 bytes, byte stores otherwise.  batch == 0 -> B200_OK with nothing written. */
+int b200_stereo_rectify_device(b200_rectifier_t h, int channels, const void* d_left, const void* d_right, size_t src_pitch, size_t src_frame_stride,
+                               void* d_out_left, void* d_out_right, size_t out_pitch, size_t out_frame_stride, int batch);
+
 /* Keyframe serialisation (SURVEY 8f N4): the byte layouts in which data::keyframe stores what the extractor produced.
  *   SQLite (data/keyframe.cc:298-347 to_db, :191-235 from_stmt): `undist_keypts` = the std::vector<cv::KeyPoint> as raw bytes (28 bytes per
  *       keypoint: pt.x, pt.y, size, angle, response, octave, class_id), `descs` = cv::Mat rows, 32 bytes each;

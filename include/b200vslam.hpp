@@ -9,6 +9,7 @@
 //   b200::match::projection / fuse / area / bow_tree / stereo  <->  match/projection.h, fuse.h, area.h, bow_tree.h, stereo.h
 //   b200::optimize::local_bundle_adjuster <-> stella_vslam::optimize::local_bundle_adjuster (optimize/local_bundle_adjuster.h:15-24)
 //   b200::optimize::pose_optimizer        <-> stella_vslam::optimize::pose_optimizer        (optimize/pose_optimizer.h:24-40)
+//   b200::util::stereo_rectifier          <-> stella_vslam::util::stereo_rectifier          (util/stereo_rectifier.h:14-46)
 #pragma once
 
 #include <cmath>
@@ -478,4 +479,41 @@ private:
     float lowe_, residual_, deg_;
 };
 }  // namespace mapping
+
+namespace util {
+// util::stereo_rectifier (util/stereo_rectifier.h): both eyes' maps are built at construction (b200_rectifier_create); rectify() is
+// cv::remap(INTER_LINEAR) of one pair of 8-bit frames in host memory, rectify_device() of a batch already on the device.
+class stereo_rectifier {
+public:
+    explicit stereo_rectifier(const b200_rectifier_params_t& params) : cols_(params.cols), rows_(params.rows) {
+        check(b200_rectifier_create(&params, &h_), "b200_rectifier_create");
+    }
+    ~stereo_rectifier() { b200_rectifier_destroy(h_); }
+    stereo_rectifier(const stereo_rectifier&) = delete;
+    stereo_rectifier& operator=(const stereo_rectifier&) = delete;
+
+    // rectify(in_img_l, in_img_r, out_img_l, out_img_r) -- stereo_rectifier.h:25-26; all four frames cols x rows x channels
+    void rectify(int channels, const uint8_t* in_l, size_t in_l_pitch, const uint8_t* in_r, size_t in_r_pitch, uint8_t* out_l, size_t out_l_pitch,
+                 uint8_t* out_r, size_t out_r_pitch) const {
+        check(b200_stereo_rectify(h_, channels, in_l, in_l_pitch, in_r, in_r_pitch, out_l, out_l_pitch, out_r, out_r_pitch), "b200_stereo_rectify");
+    }
+    void rectify_device(int channels, const void* d_l, const void* d_r, size_t src_pitch, size_t src_frame_stride, void* d_out_l, void* d_out_r,
+                        size_t out_pitch, size_t out_frame_stride, int batch) const {
+        check(b200_stereo_rectify_device(h_, channels, d_l, d_r, src_pitch, src_frame_stride, d_out_l, d_out_r, out_pitch, out_frame_stride, batch),
+              "b200_stereo_rectify_device");
+    }
+    void set_stream(void* stream, bool use_own = false) { check(b200_rectifier_set_stream(h_, stream, use_own ? 1 : 0), "b200_rectifier_set_stream"); }
+    // undist_map_{x,y}_{l,r}_ (stereo_rectifier.h:38-45): eye 0 left, 1 right; rows x cols floats each
+    void maps(int eye, std::vector<float>& map_x, std::vector<float>& map_y) const {
+        map_x.resize((size_t)cols_ * rows_);
+        map_y.resize((size_t)cols_ * rows_);
+        check(b200_rectifier_maps(h_, eye, map_x.data(), map_y.data()), "b200_rectifier_maps");
+    }
+    b200_rectifier_t handle() const { return h_; }
+
+private:
+    b200_rectifier_t h_ = nullptr;
+    int cols_, rows_;
+};
+}  // namespace util
 }  // namespace b200

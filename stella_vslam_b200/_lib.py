@@ -38,6 +38,12 @@ class CameraIntrinsics(C.Structure):
                 ("cols", C.c_double), ("rows", C.c_double)]
 
 
+class RectifierParams(C.Structure):
+    """b200_rectifier_params_t (include/b200vslam.h)."""
+    _fields_ = [("model", C.c_int32), ("cols", C.c_int32), ("rows", C.c_int32), ("K_rect", C.c_double * 9), ("K", (C.c_double * 9) * 2),
+                ("R", (C.c_double * 9) * 2), ("D", (C.c_double * 8) * 2), ("n_dist", C.c_int32 * 2), ("device", C.c_int32)]
+
+
 class GuidedProblem(C.Structure):
     """b200_guided_problem_t (include/b200vslam.h)."""
     _fields_ = [("n_train", C.c_int32), ("t_x", C.c_void_p), ("t_y", C.c_void_p), ("t_octave", C.c_void_p), ("t_angle", C.c_void_p),
@@ -139,6 +145,8 @@ SYMBOLS = [
     "b200_lba_create", "b200_lba_destroy", "b200_lba_solve", "b200_lba_solve_batch", "b200_pose_optimize", "b200_lba_last_profile", "b200_lba_enable_profile", "b200_lba_kernel_ms",
     "b200_global_ba_solve", "b200_track_local_map", "b200_track_stage_ms", "b200_orb_export_keyframe_blobs", "b200_keyframe_blob_to_keypoints",
     "b200_triangulate_pairs", "b200_create_new_landmarks",
+    "b200_rectifier_create", "b200_rectifier_destroy", "b200_rectifier_set_stream", "b200_rectifier_maps", "b200_stereo_rectify",
+    "b200_stereo_rectify_device",
 ]
 
 
@@ -194,6 +202,12 @@ def lib():
     L.b200_convert_to_grayscale.argtypes = [vp, vp, i32, i32, sz, i32, i32, vp, sz]
     L.b200_convert_to_grayscale_device.argtypes = [vp, vp, i32, i32, sz, sz, i32, i32, vp, sz, sz, i32]
     L.b200_matcher_set_stream.argtypes = [vp, vp, i32]
+    L.b200_rectifier_create.argtypes = [C.POINTER(RectifierParams), C.POINTER(vp)]
+    L.b200_rectifier_destroy.argtypes = [vp]
+    L.b200_rectifier_set_stream.argtypes = [vp, vp, i32]
+    L.b200_rectifier_maps.argtypes = [vp, i32, vp, vp]
+    L.b200_stereo_rectify.argtypes = [vp, i32, vp, sz, vp, sz, vp, sz, vp, sz]
+    L.b200_stereo_rectify_device.argtypes = [vp, i32, vp, vp, sz, sz, vp, vp, sz, sz, i32]
     _lib = L
     return L
 

@@ -19,6 +19,8 @@ SOURCES = {
     "orb_kernels.cu": ["-fmad=false"],
     "match_kernels.cu": [],
     "lba_kernels.cu": [],
+    # the rectification maps are built on the host in double; keep the host compiler from contracting them to FMA
+    "rectify_kernels.cu": ["-Xcompiler", "-ffp-contract=off"],
 }
 
 

@@ -199,6 +199,129 @@ class orb_extractor:
         return out
 
 
+class stereo_rectifier:
+    """util::stereo_rectifier (util/stereo_rectifier.cc:12-66) on the GPU: both eyes' undistort-and-rectify maps are built once when
+    the object is made, and `rectify` is cv::remap(INTER_LINEAR) of a pair, bit-exact to OpenCV.  Frames are 8-bit with 1, 3 or 4
+    channels: (h, w) or (h, w, c) numpy arrays for `rectify`, torch CUDA tensors for `rectify_device`."""
+
+    MODELS = {"perspective": 0, "fisheye": 1}
+
+    def __init__(self, model, cols, rows, K_rect, K_left, D_left, R_left, K_right, D_right, R_right, device=0):
+        if model not in self.MODELS:  # stereo_rectifier.cc:52-54 (equirectangular)
+            raise RuntimeError("Invalid model type for stereo rectification: " + str(model))
+        p = _lib.RectifierParams()
+        p.model, p.cols, p.rows, p.device = self.MODELS[model], int(cols), int(rows), int(device)
+        p.K_rect[:] = [float(v) for v in np.asarray(K_rect, np.float64).reshape(9)]
+        for eye, (K, D, R) in enumerate(((K_left, D_left, R_left), (K_right, D_right, R_right))):
+            D = np.asarray(D, np.float64).reshape(-1)
+            if len(D) > 8:
+                raise RuntimeError(f"{len(D)} distortion coefficients: the thin-prism and tilt models are not supported")
+            p.K[eye][:] = [float(v) for v in np.asarray(K, np.float64).reshape(9)]
+            p.R[eye][:] = [float(v) for v in np.asarray(R, np.float64).reshape(9)]
+            p.D[eye][:len(D)] = [float(v) for v in D]
+            p.n_dist[eye] = len(D)
+        self.model_type_, self.cols_, self.rows_ = model, int(cols), int(rows)
+        self._h = C.c_void_p()
+        check(lib().b200_rectifier_create(C.byref(p), C.byref(self._h)))
+
+    @staticmethod
+    def load_model_type(rectifier_node):
+        """stereo_rectifier::load_model_type (stereo_rectifier.cc:75-89): `model` defaults to "perspective"."""
+        m = rectifier_node.get("model", "perspective")
+        if m not in ("perspective", "fisheye", "equirectangular"):
+            raise RuntimeError("Invalid camera model: " + str(m))
+        return m
+
+    @staticmethod
+    def parse_vector_as_mat(shape, vec):
+        """stereo_rectifier::parse_vector_as_mat: the first rows x cols entries of a YAML list as a float64 matrix (row-major)."""
+        cols, rows = shape
+        v = np.asarray(vec, np.float64).reshape(-1)
+        if v.size < rows * cols:
+            raise RuntimeError(f"expected {rows * cols} values, got {v.size}")
+        return v[:rows * cols].reshape(rows, cols).copy()
+
+    @classmethod
+    def from_yaml(cls, camera_node, rectifier_node, device=0):
+        """stereo_rectifier(camera, yaml_node) (stereo_rectifier.cc:16-56).  camera_node: the `Camera:` block as a dict (the camera
+        the rectified frames feed), rectifier_node: the `StereoRectifier:` block."""
+        return cls(**cls.parse_yaml(camera_node, rectifier_node), device=device)
+
+    @classmethod
+    def parse_yaml(cls, camera_node, rectifier_node):
+        """The constructor's checks and parsing, in the reference's order, as keyword arguments of stereo_rectifier(...).  K_rect is
+        the rectified camera's cv_cam_matrix_, which the reference stores as CV_32F: fx, fy, cx, cy are rounded to float."""
+        model = cls.load_model_type(rectifier_node)
+        if camera_node.get("setup") != "stereo":
+            raise RuntimeError("When stereo rectification is used, 'setup' must be set to 'stereo'")
+        if camera_node.get("model") != "perspective":
+            raise RuntimeError("When stereo rectification is used, 'model' must be set to 'perspective'")
+        f32 = [float(np.float32(camera_node[k])) for k in ("fx", "fy", "cx", "cy")]
+        K_rect = np.array([[f32[0], 0.0, f32[2]], [0.0, f32[1], f32[3]], [0.0, 0.0, 1.0]])
+        mat = cls.parse_vector_as_mat
+        args = dict(K_left=mat((3, 3), rectifier_node["K_left"]), K_right=mat((3, 3), rectifier_node["K_right"]),
+                    R_left=mat((3, 3), rectifier_node["R_left"]), R_right=mat((3, 3), rectifier_node["R_right"]),
+                    D_left=np.asarray(rectifier_node["D_left"], np.float64).reshape(-1), D_right=np.asarray(rectifier_node["D_right"], np.float64).reshape(-1))
+        if model == "equirectangular":  # the camera's model string, as camera::base::get_model_type_string gives it
+            raise RuntimeError("Invalid model type for stereo rectification: " + camera_node["model"])
+        return dict(model=model, cols=int(camera_node["cols"]), rows=int(camera_node["rows"]), K_rect=K_rect, **args)
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h:
+            lib().b200_rectifier_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def maps(self, eye):
+        """(map_x, map_y) float32 (rows, cols) of eye 0 (left) or 1 (right): the reference's undist_map_{x,y}_{l,r}_."""
+        mx, my = np.empty((self.rows_, self.cols_), np.float32), np.empty((self.rows_, self.cols_), np.float32)
+        check(lib().b200_rectifier_maps(self._h, int(eye), ptr(mx), ptr(my)))
+        return mx, my
+
+    def _channels(self, img):
+        if img.dtype != np.uint8 or img.shape[:2] != (self.rows_, self.cols_) or img.ndim not in (2, 3) or (img.ndim == 3 and img.shape[2] not in (1, 3, 4)):
+            raise ValueError(f"expected uint8 ({self.rows_}, {self.cols_}[, 1|3|4]) frames, got {img.dtype} {img.shape}")
+        return 1 if img.ndim == 2 else img.shape[2]
+
+    def rectify(self, in_img_l, in_img_r):
+        """stereo_rectifier::rectify: (out_img_l, out_img_r) with the inputs' shape and type."""
+        l, r = np.ascontiguousarray(in_img_l), np.ascontiguousarray(in_img_r)
+        c = self._channels(l)
+        if self._channels(r) != c:
+            raise ValueError("both eyes must have the same number of channels")
+        ol, orr = np.empty_like(l), np.empty_like(r)
+        check(lib().b200_stereo_rectify(self._h, c, ptr(l), l.strides[0], ptr(r), r.strides[0], ptr(ol), ol.strides[0], ptr(orr), orr.strides[0]))
+        return ol, orr
+
+    def set_stream(self, stream=None):
+        """Run rectify_device on a torch / CUDA stream (an object with .cuda_stream, or a raw handle); None restores the own stream."""
+        if stream is None:
+            check(lib().b200_rectifier_set_stream(self._h, None, 1))
+        else:
+            check(lib().b200_rectifier_set_stream(self._h, C.c_void_p(getattr(stream, "cuda_stream", stream)), 0))
+
+    def rectify_device(self, left, right, out_left, out_right):
+        """b200_stereo_rectify_device on torch uint8 CUDA tensors of shape (B, rows, cols[, c]).  Each tensor's strides give the row
+        pitch and the frame stride (dims 0 and 1), so views such as out[0::2] / out[1::2] of one (2B, rows, cols) tensor interleave
+        the eyes.  Enqueued on the rectifier's stream (see set_stream) without synchronising."""
+        if left.dim() not in (3, 4) or tuple(left.shape[1:3]) != (self.rows_, self.cols_) or left.shape != right.shape \
+                or out_left.shape != left.shape or out_right.shape != left.shape:
+            raise ValueError("left, right and outputs must be (B, rows, cols[, c]) tensors of the rectifier's size")
+        c = 1 if left.dim() == 3 else int(left.shape[3])
+        for a, b in ((left, right), (out_left, out_right)):
+            for t in (a, b):
+                if t.stride()[:2] != a.stride()[:2] or t.stride(2) != c or (t.dim() == 4 and t.stride(3) != 1):
+                    raise ValueError("rows must be dense (channels interleaved) and both eyes must share pitch and frame stride")
+        b = int(left.shape[0])
+        check(lib().b200_stereo_rectify_device(self._h, c, ptr(left), ptr(right), left.stride(1), left.stride(0), ptr(out_left), ptr(out_right),
+                                               out_left.stride(1), out_left.stride(0), b))
+
+
 def check_pos(v):
     if v < 0:
         check(v)

@@ -414,6 +414,80 @@ def make_stereo_pair(w=752, h=480, seed=77, disparities=(9, 23, 41), noise_sigma
     return left, right
 
 
+# Stereo rectification calibrations (StereoRectifier blocks of example/euroc/EuRoC_stereo.yaml and example/tum_vi/TUM_VI_stereo.yaml):
+# K, D, R per eye (left, right), row-major; K_rect is the rectified Camera block's matrix, fxb its focal_x_baseline.
+EUROC_STEREO = dict(
+    model="perspective", cols=752, rows=480, fxb=47.90639384423901,
+    K_rect=(435.2046959714599, 0.0, 367.4517211914062, 0.0, 435.2046959714599, 252.2008514404297, 0.0, 0.0, 1.0),
+    K=((458.654, 0.0, 367.215, 0.0, 457.296, 248.375, 0.0, 0.0, 1.0), (457.587, 0.0, 379.999, 0.0, 456.134, 255.238, 0.0, 0.0, 1.0)),
+    D=((-0.28340811, 0.07395907, 0.00019359, 1.76187114e-05, 0.0), (-0.28368365, 0.07451284, -0.00010473, -3.555907e-05, 0.0)),
+    R=((0.999966347530033, -0.001422739138722922, 0.008079580483432283, 0.001365741834644127, 0.9999741760894847, 0.007055629199258132,
+        -0.008089410156878961, -0.007044357138835809, 0.9999424675829176),
+       (0.9999633526194376, -0.003625811871560086, 0.007755443660172947, 0.003680398547259526, 0.9999684752771629, -0.007035845251224894,
+        -0.007729688520722713, 0.007064130529506649, 0.999945173484644)))
+TUM_VI_STEREO = dict(
+    model="fisheye", cols=512, rows=512, fxb=6.242596912726197,
+    K_rect=(61.75453410721205, 0.0, 240.22941720459062, 0.0, 61.75453410721205, 255.73235402091632, 0.0, 0.0, 1.0),
+    K=((190.97847715128717, 0.0, 254.93170605935475, 0.0, 190.9733070521226, 256.8974428996504, 0.0, 0.0, 1.0),
+       (190.44236969414825, 0.0, 252.59949716835982, 0.0, 190.4344384721956, 254.91723064636983, 0.0, 0.0, 1.0)),
+    D=((0.0034823894022493434, 0.0007150348452162257, -0.0020532361418706202, 0.00020293673591811182),
+       (0.0034003170790442797, 0.001766278153469831, -0.00266312569781606, 0.0003299517423931039)),
+    R=((0.9997641946925044, 0.01925271884177015, 0.010044293307535757, -0.01901185247371587, 0.9995418997803748, -0.02354867403818772,
+        -0.010493068014919314, 0.02335216051329943, 0.99967223234568),
+       (0.9997411981023351, 0.01955199401713946, 0.011629976219300583, -0.019819377433695273, 0.9995311538731381, 0.02333805294307984,
+        -0.011168218078479885, -0.023562511898925578, 0.9996599816627474)))
+
+
+def _rect_forward(calib, eye, j, i):
+    """The rectification map of one eye at fractional rectified pixels (j, i): where the raw view sees that rectified pixel."""
+    K, D = np.asarray(calib["K"][eye], np.float64).reshape(3, 3), np.asarray(calib["D"][eye], np.float64)
+    iR = np.linalg.inv(np.asarray(calib["K_rect"], np.float64).reshape(3, 3) @ np.asarray(calib["R"][eye], np.float64).reshape(3, 3))
+    _x, _y, _w = (iR[r, 0] * j + iR[r, 1] * i + iR[r, 2] for r in range(3))
+    x, y = _x / _w, _y / _w
+    if calib["model"] == "fisheye":
+        r = np.sqrt(x * x + y * y)
+        th = np.arctan(r)
+        th2 = th * th
+        s = np.where(r > 0, th * (1 + D[0] * th2 + D[1] * th2 ** 2 + D[2] * th2 ** 3 + D[3] * th2 ** 4) / np.maximum(r, 1e-300), 1.0)
+        xd, yd = x * s, y * s
+    else:
+        k = np.concatenate([D, np.zeros(8)])[:8]
+        r2 = x * x + y * y
+        kr = (1 + ((k[4] * r2 + k[1]) * r2 + k[0]) * r2) / (1 + ((k[7] * r2 + k[6]) * r2 + k[5]) * r2)
+        xd = x * kr + 2 * k[2] * x * y + k[3] * (r2 + 2 * x * x)
+        yd = y * kr + k[2] * (r2 + 2 * y * y) + 2 * k[3] * x * y
+    return K[0, 0] * xd + K[0, 2], K[1, 1] * yd + K[1, 2]
+
+
+def make_raw_stereo_pair(calib, seed=77, disparities=(9, 23, 41), noise_sigma=2.0):
+    """(left, right) RAW views of a rig with calibration `calib` (EUROC_STEREO / TUM_VI_STEREO layout): make_stereo_pair's rectified
+    frames seen through the distortion and rotation of each eye, so that rectifying them gives back approximately the rectified pair.
+    Each raw pixel samples the rectified frame (bilinearly) at an approximate inverse of the rectification map, found by a few
+    fixed-point iterations; the inverse only has to be good enough for the stereo matcher to find the bands' disparities."""
+    w, h = calib["cols"], calib["rows"]
+    rect = make_stereo_pair(w, h, seed=seed, disparities=disparities, noise_sigma=noise_sigma)
+    v, u = np.mgrid[0:h, 0:w].astype(np.float64)
+    out = []
+    for eye in range(2):
+        j, i = u.copy(), v.copy()
+        for _ in range(8):
+            fu, fv = _rect_forward(calib, eye, j, i)
+            ok = np.isfinite(fu) & np.isfinite(fv)
+            j = np.where(ok, j + (u - fu), j)
+            i = np.where(ok, i + (v - fv), i)
+            j, i = np.clip(j, -w, 2 * w), np.clip(i, -h, 2 * h)
+        img = rect[eye].astype(np.float64)
+        j0, i0 = np.floor(j).astype(np.int64), np.floor(i).astype(np.int64)
+        a, b = j - j0, i - i0
+
+        def px(y, x):
+            return img[np.clip(y, 0, h - 1), np.clip(x, 0, w - 1)]
+
+        s = (1 - b) * ((1 - a) * px(i0, j0) + a * px(i0, j0 + 1)) + b * ((1 - a) * px(i0 + 1, j0) + a * px(i0 + 1, j0 + 1))
+        out.append(np.clip(np.rint(s), 0, 255).astype(np.uint8))
+    return tuple(out)
+
+
 def make_tracking_frame(kps, desc, camera, scale_factors, seed=0, stereo=False, landmark_frac=0.7, clutter_frac=0.3, pre_matched_frac=0.15,
                         pixel_sigma=1.0, rot_deg=0.5, trans_m=0.05, max_flips=30):
     """A local map for one extracted frame (track_local_map workload): most keypoints get a landmark at a random depth (descriptor = the
