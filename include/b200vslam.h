@@ -633,6 +633,71 @@ typedef struct b200_new_landmarks_problem {
 int b200_create_new_landmarks(b200_matcher_t h, int n_keyframes, b200_new_landmarks_problem_t* problems, float lowe_ratio, float residual_rad_thr,
                               float rays_parallax_deg_thr, int max_candidates);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Relocalisation's PnP: solve::pnp_solver (src/stella_vslam/solve/pnp_solver.{h,cc}) -- EPnP (Lepetit et al., IJCV 2009) inside
+ * RANSAC -- for many problems (lost frame x candidate keyframe) in one launch sequence on the b200_lba_t handle's stream, so the pose
+ * goes straight on to b200_pose_optimize.  fp64 in the CPU restatement's evaluation order (sums left to right; Eigen's JacobiSVD,
+ * ColPivHouseholderQR-preconditioned JacobiSVD::solve and HouseholderQR::solve restated).  Deviations (DESIGN.md section 8): Eigen's
+ * vectorised summation order is not reproduced; a hypothesis whose compute_pose writes no pose is rejected (the reference scores the
+ * previous hypothesis' pose again, which can never win, and reads uninitialised memory for hypothesis 0); Jacobi sweeps are bounded.
+ * ---------------------------------------------------------------------------------------------------------------- */
+typedef struct b200_pnp_problem {
+    int32_t n_matches;
+    const double* bearings;         /* n x 3: frm_obs_.bearings_ of the valid matches */
+    const double* points;           /* n x 3: landmark::get_pos_in_world() */
+    const int32_t* octaves;         /* n: undist_keypts_[i].octave */
+    int32_t num_levels;             /* entries of scale_factors */
+    const float* scale_factors;     /* orb_params_->scale_factors_ */
+    uint32_t min_num_inliers;       /* relocalizer: 10 */
+    uint32_t gauss_newton_num_iter; /* constructor default 10 */
+    uint32_t max_num_iter;          /* relocalizer: max_num_ransac_iter_ = 30 */
+    int32_t recompute;              /* find_via_ransac's recompute */
+    const int32_t* min_sets;        /* max_num_iter x 4: the draws of util::create_random_array, in draw order (b200_pnp_draw_min_sets) */
+    /* out */
+    int32_t status;                 /* B200_OK, or B200_ERR_INVALID when a Jacobi SVD hit its sweep bound (the results are then unreliable) */
+    int32_t valid;                  /* solution_is_valid() */
+    int32_t best_iter;              /* hypothesis that won (-1 none) */
+    int32_t num_inliers;            /* of the winning hypothesis */
+    double min_cost;                /* of the winning hypothesis (DBL_MAX when none) */
+    double rot_cw[9];               /* row-major; written only when valid (get_best_rotation) */
+    double trans_cw[3];             /* written only when valid */
+    uint8_t* inlier_flags;          /* n: get_inlier_flags(); all 0 when not valid; untouched on the early return (n < 4 or n < min_num_inliers) */
+} b200_pnp_problem_t;
+/* find_via_ransac(max_num_iter, recompute) for every problem: one upload, the hypothesis and selection launches, one download.
+ * B200_ERR_INVALID (nothing written) for a negative count, a null required pointer, an octave outside [0, num_levels) or a min_sets index
+ * outside [0, n) of a problem that runs RANSAC. */
+int b200_pnp_ransac(b200_lba_t h, int n_problems, b200_pnp_problem_t* problems);
+
+typedef struct b200_epnp_problem {
+    int32_t n;                      /* >= 1 */
+    const double* bearings;         /* n x 3 */
+    const double* points;           /* n x 3 */
+    uint32_t num_iter;              /* Gauss-Newton iterations (the reference's default argument: 5) */
+    /* in / out: kept as given unless a candidate N reaches reproj_error < DBL_MAX, as the reference writes rot_cw / trans_cw */
+    double rot_cw[9];
+    double trans_cw[3];
+    /* out */
+    double reproj_error;            /* return value of compute_pose */
+    int32_t wrote;                  /* rot_cw / trans_cw were written */
+    int32_t status;                 /* B200_OK, or B200_ERR_INVALID when a Jacobi SVD hit its sweep bound */
+} b200_epnp_problem_t;
+/* pnp_solver::compute_pose (static; also marker_detector::base's per-marker pose) for every problem in one launch. */
+int b200_epnp_compute_pose(b200_lba_t h, int n_problems, b200_epnp_problem_t* problems);
+
+/* std::mt19937 as libstdc++ implements it, and util::create_random_array(4, 0, n - 1, engine) as find_via_ransac draws its minimal
+ * sets (std::uniform_int_distribution<unsigned>, sort, unique, std::shuffle).  Host only.  The draws reproduce a reference built
+ * against libstdc++ (GCC 11 or later: Lemire's nearly divisionless uniform_int_distribution). */
+typedef struct b200_mt19937 {
+    uint32_t state[624];
+    uint32_t index;
+} b200_mt19937_t;
+/* n_seed == 0: a default-constructed engine (seed 5489, util::create_random_engine(true)); otherwise std::seed_seq over the words. */
+int b200_mt19937_seed(b200_mt19937_t* engine, const uint32_t* seed_seq, int n_seed);
+/* The next 32-bit output of the engine (the raw stream). */
+uint32_t b200_mt19937_next(b200_mt19937_t* engine);
+/* max_num_iter minimal sets (out: max_num_iter x 4) from one engine, continuing its state; n_matches >= 4. */
+int b200_pnp_draw_min_sets(b200_mt19937_t* engine, uint32_t n_matches, uint32_t max_num_iter, int32_t* out);
+
 /* Profiling mode: an event after every launch of the following solves (adds a few microseconds per launch; off by default).
  * b200_lba_kernel_ms reports, for the LAST batch, the summed device time and the number of intervals of
  *   kernel 0 plan (5 launches, one interval), 1 landmark pass / build, 2 keyframe rows, 3 Schur rows, 4 reduced-system Cholesky,

@@ -10,10 +10,12 @@
 //   b200::optimize::local_bundle_adjuster <-> stella_vslam::optimize::local_bundle_adjuster (optimize/local_bundle_adjuster.h:15-24)
 //   b200::optimize::pose_optimizer        <-> stella_vslam::optimize::pose_optimizer        (optimize/pose_optimizer.h:24-40)
 //   b200::util::stereo_rectifier          <-> stella_vslam::util::stereo_rectifier          (util/stereo_rectifier.h:14-46)
+//   b200::solve::pnp_solver               <-> stella_vslam::solve::pnp_solver               (solve/pnp_solver.h:13-142)
 #pragma once
 
 #include <cmath>
 #include <cstdint>
+#include <random>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -516,4 +518,125 @@ private:
     int cols_, rows_;
 };
 }  // namespace util
+}  // namespace b200
+
+namespace b200 {
+namespace solve {
+
+// util::create_random_array(4, 0, n - 1, engine), max_num_iter times from one engine (b200_pnp_draw_min_sets), max_num_iter x 4
+inline std::vector<int32_t> draw_min_sets(b200_mt19937_t& engine, uint32_t n_matches, uint32_t max_num_iter) {
+    std::vector<int32_t> out(4 * (size_t)max_num_iter);
+    check(b200_pnp_draw_min_sets(&engine, n_matches, max_num_iter, out.data()), "b200_pnp_draw_min_sets");
+    return out;
+}
+
+// find_via_ransac for many problems in one call (b200_pnp_ransac); the problems' out fields are filled
+inline void pnp_ransac_batch(b200_lba_t h, std::vector<b200_pnp_problem_t>& problems) {
+    check(b200_pnp_ransac(h, (int)problems.size(), problems.data()), "b200_pnp_ransac");
+}
+
+// solve::pnp_solver (solve/pnp_solver.h:13-142).  bearings / points: n x 3 row-major; rotations row-major 3 x 3.  The engine is the
+// solver's member: find_via_ransac continues its state across calls.  The solver owns a b200_lba_t handle unless one is given.
+class pnp_solver {
+public:
+    pnp_solver(const std::vector<double>& valid_bearings, const std::vector<int>& octaves, const std::vector<double>& valid_points,
+               const std::vector<float>& scale_factors, unsigned int min_num_inliers = 10, bool use_fixed_seed = false,
+               unsigned int gauss_newton_num_iter = 10, b200_lba_t handle = nullptr)
+        : num_matches_((unsigned int)octaves.size()), bearings_(valid_bearings), points_(valid_points), octaves_(octaves.begin(), octaves.end()),
+          scale_factors_(scale_factors), min_num_inliers_(min_num_inliers), gauss_newton_num_iter_(gauss_newton_num_iter), h_(handle) {
+        if (bearings_.size() != 3 * (size_t)num_matches_ || points_.size() != 3 * (size_t)num_matches_)
+            throw std::invalid_argument("pnp_solver: bearings, octaves and points must have one entry per match");
+        for (int32_t o : octaves_)
+            if (o < 0 || (size_t)o >= scale_factors_.size()) throw std::out_of_range("pnp_solver: octave outside the scale factors");
+        if (use_fixed_seed) {  // util::create_random_engine
+            check(b200_mt19937_seed(&engine_, nullptr, 0), "b200_mt19937_seed");
+        } else {
+            std::random_device rd;
+            uint32_t words[10];
+            for (auto& w : words) w = rd();
+            check(b200_mt19937_seed(&engine_, words, 10), "b200_mt19937_seed");
+        }
+        if (!h_) {
+            check(b200_lba_create(0, &h_), "b200_lba_create");
+            own_ = true;
+        }
+    }
+    ~pnp_solver() {
+        if (own_) b200_lba_destroy(h_);
+    }
+    pnp_solver(const pnp_solver&) = delete;
+    pnp_solver& operator=(const pnp_solver&) = delete;
+
+    void find_via_ransac(unsigned int max_num_iter, bool recompute = true) {
+        if (num_matches_ < 4 || num_matches_ < min_num_inliers_) {  // before any draw (pnp_solver.cc:48-52)
+            solution_is_valid_ = false;
+            return;
+        }
+        const std::vector<int32_t> sets = draw_min_sets(engine_, num_matches_, max_num_iter);
+        std::vector<uint8_t> flags(num_matches_);
+        b200_pnp_problem_t P{};
+        P.n_matches = (int32_t)num_matches_;
+        P.bearings = bearings_.data();
+        P.points = points_.data();
+        P.octaves = octaves_.data();
+        P.num_levels = (int32_t)scale_factors_.size();
+        P.scale_factors = scale_factors_.data();
+        P.min_num_inliers = min_num_inliers_;
+        P.gauss_newton_num_iter = gauss_newton_num_iter_;
+        P.max_num_iter = max_num_iter;
+        P.recompute = recompute ? 1 : 0;
+        P.min_sets = sets.data();
+        P.inlier_flags = flags.data();
+        check(b200_pnp_ransac(h_, 1, &P), "b200_pnp_ransac");
+        status_ = P.status;
+        solution_is_valid_ = P.valid != 0;
+        if (solution_is_valid_) {
+            for (int k = 0; k < 9; ++k) best_rot_cw_[k] = P.rot_cw[k];
+            for (int k = 0; k < 3; ++k) best_trans_cw_[k] = P.trans_cw[k];
+        }
+        is_inlier_match_.assign(flags.begin(), flags.end());
+    }
+    bool solution_is_valid() const { return solution_is_valid_; }
+    const double* get_best_rotation() const { return best_rot_cw_; }
+    const double* get_best_translation() const { return best_trans_cw_; }
+    void get_best_cam_pose(double (&pose_cw)[16]) const {
+        for (int r = 0; r < 4; ++r)
+            for (int c = 0; c < 4; ++c) pose_cw[r * 4 + c] = r < 3 ? (c < 3 ? best_rot_cw_[r * 3 + c] : best_trans_cw_[r]) : (c == 3 ? 1.0 : 0.0);
+    }
+    std::vector<bool> get_inlier_flags() const { return is_inlier_match_; }
+    int status() const { return status_; }  // B200_ERR_INVALID when a Jacobi SVD of the last call hit its sweep bound
+
+    // compute_pose (pnp_solver.h:95-97): rot_cw / trans_cw are written only when a candidate reaches reproj_error < DBL_MAX
+    static double compute_pose(b200_lba_t h, const std::vector<double>& bearing_vectors, const std::vector<double>& pos_ws, double (&rot_cw)[9],
+                               double (&trans_cw)[3], unsigned int num_iter = 5) {
+        b200_epnp_problem_t P{};
+        P.n = (int32_t)(bearing_vectors.size() / 3);
+        P.bearings = bearing_vectors.data();
+        P.points = pos_ws.data();
+        P.num_iter = num_iter;
+        for (int k = 0; k < 9; ++k) P.rot_cw[k] = rot_cw[k];
+        for (int k = 0; k < 3; ++k) P.trans_cw[k] = trans_cw[k];
+        check(b200_epnp_compute_pose(h, 1, &P), "b200_epnp_compute_pose");
+        check(P.status, "b200_epnp_compute_pose: Jacobi SVD");
+        for (int k = 0; k < 9; ++k) rot_cw[k] = P.rot_cw[k];
+        for (int k = 0; k < 3; ++k) trans_cw[k] = P.trans_cw[k];
+        return P.reproj_error;
+    }
+
+private:
+    unsigned int num_matches_;
+    std::vector<double> bearings_, points_;
+    std::vector<int32_t> octaves_;
+    std::vector<float> scale_factors_;
+    unsigned int min_num_inliers_, gauss_newton_num_iter_;
+    b200_mt19937_t engine_;
+    b200_lba_t h_ = nullptr;
+    bool own_ = false;
+    bool solution_is_valid_ = false;
+    int status_ = B200_OK;
+    double best_rot_cw_[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, best_trans_cw_[3] = {0, 0, 0};
+    std::vector<bool> is_inlier_match_;
+};
+
+}  // namespace solve
 }  // namespace b200

@@ -2864,6 +2864,23 @@ struct b200_lba_s {
     b200::lba::Solver s;
 };
 
+namespace b200 {
+namespace lba {
+// The device, stream and buffers of a handle, for entry points of other translation units that run on its stream (the PnP solver,
+// pnp_kernels.cu): at least dev_bytes of device arena and host_bytes of pinned staging, valid until the handle's next call.
+int borrow_buffers(b200_lba_t h, size_t dev_bytes, size_t host_bytes, cudaStream_t* stream, unsigned char** d, unsigned char** hst) {
+    Solver& S = h->s;
+    B200_CUDA(cudaSetDevice(S.device));
+    const int rc = S.ensure(dev_bytes, host_bytes, 0);
+    if (rc) return rc;
+    *stream = S.stream;
+    *d = S.d_arena;
+    *hst = S.h_stage;
+    return B200_OK;
+}
+}  // namespace lba
+}  // namespace b200
+
 static int lba_check_problem(const b200_lba_problem_t* P, const char* who) {
     if (P->n_poses < 0 || P->n_points < 0 || P->n_edges < 0 || P->n_cams < 0 || (P->n_poses > 0 && (!P->pose_cw || !P->pose_fixed))
         || (P->n_points > 0 && !P->points)

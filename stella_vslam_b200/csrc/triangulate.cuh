@@ -8,12 +8,10 @@
 // reprojection) are CUDA's libm, within 1-2 ulp of glibc; they only feed accept / reject comparisons (DESIGN.md section 4).
 #pragma once
 
-#include <cfloat>
+#include "jacobi.cuh"
 
 namespace b200 {
 namespace tri {
-
-constexpr int kMaxSweeps = 64;  // a 4x4 converges in a handful of sweeps; hitting the bound is reported, never looped on
 
 // One keyframe as the triangulator reads it (device copy of b200_tri_keyframe_t with device pointers).
 struct TriKfDev {
@@ -24,21 +22,6 @@ struct TriKfDev {
     const int* octave;
     const double* bearings;
 };
-
-__device__ __forceinline__ double dm(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double da(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double ds(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ double dd(double a, double b) { return __ddiv_rn(a, b); }
-__device__ __forceinline__ double dot3(double a0, double a1, double a2, double b0, double b1, double b2) {
-    return da(da(dm(a0, b0), dm(a1, b1)), dm(a2, b2));
-}
-
-// apply_rotation_in_the_plane(x, y, (c, s)) on element k of two vectors
-__device__ __forceinline__ void rot2(double& x, double& y, double c, double s) {
-    const double xi = x, yi = y;
-    x = da(dm(c, xi), dm(s, yi));
-    y = da(dm(-s, xi), dm(c, yi));
-}
 
 // Null vector (column of V for the smallest singular value) of the row-major 4x4 A.  Returns false when the sweeps did not converge.
 __device__ __forceinline__ bool jacobi_svd4_null(const double (&A)[16], double (&v)[4]) {
@@ -72,35 +55,8 @@ __device__ __forceinline__ bool jacobi_svd4_null(const double (&A)[16], double (
                 const double threshold = DBL_MIN < pm ? pm : DBL_MIN;
                 if (!(fabs(W[p * 4 + q]) > threshold || fabs(W[q * 4 + p]) > threshold)) continue;
                 finished = false;
-                // real_2x2_jacobi_svd
-                double m00 = W[p * 4 + p], m01 = W[p * 4 + q], m10 = W[q * 4 + p], m11 = W[q * 4 + q];
-                double c1 = 1.0, s1 = 0.0;
-                const double t = da(m00, m11), d = ds(m10, m01);
-                if (!(fabs(d) < DBL_MIN)) {
-                    const double u = dd(t, d);
-                    const double tmp = __dsqrt_rn(da(1.0, dm(u, u)));
-                    s1 = dd(1.0, tmp);
-                    c1 = dd(u, tmp);
-                }
-                if (!(c1 == 1.0 && s1 == 0.0)) {
-                    rot2(m00, m10, c1, s1);
-                    rot2(m01, m11, c1, s1);
-                }
-                // makeJacobi(m00, m01, m11)
-                double cr = 1.0, sr = 0.0;
-                const double deno = dm(2.0, fabs(m01));
-                if (!(deno < DBL_MIN)) {
-                    const double tau = dd(ds(m00, m11), deno);
-                    const double w = __dsqrt_rn(da(dm(tau, tau), 1.0));
-                    const double tt = tau > 0.0 ? dd(1.0, da(tau, w)) : dd(1.0, ds(tau, w));
-                    const double sign_t = tt > 0.0 ? 1.0 : -1.0;
-                    const double n = dd(1.0, __dsqrt_rn(da(dm(tt, tt), 1.0)));
-                    sr = dm(dm(dm(-sign_t, dd(m01, fabs(m01))), fabs(tt)), n);
-                    cr = n;
-                }
-                // j_left = rot1 * j_right^T
-                const double cl = ds(dm(c1, cr), dm(s1, -sr));
-                const double sl = da(dm(c1, -sr), dm(s1, cr));
+                double cl, sl, cr, sr;
+                jacobi_2x2(W[p * 4 + p], W[p * 4 + q], W[q * 4 + p], W[q * 4 + q], cl, sl, cr, sr);
                 if (!(cl == 1.0 && sl == 0.0)) {
 #pragma unroll
                     for (int k = 0; k < 4; ++k) rot2(W[p * 4 + k], W[q * 4 + k], cl, sl);

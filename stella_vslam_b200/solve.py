@@ -1,0 +1,201 @@
+"""Host-side mirror of solve::pnp_solver (src/stella_vslam/solve/pnp_solver.{h,cc}): EPnP inside RANSAC on the device
+(b200_pnp_ransac / b200_epnp_compute_pose on a b200_lba_t handle), with the minimal sets drawn on the host exactly as
+util::create_random_array draws them from the solver's std::mt19937 (b200_pnp_draw_min_sets).
+
+Arrays: bearings and points are (n, 3) float64, octaves (n,) int, scale_factors the ORB pyramid's float32 scale factors.
+"""
+import ctypes as C
+
+import numpy as np
+
+from ._lib import check, lib
+
+
+class PnpProblem(C.Structure):
+    """b200_pnp_problem_t (include/b200vslam.h)."""
+    _fields_ = [("n_matches", C.c_int32), ("bearings", C.c_void_p), ("points", C.c_void_p), ("octaves", C.c_void_p),
+                ("num_levels", C.c_int32), ("scale_factors", C.c_void_p), ("min_num_inliers", C.c_uint32),
+                ("gauss_newton_num_iter", C.c_uint32), ("max_num_iter", C.c_uint32), ("recompute", C.c_int32), ("min_sets", C.c_void_p),
+                ("status", C.c_int32), ("valid", C.c_int32), ("best_iter", C.c_int32), ("num_inliers", C.c_int32),
+                ("min_cost", C.c_double), ("rot_cw", C.c_double * 9), ("trans_cw", C.c_double * 3), ("inlier_flags", C.c_void_p)]
+
+
+class EpnpProblem(C.Structure):
+    """b200_epnp_problem_t (include/b200vslam.h)."""
+    _fields_ = [("n", C.c_int32), ("bearings", C.c_void_p), ("points", C.c_void_p), ("num_iter", C.c_uint32),
+                ("rot_cw", C.c_double * 9), ("trans_cw", C.c_double * 3), ("reproj_error", C.c_double), ("wrote", C.c_int32),
+                ("status", C.c_int32)]
+
+
+class Mt19937(C.Structure):
+    """b200_mt19937_t: std::mt19937's state."""
+    _fields_ = [("state", C.c_uint32 * 624), ("index", C.c_uint32)]
+
+
+def _L():
+    L = lib()
+    if not getattr(L, "_pnp_bound", False):
+        vp = C.c_void_p
+        L.b200_lba_create.argtypes = [C.c_int, C.POINTER(vp)]
+        L.b200_pnp_ransac.argtypes = [vp, C.c_int, C.POINTER(PnpProblem)]
+        L.b200_epnp_compute_pose.argtypes = [vp, C.c_int, C.POINTER(EpnpProblem)]
+        L.b200_mt19937_seed.argtypes = [C.POINTER(Mt19937), C.POINTER(C.c_uint32), C.c_int]
+        L.b200_mt19937_next.argtypes = [C.POINTER(Mt19937)]
+        L.b200_mt19937_next.restype = C.c_uint32
+        L.b200_pnp_draw_min_sets.argtypes = [C.POINTER(Mt19937), C.c_uint32, C.c_uint32, C.POINTER(C.c_int32)]
+        L._pnp_bound = True
+    return L
+
+
+_HANDLES = {}
+
+
+def _handle(device=0):
+    """One b200_lba_t per device for the PnP entry points (the handle of optimize.pose_optimizer serves as well)."""
+    if device not in _HANDLES:
+        h = C.c_void_p()
+        check(_L().b200_lba_create(device, C.byref(h)))
+        _HANDLES[device] = h
+    return _HANDLES[device]
+
+
+def mt19937(seed_seq=None):
+    """A std::mt19937: default-constructed (seed 5489) when seed_seq is None or empty, else seeded by std::seed_seq over the words."""
+    e = Mt19937()
+    words = np.ascontiguousarray(np.asarray([] if seed_seq is None else seed_seq, np.uint32))
+    check(_L().b200_mt19937_seed(C.byref(e), words.ctypes.data_as(C.POINTER(C.c_uint32)) if len(words) else None, len(words)))
+    return e
+
+
+def draw_min_sets(n_matches, max_num_iter, engine=None):
+    """max_num_iter calls of util::create_random_array(4, 0, n_matches - 1, engine), (max_num_iter, 4) int32.  engine: an Mt19937
+    (advanced in place) or None for a default-constructed one."""
+    e = mt19937() if engine is None else engine
+    out = np.zeros((max(int(max_num_iter), 1), 4), np.int32)
+    check(_L().b200_pnp_draw_min_sets(C.byref(e), int(n_matches), int(max_num_iter), out.ctypes.data_as(C.POINTER(C.c_int32))))
+    return out[:int(max_num_iter)]
+
+
+def _pack(prob, keep):
+    S = PnpProblem()
+    b = np.ascontiguousarray(np.asarray(prob["bearings"], np.float64).reshape(-1, 3))
+    p = np.ascontiguousarray(np.asarray(prob["points"], np.float64).reshape(-1, 3))
+    o = np.ascontiguousarray(np.asarray(prob["octaves"], np.int32).reshape(-1))
+    sf = np.ascontiguousarray(np.asarray(prob["scale_factors"], np.float32).reshape(-1))
+    ms = np.ascontiguousarray(np.asarray(prob.get("min_sets", np.zeros((0, 4))), np.int32).reshape(-1, 4))
+    fl = np.zeros(max(len(b), 1), np.uint8)
+    keep += [b, p, o, sf, ms, fl]
+    S.n_matches = len(b)
+    S.bearings, S.points, S.octaves = b.ctypes.data, p.ctypes.data, o.ctypes.data
+    S.num_levels, S.scale_factors = len(sf), sf.ctypes.data
+    S.min_num_inliers = int(prob.get("min_num_inliers", 10))
+    S.gauss_newton_num_iter = int(prob.get("gauss_newton_num_iter", 10))
+    S.max_num_iter = len(ms)
+    S.recompute = int(bool(prob.get("recompute", True)))
+    S.min_sets = ms.ctypes.data
+    S.inlier_flags = fl.ctypes.data
+    return S, fl
+
+
+def pnp_ransac_batch(problems, device=0):
+    """b200_pnp_ransac over dicts(bearings, points, octaves, scale_factors, min_sets (max_num_iter x 4), min_num_inliers=10,
+    gauss_newton_num_iter=10, recompute=True).  Returns per problem dict(status, valid, best_iter, num_inliers, min_cost, rot_cw, trans_cw,
+    inlier_flags (None on the early return)); rot_cw / trans_cw are None unless valid."""
+    keep, flags = [], []
+    arr = (PnpProblem * max(len(problems), 1))()
+    for i, pr in enumerate(problems):
+        arr[i], fl = _pack(pr, keep)
+        flags.append(fl)
+    check(_L().b200_pnp_ransac(_handle(device), len(problems), arr))
+    out = []
+    for i, pr in enumerate(problems):
+        S, n = arr[i], arr[i].n_matches
+        early = n < 4 or n < S.min_num_inliers
+        out.append(dict(status=S.status, valid=bool(S.valid), best_iter=S.best_iter, num_inliers=S.num_inliers, min_cost=S.min_cost,
+                        rot_cw=np.array(S.rot_cw).reshape(3, 3) if S.valid else None, trans_cw=np.array(S.trans_cw) if S.valid else None,
+                        inlier_flags=None if early else flags[i][:n].astype(bool)))
+    return out
+
+
+def compute_pose_batch(problems, device=0):
+    """b200_epnp_compute_pose over dicts(bearings, points, num_iter=5, rot_cw=None, trans_cw=None).  Returns per problem
+    dict(rot_cw, trans_cw, reproj_error, wrote, status); rot_cw / trans_cw are the given ones (zeros if None) when nothing was written."""
+    keep = []
+    arr = (EpnpProblem * max(len(problems), 1))()
+    for i, pr in enumerate(problems):
+        b = np.ascontiguousarray(np.asarray(pr["bearings"], np.float64).reshape(-1, 3))
+        p = np.ascontiguousarray(np.asarray(pr["points"], np.float64).reshape(-1, 3))
+        keep += [b, p]
+        S = arr[i]
+        S.n, S.bearings, S.points, S.num_iter = len(b), b.ctypes.data, p.ctypes.data, int(pr.get("num_iter", 5))
+        S.rot_cw[:] = [float(v) for v in np.asarray(pr["rot_cw"] if pr.get("rot_cw") is not None else np.zeros(9), np.float64).reshape(9)]
+        S.trans_cw[:] = [float(v) for v in np.asarray(pr["trans_cw"] if pr.get("trans_cw") is not None else np.zeros(3), np.float64).reshape(3)]
+    check(_L().b200_epnp_compute_pose(_handle(device), len(problems), arr))
+    return [dict(rot_cw=np.array(arr[i].rot_cw).reshape(3, 3), trans_cw=np.array(arr[i].trans_cw), reproj_error=arr[i].reproj_error,
+                 wrote=bool(arr[i].wrote), status=arr[i].status) for i in range(len(problems))]
+
+
+class pnp_solver:
+    """solve::pnp_solver.  The engine is the solver's member: find_via_ransac continues its state across calls."""
+
+    def __init__(self, valid_bearings, octaves, valid_points, scale_factors, min_num_inliers=10, use_fixed_seed=False,
+                 gauss_newton_num_iter=10, device=0):
+        self.bearings_ = np.ascontiguousarray(np.asarray(valid_bearings, np.float64).reshape(-1, 3))
+        self.points_ = np.ascontiguousarray(np.asarray(valid_points, np.float64).reshape(-1, 3))
+        self.octaves_ = np.asarray(octaves, np.int32).reshape(-1)
+        self.scale_factors_ = np.asarray(scale_factors, np.float32).reshape(-1)
+        n = len(self.bearings_)
+        if len(self.points_) != n or len(self.octaves_) != n:
+            raise ValueError("bearings, octaves and points must have one entry per match")
+        if n and (self.octaves_.min() < 0 or self.octaves_.max() >= len(self.scale_factors_)):
+            raise IndexError("octave outside the scale factors")  # std::vector::at throws in the reference
+        self.num_matches_ = n
+        self.min_num_inliers_ = int(min_num_inliers)
+        self.gauss_newton_num_iter_ = int(gauss_newton_num_iter)
+        self.device = device
+        # create_random_engine: a default-constructed engine, or one seeded by std::seed_seq over ten std::random_device words
+        self.random_engine_ = mt19937(None if use_fixed_seed else np.frombuffer(np.random.bytes(40), np.uint32))
+        self.solution_is_valid_ = False
+        self.best_rot_cw_ = np.zeros((3, 3))
+        self.best_trans_cw_ = np.zeros(3)
+        self.is_inlier_match = []
+        self.status_ = 0
+
+    def find_via_ransac(self, max_num_iter, recompute=True):
+        n = self.num_matches_
+        if n < 4 or n < self.min_num_inliers_:
+            self.solution_is_valid_ = False
+            return
+        ms = draw_min_sets(n, max_num_iter, self.random_engine_)
+        r = pnp_ransac_batch([dict(bearings=self.bearings_, points=self.points_, octaves=self.octaves_, scale_factors=self.scale_factors_,
+                                   min_num_inliers=self.min_num_inliers_, gauss_newton_num_iter=self.gauss_newton_num_iter_,
+                                   recompute=recompute, min_sets=ms)], self.device)[0]
+        self.status_ = r["status"]
+        self.solution_is_valid_ = r["valid"]
+        if r["valid"]:
+            self.best_rot_cw_, self.best_trans_cw_ = r["rot_cw"], r["trans_cw"]
+        self.is_inlier_match = [bool(v) for v in r["inlier_flags"]]
+
+    def solution_is_valid(self):
+        return self.solution_is_valid_
+
+    def get_best_rotation(self):
+        return self.best_rot_cw_.copy()
+
+    def get_best_translation(self):
+        return self.best_trans_cw_.copy()
+
+    def get_best_cam_pose(self):
+        T = np.eye(4)
+        T[:3, :3], T[:3, 3] = self.best_rot_cw_, self.best_trans_cw_
+        return T
+
+    def get_inlier_flags(self):
+        return list(self.is_inlier_match)
+
+    @staticmethod
+    def compute_pose(bearing_vectors, pos_ws, rot_cw=None, trans_cw=None, num_iter=5, device=0):
+        """Returns (reproj_error, rot_cw, trans_cw); the given rot_cw / trans_cw come back unchanged when no candidate was written."""
+        r = compute_pose_batch([dict(bearings=bearing_vectors, points=pos_ws, num_iter=num_iter, rot_cw=rot_cw, trans_cw=trans_cw)], device)[0]
+        check(r["status"])
+        return r["reproj_error"], r["rot_cw"], r["trans_cw"]

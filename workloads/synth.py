@@ -686,3 +686,65 @@ def make_mapping_problem(seed, n_neighbours=10, n_keypoints=2000, model="perspec
         R = _rodrigues(rng.normal(0, 0.06, 3))
         neighbours.append(view(R, c, n_keypoints, 0.7, 0.05))
     return cur, neighbours
+
+
+def make_pnp_problem(seed=0, n=300, inlier_frac=0.5, model="perspective", case=None):
+    """2D-3D matches of a lost frame for solve::pnp_solver, on make_pose_problem's geometry: a true pose, points at 2-60 m, inlier
+    bearings rotated away from the true ray by less than half of their octave's threshold (scale_factors[octave] degrees), outliers with
+    random bearings, octaves 0-7 with the float 1.2 recurrence.  model: "perspective" (bearings with z > 0, KITTI frustum) or "equirect"
+    (all directions, negative z included, so compute_pcs' sign flip is exercised).  case: None, "coplanar" (world points on one plane:
+    the pseudo-inverse of the barycentric coordinates drops a singular value <= 1e-6) or "min_inliers" (exactly 10 true inliers).
+    Returns dict(bearings, points, octaves, scale_factors, gt_rot_cw, gt_trans_cw, gt_inlier); min sets are drawn by the caller."""
+    rng = np.random.default_rng(seed)
+    equirect = model == "equirect"
+    sf = np.cumprod(np.concatenate([[np.float32(1.0)], np.full(7, np.float32(1.2))])).astype(np.float32)
+    Rcw = _rot_y(0.3 * rng.standard_normal()) @ _rodrigues(0.05 * rng.standard_normal(3))
+    tcw = rng.normal(0, 2.0, 3)
+    depth = rng.uniform(2, 60, n)
+    if equirect:
+        d = rng.standard_normal((n, 3))
+        pc = d / np.linalg.norm(d, axis=1, keepdims=True) * depth[:, None]
+    else:
+        u, v = rng.uniform(20, KITTI["cols"] - 20, n), rng.uniform(20, KITTI["rows"] - 20, n)
+        pc = np.stack([(u - KITTI["cx"]) / KITTI["fx"] * depth, (v - KITTI["cy"]) / KITTI["fy"] * depth, depth], 1)
+    if case == "coplanar" and n:
+        # a plane in the world: the camera-frame points are pushed onto R (z_w = 0) expressed in the camera
+        pw0 = (pc - tcw) @ Rcw
+        pw0[:, 2] = 0.0
+        pc = pw0 @ Rcw.T + tcw
+        if not equirect:
+            pc[:, 2] = np.abs(pc[:, 2]) + 2.0
+            pw0 = (pc - tcw) @ Rcw
+            pw0[:, 2] = 0.0
+            pc = pw0 @ Rcw.T + tcw
+    pw = (pc - tcw) @ Rcw
+    if case == "coplanar":
+        pw[:, 2] = 0.0
+        pc = pw @ Rcw.T + tcw
+    octaves = rng.integers(0, 8, n).astype(np.int32)
+    n_in = 10 if case == "min_inliers" else int(round(inlier_frac * n))
+    inl = np.zeros(n, bool)
+    inl[rng.permutation(n)[:n_in]] = True
+    ray = pc / np.linalg.norm(pc, axis=1, keepdims=True)
+    thr = np.deg2rad(sf[octaves].astype(np.float64))
+    # a perpendicular direction per ray, then a rotation by 5-45 % of the threshold: far from the decision boundary
+    perp = np.cross(ray, rng.standard_normal((n, 3)))
+    perp /= np.linalg.norm(perp, axis=1, keepdims=True)
+    ang = rng.uniform(0.05, 0.45, n) * thr
+    bear = np.cos(ang)[:, None] * ray + np.sin(ang)[:, None] * perp
+    out = ~inl
+    if out.any():
+        if equirect:
+            o = rng.standard_normal((out.sum(), 3))
+        else:
+            uo, vo = rng.uniform(20, KITTI["cols"] - 20, out.sum()), rng.uniform(20, KITTI["rows"] - 20, out.sum())
+            o = np.stack([(uo - KITTI["cx"]) / KITTI["fx"], (vo - KITTI["cy"]) / KITTI["fy"], np.ones(out.sum())], 1)
+        o /= np.linalg.norm(o, axis=1, keepdims=True)
+        # keep the outliers clearly outside their threshold (at least 3 x the octave's threshold off the true ray): a random bearing
+        # too close to the ray is replaced by the ray turned 4-6 thresholds away (z stays positive for the perspective frustum)
+        far = np.sum(o * ray[out], 1) < np.cos(3 * thr[out])
+        a = rng.uniform(4.0, 6.0, out.sum()) * thr[out]
+        turned = np.cos(a)[:, None] * ray[out] + np.sin(a)[:, None] * perp[out]
+        o[~far] = turned[~far]
+        bear[out] = o
+    return dict(bearings=bear, points=pw, octaves=octaves, scale_factors=sf, gt_rot_cw=Rcw, gt_trans_cw=tcw, gt_inlier=inl)
