@@ -12,9 +12,10 @@
 //
 // Layout: edges are sorted by landmark (CSR, built on the device), so every landmark-side quantity (Hll, bl, Dinv,
 // back-substitution) is a contiguous, atomics-free reduction; pose-side blocks are built by one CTA per free keyframe; the Schur
-// complement is a block-sparse  Hschur(i,j) = Hpp(i,j) - sum_l Hpl(i,l) Dinv(l) Hpl(j,l)^T  evaluated by one CTA per block row
-// whose 6x3 * 3x6 products are fp64 tensor-core instructions (DMMA).  Many windows are solved per launch sequence
-// (b200_lba_solve_batch).  Everything is deterministic (fixed reduction orders, no floating-point atomics).
+// complement is a block-sparse  Hschur(i,j) = Hpp(i,j) - sum_l Hpl(i,l) Dinv(l) Hpl(j,l)^T  evaluated from device-built lists of
+// the edge pairs that share a landmark, one list per block (i, j >= i), cut into chunks whose 6x6 partials are small GEMMs on the
+// fp64 tensor cores (DMMA).  Many windows are solved per launch sequence (b200_lba_solve_batch).  Everything is deterministic
+// (fixed reduction orders, no floating-point atomics).
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -247,12 +248,7 @@ struct WinDev {
     int* pose_start;  // Kf+1
     int* pose_edges;  // sorted-edge ids grouped by free pose, ascending (= landmark order)
     int4* rowrec;     // aligned with pose_edges: {edge a, its landmark (-1: the landmark is fixed), first edge of that landmark, its edge count}
-    int schur_split;  // CTAs that share one block row of the Schur complement (a function of the window's own size only)
-    int pad1;
-    double* schur_part;  // [Kf][schur_split][Kf - i tiles of 64]: partial accumulator tiles when schur_split > 1
-    int* row_tickets;    // (zeroed) Kf "last CTA of the row" tickets
-    const double* zeros; // (zeroed) what the lanes outside a 6x3 fragment read: >= kSchurFan records
-    // pair-list form of the Schur complement (default): the (edge a, edge c) pairs that share a landmark, grouped by the upper block
+    // pair-list form of the Schur complement: the (edge a, edge c) pairs that share a landmark, grouped by the upper block
     // (i <= j) of the reduced system they fall into, in landmark order, cut into chunks of kSchurChunk pairs
     unsigned long long* lm_mask;  // L x mask_words: bit p set <=> the (free) landmark has an edge of free keyframe column p
     int mask_words, n_blocks;
@@ -926,167 +922,15 @@ __global__ void __launch_bounds__(kRowThreads) pose_rows_kernel(const WinDev* __
     lm_after_build(W, stage);
 }
 
-// K3: Schur complement of the landmarks, one CTA per block ROW i of the reduced system:
-//        S(i,j) = sum_l Hpl(i,l) Dinv(l) Hpl(j,l)^T   (j >= i),     rhs_i = sum_l Hpl(i,l) Dinv(l) bl(l)
-//     The CTA walks the edges a of keyframe i in landmark order; for each one T = Hpl(a) Dinv(l) and then, for every edge c of the
-//     same landmark whose keyframe column is >= i (the landmark's edges are contiguous), the 6x6 product T Hpl(c)^T is ONE fp64
-//     tensor-core instruction (mma.sync m8n8k4: T padded to 8x4 as the A fragment, Hpl(c)^T padded to 4x8 as B -- for c == a column 6
-//     of B carries bl(l), so the same instruction yields the right-hand side) accumulated into the 8x8 accumulator tile of block
-//     (i, j) in shared memory, which is stored in fragment order (lane t owns elements 2t, 2t+1).  Every warp owns a contiguous
-//     part of keyframe i's edge list and a private set of accumulator tiles; the warps' tiles are added in index order, so the
-//     result is deterministic.  Output: block column i of  M = [Hpp + lambda I - S ; (bp - rhs)^T].
+// one fp64 tensor-core instruction (DMMA): D (8x8) += A (8x4) B (4x8); every lane holds one element of A, one of B and two of D
 __device__ __forceinline__ void dmma_m8n8k4(double& c0, double& c1, double a, double b) {
     asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
-constexpr int kSchurMaxWarps = 4;
-// kSchurUnroll (template): edges a in flight per warp (memory-level parallelism: the loop is a chain of L2 latencies otherwise)
-constexpr int kSchurFan = 8;     // edges c of a's landmark whose B fragments are prefetched; longer landmarks take the slow path
-// element (rr, nn) of block (i, i + jb) from the complete accumulator tile value s
-__device__ __forceinline__ void schur_store(const WinDev& W, int i, int jb, int el, double s, double lambda) {
-    const int rr = el >> 3, nn = el & 7;
-    if (rr >= 6 || nn >= 7 || (nn == 6 && jb != 0)) return;
-    const int n = W.n, ld = W.ld;
-    double* __restrict__ M = W.M;
-    if (nn == 6) {
-        M[(size_t)n * ld + 6 * i + rr] = W.bp[(size_t)i * 6 + rr] - s;  // rhs row
-    } else if (jb == 0) {
-        if (nn >= rr) M[(size_t)(6 * i + nn) * ld + 6 * i + rr] = W.Hpp[(size_t)i * 36 + rr * 6 + nn] + (rr == nn ? lambda : 0.0) - s;
-    } else {
-        M[(size_t)(6 * (i + jb) + nn) * ld + 6 * i + rr] = -s;  // lower triangle (j > i)
-    }
-}
-template <int kSchurUnroll>
-__global__ void __launch_bounds__(32 * kSchurMaxWarps) schur_rows_kernel(const WinDev* __restrict__ wins, int n_warps) {
-    extern __shared__ __align__(16) double sacc[];  // [n_warps][Kf - i][64]
-    const WinDev& W = wins[blockIdx.y];
-    const LmCtl* ctl = W.ctl;
-    if (!ctl->outer_go) return;
-    const int Kf = W.Kf, i = blockIdx.x, split = W.schur_split, part = blockIdx.z;
-    if (i >= Kf || part >= split) return;
-    const int nb = Kf - i;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int r = lane >> 2, k = lane & 3;  // A fragment: T[r][k];  B fragment: B[k][r] = Hpl(c)[r][k]
-    if (warp < n_warps) {
-        double2* __restrict__ acc = reinterpret_cast<double2*>(sacc + (size_t)warp * nb * 64);
-        for (int jb = 0; jb < nb; ++jb) acc[jb * 32 + lane] = make_double2(0.0, 0.0);
-        __syncwarp();
-        // this CTA's share of keyframe i's edge list, then this warp's share of that
-        const int a_lo = W.pose_start[i], a_hi = W.pose_start[i + 1];
-        const int per_cta = ceil_div(max(a_hi - a_lo, 1), split);
-        const int c_lo_ = a_lo + part * per_cta, c_hi_ = min(a_hi, c_lo_ + per_cta);
-        const int per = ceil_div(max(c_hi_ - c_lo_, 1), n_warps);
-        const int lo = c_lo_ + warp * per, hi = min(c_hi_, lo + per);
-        const int Lf = W.Lf;
-        const double* __restrict__ Hpl = W.Hpl;
-        const double* __restrict__ Dinv = W.Dinv;
-        const double* __restrict__ bl = W.bl;
-        const int* __restrict__ epcol = W.epcol;
-        const int4* __restrict__ recs = W.rowrec;
-        // D is symmetric, stored as (00, 01, 02, 11, 12, 22): column k of D
-        const int d0 = (k == 0) ? 0 : ((k == 1) ? 1 : 2), d1 = (k == 0) ? 1 : ((k == 1) ? 3 : 4), d2 = (k == 0) ? 2 : ((k == 1) ? 4 : 5);
-        const double* __restrict__ D0 = Dinv + (size_t)d0 * Lf;
-        const double* __restrict__ D1 = Dinv + (size_t)d1 * Lf;
-        const double* __restrict__ D2 = Dinv + (size_t)d2 * Lf;
-        const bool a_lane = r < 6 && k < 3, rhs_lane = r == 6 && k < 3;
-        // Lanes outside the 6x3 fragments read a block of zeros instead of being predicated off: every load below is unconditional
-        // with an immediate offset (the address arithmetic was two thirds of the instructions of the predicated form).
-        const double* __restrict__ zeros = W.zeros;
-        const double* __restrict__ bl_k = rhs_lane ? bl + (size_t)k * Lf : zeros;
-        const int frag = a_lane ? r * 3 + k : 0, row3 = a_lane ? r * 3 : 0;
-        double2 cd = make_double2(0.0, 0.0);  // tile of the diagonal block (i, i) + rhs column: touched by every edge, kept in registers
-        for (int pos = lo; pos < hi; pos += kSchurUnroll) {
-            int4 rec[kSchurUnroll];
-#pragma unroll
-            for (int u = 0; u < kSchurUnroll; ++u) rec[u] = (pos + u < hi) ? recs[pos + u] : make_int4(0, -1, 0, 0);
-            double t[kSchurUnroll], bdiag[kSchurUnroll], bv[kSchurUnroll][kSchurFan];
-            int pcs[kSchurUnroll];
-            // every load of the group is issued before the first tensor-core instruction consumes one
-#pragma unroll
-            for (int u = 0; u < kSchurUnroll; ++u) {
-                const int a = rec[u].x, lc = rec[u].y >= 0 ? W.pt_col[rec[u].y] : 0, c0 = rec[u].z, cnt = rec[u].y >= 0 ? rec[u].w : 0;
-                const double* __restrict__ ha = a_lane ? Hpl + (size_t)a * kHplStride + row3 : zeros;
-                const double h0 = ha[0], h1 = ha[1], h2 = ha[2];
-                t[u] = h0 * D0[lc] + h1 * D1[lc] + h2 * D2[lc];  // T = Hpl(a) Dinv(l); zero outside the fragment
-                // B of the diagonal pair (c == a): Hpl(a)^T in columns 0..5, bl(l) in column 6 (the right-hand side)
-                bdiag[u] = a_lane ? (k == 0 ? h0 : (k == 1 ? h1 : h2)) : bl_k[rhs_lane ? lc : 0];
-                pcs[u] = (lane < cnt) ? epcol[c0 + lane] : -1;
-                const double* __restrict__ hb = a_lane ? Hpl + (size_t)c0 * kHplStride + frag : zeros;  // (Hpl has kSchurFan records of slack)
-#pragma unroll
-                for (int j = 0; j < kSchurFan; ++j) bv[u][j] = hb[j * kHplStride];
-            }
-#pragma unroll
-            for (int u = 0; u < kSchurUnroll; ++u) {
-                const int cnt = rec[u].y >= 0 ? rec[u].w : 0;
-                if (cnt == 0) continue;
-                dmma_m8n8k4(cd.x, cd.y, t[u], bdiag[u]);
-                // A keyframe observes a landmark once, so the other edges c of the landmark fall into DIFFERENT accumulator tiles: their
-                // read-modify-write chains (LDS -> DMMA -> STS) are independent and are issued phase by phase instead of pair by pair.
-                // (A landmark listing the same keyframe twice, or one seen by more than kSchurFan keyframes, takes the serial path.)
-                const bool mine = lane < cnt && pcs[u] > i;
-                const unsigned peers = __match_any_sync(0xFFFFFFFFu, mine ? pcs[u] : -2 - lane);
-                const bool serial = cnt > kSchurFan || __any_sync(0xFFFFFFFFu, __popc(peers) > 1);
-                if (!serial) {
-                    double2 cc[kSchurFan];
-                    int tile[kSchurFan];
-#pragma unroll
-                    for (int j = 0; j < kSchurFan; ++j) {
-                        const int pc = __shfl_sync(0xFFFFFFFFu, pcs[u], j);
-                        tile[j] = (j < cnt && pc > i) ? (pc - i) * 32 + lane : -1;
-                        if (tile[j] >= 0) cc[j] = acc[tile[j]];
-                    }
-#pragma unroll
-                    for (int j = 0; j < kSchurFan; ++j)
-                        if (tile[j] >= 0) dmma_m8n8k4(cc[j].x, cc[j].y, t[u], bv[u][j]);
-#pragma unroll
-                    for (int j = 0; j < kSchurFan; ++j)
-                        if (tile[j] >= 0) acc[tile[j]] = cc[j];
-                    continue;
-                }
-                for (int j = 0; j < cnt; ++j) {
-                    const int c = rec[u].z + j;
-                    const int pc = epcol[c];
-                    if (pc <= i) continue;
-                    const double bq = a_lane ? Hpl[(size_t)c * kHplStride + frag] : 0.0;
-                    double2* slot = acc + (pc - i) * 32 + lane;
-                    double2 cc1 = *slot;
-                    dmma_m8n8k4(cc1.x, cc1.y, t[u], bq);
-                    *slot = cc1;
-                }
-            }
-        }
-        acc[lane] = cd;  // tile 0
-    }
-    __syncthreads();
-    const double lambda = ctl->lambda;
-    if (split == 1) {  // the CTA holds the complete row: add the warps' tiles in index order and write the block column
-        for (int idx = tid; idx < nb * 64; idx += blockDim.x) {
-            double s = 0.0;
-            for (int w2 = 0; w2 < n_warps; ++w2) s += sacc[(size_t)w2 * nb * 64 + idx];
-            schur_store(W, i, idx >> 6, idx & 63, s, lambda);
-        }
-        return;
-    }
-    // several CTAs share the row: publish this CTA's tiles, the last one to arrive adds the CTAs' tiles in index order
-    double* __restrict__ row_part = W.schur_part + ((size_t)Kf * (Kf + 1) / 2 - (size_t)nb * (nb + 1) / 2) * 64 * split;  // rows before i hold Kf .. nb+1 tiles
-    double* __restrict__ mine = row_part + (size_t)part * nb * 64;
-    for (int idx = tid; idx < nb * 64; idx += blockDim.x) {
-        double s = 0.0;
-        for (int w2 = 0; w2 < n_warps; ++w2) s += sacc[(size_t)w2 * nb * 64 + idx];
-        mine[idx] = s;
-    }
-    __shared__ int last_flag;
-    if (!last_cta_arrives(W.row_tickets + i, split, &last_flag)) return;
-    for (int idx = tid; idx < nb * 64; idx += blockDim.x) {
-        double s = 0.0;
-        for (int p2 = 0; p2 < split; ++p2) s += __ldcg(row_part + (size_t)p2 * nb * 64 + idx);
-        schur_store(W, i, idx >> 6, idx & 63, s, lambda);
-    }
-}
 
-// K5 (default): Schur complement from the pair list.  One warp reduces one chunk of <= 64 pairs of one block, every lane a pair:
-//        partial = sum T(a) Hpl(c)^T,  T(a) = Hpl(a) Dinv(l)   (+ for diagonal blocks  sum T(a) bl(l))
-//     with 42 register accumulators; the warp that publishes a block's last chunk adds the chunk partials in index order
-//     (deterministic) into  M = [Hpp + lambda I - sum ; (bp - sum)^T].  Blocks without any pair are filled by the warps past the chunks.
+// K5: Schur complement from the pair lists.  One warp (schur_mma_kernel) reduces one chunk of <= kSchurChunk pairs of one block:
+//        partial = sum T(a) Hpl(c)^T,  T(a) = Hpl(a) Dinv(l)   (+ for diagonal blocks  sum T(a) bl(l));
+//     the warp that publishes a block's last chunk adds the chunk partials in index order (deterministic) into
+//     M = [Hpp + lambda I - sum ; (bp - sum)^T].  Blocks without any pair are filled by the warps past the chunks.
 __device__ __forceinline__ void schur_finish_block(const WinDev& W, const SchurBlock sb, double lambda, int lane) {
     const double* __restrict__ partials = W.chunk_part;
     double* __restrict__ M = W.M;
@@ -1106,69 +950,6 @@ __device__ __forceinline__ void schur_finish_block(const WinDev& W, const SchurB
             M[(size_t)n * ld + 6 * sb.i + r] = W.bp[(size_t)sb.i * 6 + r] - sacc;  // rhs row
         }
     }
-}
-__global__ void __launch_bounds__(128) schur_chunks_kernel(const WinDev* __restrict__ wins) {
-    const WinDev& W = wins[blockIdx.y];
-    const LmCtl* ctl = W.ctl;
-    if (!ctl->outer_go) return;
-    const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    const int n_blocks = W.n_blocks, n_chunks = W.blk_chunk_start[n_blocks];
-    if (wid >= n_chunks) {
-        const int e = wid - n_chunks;
-        if (e < n_blocks) {
-            const SchurBlock sb = W.blocks[e];
-            if (sb.chunk_start == sb.chunk_end) schur_finish_block(W, sb, ctl->lambda, lane);  // no pair: just Hpp + lambda I, or zero
-        }
-        return;
-    }
-    const SchurChunk ch = W.chunks[wid];
-    const int Lf = W.Lf;
-    const double* __restrict__ Hpl = W.Hpl;
-    const double* __restrict__ Dinv = W.Dinv;
-    double acc[42];
-#pragma unroll
-    for (int i = 0; i < 42; ++i) acc[i] = 0.0;
-    for (int k = ch.start + lane; k < ch.end; k += 32) {
-        const int4 pr = W.pairs[k];
-        double ha[18], hc[18], t[18];
-        load18(Hpl + (size_t)pr.x * kHplStride, ha);
-        load18(Hpl + (size_t)pr.y * kHplStride, hc);
-        const int lc = pr.z;
-        const double D0 = Dinv[lc], D1 = Dinv[(size_t)Lf + lc], D2 = Dinv[(size_t)2 * Lf + lc];
-        const double D4 = Dinv[(size_t)3 * Lf + lc], D5 = Dinv[(size_t)4 * Lf + lc], D8 = Dinv[(size_t)5 * Lf + lc];
-#pragma unroll
-        for (int r = 0; r < 6; ++r) {
-            t[r * 3] = ha[r * 3] * D0 + ha[r * 3 + 1] * D1 + ha[r * 3 + 2] * D2;
-            t[r * 3 + 1] = ha[r * 3] * D1 + ha[r * 3 + 1] * D4 + ha[r * 3 + 2] * D5;
-            t[r * 3 + 2] = ha[r * 3] * D2 + ha[r * 3 + 1] * D5 + ha[r * 3 + 2] * D8;
-        }
-#pragma unroll
-        for (int r = 0; r < 6; ++r)
-#pragma unroll
-            for (int c = 0; c < 6; ++c) acc[r * 6 + c] += t[r * 3] * hc[c * 3] + t[r * 3 + 1] * hc[c * 3 + 1] + t[r * 3 + 2] * hc[c * 3 + 2];
-        if (ch.diag) {  // pr.x == pr.y: the edge of keyframe i to this landmark
-            const double b0 = W.bl[lc], b1 = W.bl[(size_t)Lf + lc], b2 = W.bl[(size_t)2 * Lf + lc];
-#pragma unroll
-            for (int r = 0; r < 6; ++r) acc[36 + r] += t[r * 3] * b0 + t[r * 3 + 1] * b1 + t[r * 3 + 2] * b2;
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < 42; ++i)
-#pragma unroll
-        for (int s = 16; s > 0; s >>= 1) acc[i] += __shfl_down_sync(0xFFFFFFFFu, acc[i], s);
-    const SchurBlock sb = W.blocks[ch.block];
-    int arrived = 0;
-    if (lane == 0) {
-#pragma unroll
-        for (int i = 0; i < 42; ++i) W.chunk_part[(size_t)wid * 42 + i] = acc[i];
-        __threadfence();
-        arrived = atomicAdd(&W.blk_done[ch.block], 1);
-    }
-    arrived = __shfl_sync(0xFFFFFFFFu, arrived, 0);
-    if (arrived != sb.chunk_end - sb.chunk_start - 1) return;
-    __threadfence();
-    schur_finish_block(W, sb, ctl->lambda, lane);
-    if (lane == 0) W.blk_done[ch.block] = 0;  // re-armed for the next trial
 }
 
 // K6: dense Cholesky of the reduced system (<= 6*Kf unknowns), solve, then the keyframe updates
@@ -1453,13 +1234,13 @@ __global__ void __launch_bounds__(kCholThreads) chol_solve_kernel(const WinDev* 
     }
 }
 
-// K5 (default since round 2b): the same pair-list chunks, but a chunk's block partial is formed as a small GEMM on the fp64 tensor cores:
+// K5 (pair-list chunks, one warp per chunk): a chunk's block partial is formed as a small GEMM on the fp64 tensor cores:
 //        S (6 x 6 | rhs) = [T_1 ... T_P] (6 x 3P) . [H_1 | b_1 ... H_P | b_P]^T (3P x 7),   T_p = Hpl(a_p) Dinv(l_p),  H_p = Hpl(c_p)
 //     Phase 1 (lane = pair, 32 pairs per pass): load the two 160-byte records and Dinv, form T, park T and H (and bl for diagonal
 //     blocks) in the warp's shared-memory operand tiles, r-major with a row stride of 100 doubles (conflict-free fragment loads).
 //     Phase 2: 24 x mma.sync.m8n8k4.f64 (DMMA) per pass, two LDS + one DMMA per lane and step; the 8 x 8 accumulator tile lives in two
-//     registers per lane for the whole chunk.  Against the lane-per-pair kernel above this removes the 42-accumulator warp reduction
-//     (630 of ~1050 instructions per chunk) and the 168-register footprint.  Summation order is fixed => deterministic.
+//     registers per lane for the whole chunk, so no per-lane accumulators have to be reduced across the warp.  Summation order is
+//     fixed => deterministic.
 constexpr int kSmmaKS = 100;                               // row stride of the operand tiles (K = 96 per pass, +4: bank spread)
 constexpr int kSmmaWarpDoubles = (6 + 7) * kSmmaKS;        // A: 6 rows, B: 7 rows (6 columns of H + the rhs column)
 __global__ void __launch_bounds__(128) schur_mma_kernel(const WinDev* __restrict__ wins) {
@@ -2221,12 +2002,7 @@ struct Solver {
     std::vector<int> prof_kind;
     float prof_ms[8] = {};
     int prof_n[8] = {};
-    // Schur complement: pair lists reduced by scalar fp64 FMAs (default) or block rows with fp64 tensor-core products
-    // (B200_LBA_SCHUR_MODE=rows; tuning knobs B200_LBA_SCHUR=unroll,warps,ctas)
-    bool schur_rows = false;
     bool force_offchip = false;
-    int schur_mode = 0;  // 0: pair-list chunks on the fp64 tensor cores (default), 1: pair-list chunks with FMA, 2: DMMA rows
-    int schur_unroll = 4, schur_warps = kSchurMaxWarps, schur_ctas = 160;
     int chol_cluster = kCholCluster;  // CTAs sharing one factorisation (B200_LBA_CLUSTER overrides: 1, 2, 4 or 8)
     bool chol_cluster_pinned = false;
     // Waiting for the stream (a few times per batch).  B200_LBA_WAIT=spin|block|yield|nap overrides.
@@ -2305,8 +2081,8 @@ struct Carver {
 // per-window byte offsets into the arena
 struct WinOff {
     size_t cams, e_pose, e_point, e_cam, e_robust, e_can, e_obs, e_isig, e_delta, pose_col, pt_col, q0, t0, Rt0, pts0;  // uploaded
-    size_t pt_cnt, pose_cnt, level, chi0, fail, tickets, bad, row_tickets, blk_done;                                                         // zeroed
-    size_t pt_start, order, edges, epcol, pose_start, pose_edges, rowrec, schur_part, lm_mask, blk_cnt, blk_pair_start, blk_chunk_start, pairs, blocks, chunks,
+    size_t pt_cnt, pose_cnt, level, chi0, fail, tickets, bad, blk_done;                                                                      // zeroed
+    size_t pt_start, order, edges, epcol, pose_start, pose_edges, rowrec, lm_mask, blk_cnt, blk_pair_start, blk_chunk_start, pairs, blocks, chunks,
         chunk_part, robust, q1, t1, Rt1, pts1, chi1, Hpl, Hll, bl, Dinv, Hpp, bp, M, xp, r_chi,
         r_diag, r_scale, r_result, gP, gD, ginvd;                                                                     // scratch
     size_t exp_begin, qf, tf, pf, out, exp_end;                                                                       // export block
@@ -2347,12 +2123,12 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
     if (nw == 0) return ret;
     // ---- per-window sizes and the free-vertex columns (O(K + L) on the host; everything O(E) happens on the device) ----------
     struct HostWin {
-        int K, L, E, Kf, Lf, n, ld, lbc, split, mask_words, n_blocks, n_chunks_bound;
+        int K, L, E, Kf, Lf, n, ld, lbc, mask_words, n_blocks, n_chunks_bound;
         size_t n_pairs;
         std::vector<int> pose_col, pt_col;
     };
     std::vector<HostWin> hw(nw);
-    int maxE = 1, maxL = 1, maxKf = 1, maxK = 1, max_n = 0, max_lbc = 1, max_split = 1, max_blocks = 1, max_chunk_warps = 1;
+    int maxE = 1, maxL = 1, maxKf = 1, maxK = 1, max_n = 0, max_lbc = 1, max_blocks = 1, max_chunk_warps = 1;
     std::vector<int> deg;
     for (int x = 0; x < nw; ++x) {
         const b200_lba_problem_t& P = Ps[act[x]];
@@ -2371,23 +2147,17 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
         h.n = 6 * h.Kf;
         h.ld = h.n + 2;
         h.lbc = std::max(1, ceil_div(h.L, 16));
-        // CTAs per block row of the Schur complement: enough CTAs for one window to fill the chip, chosen from the window's own size
-        // only so that a window gives the same bits whatever batch it is solved in
-        h.split = std::max(1, std::min(8, ceil_div(S.schur_ctas, std::max(h.Kf, 1))));
-        max_split = std::max(max_split, h.split);
         // pairs of the Schur complement: every landmark with m free-keyframe observations contributes m (m + 1) / 2 (one counting pass
         // over the observations; everything else that is O(E) happens on the device)
         h.mask_words = std::max(1, ceil_div(h.Kf, 64));
         h.n_blocks = h.Kf * (h.Kf + 1) / 2;
         h.n_pairs = 0;
-        if (!S.schur_rows) {
-            deg.assign(std::max(h.L, 1), 0);
-            for (int e = 0; e < h.E; ++e) {
-                const int p = P.e_point[e], k = P.e_pose[e];
-                if (p >= 0 && p < h.L && k >= 0 && k < h.K && h.pose_col[k] >= 0 && h.pt_col[p] >= 0) deg[p]++;
-            }
-            for (int l = 0; l < h.L; ++l) h.n_pairs += (size_t)deg[l] * (deg[l] + 1) / 2;
+        deg.assign(std::max(h.L, 1), 0);
+        for (int e = 0; e < h.E; ++e) {
+            const int p = P.e_point[e], k = P.e_pose[e];
+            if (p >= 0 && p < h.L && k >= 0 && k < h.K && h.pose_col[k] >= 0 && h.pt_col[p] >= 0) deg[p]++;
         }
+        for (int l = 0; l < h.L; ++l) h.n_pairs += (size_t)deg[l] * (deg[l] + 1) / 2;
         h.n_chunks_bound = (int)(h.n_pairs / kSchurChunk) + h.n_blocks + 1;
         max_blocks = std::max(max_blocks, h.n_blocks);
         max_chunk_warps = std::max(max_chunk_warps, h.n_chunks_bound + h.n_blocks);
@@ -2414,10 +2184,8 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
         const HostWin& h = hw[x];
         WinOff& o = wo[x];
         o.pt_cnt = cv.take<int>(h.L); o.pose_cnt = cv.take<int>(h.Kf); o.level = cv.take<unsigned char>(h.E); o.chi0 = cv.take<double>(h.E);
-        o.fail = cv.take<int>(1); o.tickets = cv.take<int>(2); o.bad = cv.take<int>(1); o.row_tickets = cv.take<int>(h.Kf);
-        o.blk_done = cv.take<int>(h.n_blocks);
+        o.fail = cv.take<int>(1); o.tickets = cv.take<int>(2); o.bad = cv.take<int>(1); o.blk_done = cv.take<int>(h.n_blocks);
     }
-    const size_t o_zeros = cv.take<double>(kHplStride * (kSchurFan + 1));
     const size_t zero_end = round_up(cv.off, (size_t)256);
     cv.off = zero_end;
     for (int x = 0; x < nw; ++x) {
@@ -2426,13 +2194,12 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
         const size_t E = h.E, K = h.K, L = h.L, Kf = h.Kf, Lf = h.Lf;
         o.pt_start = cv.take<int>(L + 1); o.order = cv.take<int>(E); o.edges = cv.take<EdgeS>(E); o.epcol = cv.take<int>(E);
         o.pose_start = cv.take<int>(Kf + 1); o.pose_edges = cv.take<int>(E); o.rowrec = cv.take<int4>(E);
-        o.schur_part = cv.take<double>((S.schur_rows && h.split > 1) ? (size_t)h.split * 64 * (Kf * (Kf + 1) / 2) : 0);
         o.lm_mask = cv.take<unsigned long long>(L * (size_t)h.mask_words); o.blk_cnt = cv.take<int>(h.n_blocks);
         o.blk_pair_start = cv.take<int>(h.n_blocks + 1); o.blk_chunk_start = cv.take<int>(h.n_blocks + 1); o.pairs = cv.take<int4>(h.n_pairs);
         o.blocks = cv.take<SchurBlock>(h.n_blocks); o.chunks = cv.take<SchurChunk>(h.n_chunks_bound);
         o.chunk_part = cv.take<double>(42 * (size_t)h.n_chunks_bound); o.robust = cv.take<unsigned char>(E);
         o.q1 = cv.take<double>(4 * K); o.t1 = cv.take<double>(3 * K); o.Rt1 = cv.take<double>(12 * K); o.pts1 = cv.take<double>(3 * L);
-        o.chi1 = cv.take<double>(E); o.Hpl = cv.take<double>(kHplStride * (E + kSchurFan)); o.Hll = cv.take<double>(6 * Lf); o.bl = cv.take<double>(3 * Lf);
+        o.chi1 = cv.take<double>(E); o.Hpl = cv.take<double>(kHplStride * E); o.Hll = cv.take<double>(6 * Lf); o.bl = cv.take<double>(3 * Lf);
         o.Dinv = cv.take<double>(6 * Lf); o.Hpp = cv.take<double>(36 * Kf); o.bp = cv.take<double>(6 * Kf);
         o.M = cv.take<double>((size_t)(h.n + 1) * h.ld); o.xp = cv.take<double>(h.n);
         o.gP = o.gD = o.ginvd = 0;
@@ -2513,8 +2280,7 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
         W.pt_cnt = (int*)(d + o.pt_cnt); W.pt_start = (int*)(d + o.pt_start); W.order = (int*)(d + o.order); W.edges = (EdgeS*)(d + o.edges);
         W.epcol = (int*)(d + o.epcol); W.pose_cnt = (int*)(d + o.pose_cnt); W.pose_start = (int*)(d + o.pose_start);
         W.pose_edges = (int*)(d + o.pose_edges); W.level = d + o.level; W.robust = d + o.robust;
-        W.rowrec = (int4*)(d + o.rowrec); W.schur_split = h.split; W.schur_part = (double*)(d + o.schur_part); W.row_tickets = (int*)(d + o.row_tickets);
-        W.zeros = (const double*)(d + o_zeros);
+        W.rowrec = (int4*)(d + o.rowrec);
         W.lm_mask = (unsigned long long*)(d + o.lm_mask); W.mask_words = h.mask_words; W.n_blocks = h.n_blocks; W.blk_cnt = (int*)(d + o.blk_cnt);
         W.blk_pair_start = (int*)(d + o.blk_pair_start); W.blk_chunk_start = (int*)(d + o.blk_chunk_start); W.pairs = (int4*)(d + o.pairs);
         W.blocks = (SchurBlock*)(d + o.blocks); W.chunks = (SchurChunk*)(d + o.chunks); W.chunk_part = (double*)(d + o.chunk_part);
@@ -2563,25 +2329,16 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
     plan_place_kernel<<<dim3(ceil_div(maxE, 256), nw), 256, 0, st>>>(wins);
     plan_sort_kernel<<<dim3(ceil_div(maxL, 128), nw), 128, 0, st>>>(wins);
     plan_pose_lists_kernel<<<dim3(maxKf, nw), kListThreads, 0, st>>>(wins);
-    launches += 5;
-    if (!S.schur_rows) {
-        plan_pairs_kernel<false><<<dim3(ceil_div(max_blocks, 4), nw), 128, 0, st>>>(wins);
-        plan_pair_scan_kernel<<<nw, 1024, 0, st>>>(wins);
-        plan_pairs_kernel<true><<<dim3(ceil_div(max_blocks, 4), nw), 128, 0, st>>>(wins);
-        launches += 3;
-    }
+    plan_pairs_kernel<false><<<dim3(ceil_div(max_blocks, 4), nw), 128, 0, st>>>(wins);
+    plan_pair_scan_kernel<<<nw, 1024, 0, st>>>(wins);
+    plan_pairs_kernel<true><<<dim3(ceil_div(max_blocks, 4), nw), 128, 0, st>>>(wins);
+    launches += 8;
     if ((rc = mark(0))) return rc;
     B200_RANGE("b200:lba:rounds+export");  // (the plan above is the part of b200:lba:batch outside this range)
     // ---- LM rounds in lockstep ---------------------------------------------------------------------------------------------------
     const bool large = max_n > kCholOnChipMax || S.force_offchip;  // (B200_LBA_FORCE_OFFCHIP: the panel-by-panel path on any size, for tests)
     const size_t chol_smem = sizeof(double) * ((size_t)kNB * (kNB + 1) + 4 + (size_t)((std::min(max_n, kCholOnChipMax) + 1 + 3) & ~3) * kNB);
     B200_CUDA(cudaFuncSetAttribute(chol_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)chol_smem));
-    // warps per Schur row CTA: every warp owns Kf accumulator tiles of 512 bytes
-    int schur_warps = std::min(kSchurMaxWarps, std::max(1, S.schur_warps));
-    while (schur_warps > 1 && (size_t)schur_warps * maxKf * 512 > 200 * 1024) schur_warps >>= 1;
-    const size_t schur_smem = (size_t)schur_warps * maxKf * 512;
-    B200_CUDA(cudaFuncSetAttribute(schur_rows_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)schur_smem));
-    B200_CUDA(cudaFuncSetAttribute(schur_rows_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)schur_smem));
     // 8-CTA clusters must sit inside one GPC, so not many of them are co-resident: batches use the smaller cluster (H100 SXM, four
     // windows per batch: 0.18 ms per factorisation with clusters of 4, 0.20 with 2, 0.28 with 8); B200_LBA_CLUSTER pins it
     const int chol_cluster = S.chol_cluster_pinned ? S.chol_cluster : (nw <= 2 ? 8 : 4);
@@ -2593,10 +2350,7 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
         pose_rows_kernel<<<dim3(maxKf, nw), kRowThreads, 0, st>>>(wins);
         if ((rcm = mark(2))) return rcm;
         // one LM trial (every window that is still iterating)
-        if (S.schur_mode == 0) schur_mma_kernel<<<dim3(ceil_div(max_chunk_warps, 4), nw), 128, 4 * kSmmaWarpDoubles * sizeof(double), st>>>(wins);
-        else if (S.schur_mode == 1) schur_chunks_kernel<<<dim3(ceil_div(max_chunk_warps, 4), nw), 128, 0, st>>>(wins);
-        else if (S.schur_unroll == 2) schur_rows_kernel<2><<<dim3(maxKf, nw, max_split), 32 * schur_warps, schur_smem, st>>>(wins, schur_warps);
-        else schur_rows_kernel<4><<<dim3(maxKf, nw, max_split), 32 * schur_warps, schur_smem, st>>>(wins, schur_warps);
+        schur_mma_kernel<<<dim3(ceil_div(max_chunk_warps, 4), nw), 128, 4 * kSmmaWarpDoubles * sizeof(double), st>>>(wins);
         if ((rcm = mark(3))) return rcm;
         if (large) {  // panel by panel over the whole chip (every window of the batch takes this path; small ones finish early)
             for (int kb = 0; kb < max_n; kb += kNB) {
@@ -2921,18 +2675,6 @@ int b200_lba_create(int device, b200_lba_t* out) {
         }
     }
     if (const char* fo = getenv("B200_LBA_FORCE_OFFCHIP")) h->s.force_offchip = fo[0] == '1';
-    if (const char* sm = getenv("B200_LBA_SCHUR_MODE")) {  // mma (default) | pairs | rows
-        h->s.schur_mode = sm[0] == 'r' ? 2 : (sm[0] == 'p' ? 1 : 0);
-        h->s.schur_rows = sm[0] == 'r';
-    }
-    if (const char* sc = getenv("B200_LBA_SCHUR")) {
-        int u = 4, w2 = 4, c2 = 160;
-        if (sscanf(sc, "%d,%d,%d", &u, &w2, &c2) >= 1) {
-            h->s.schur_unroll = (u == 2) ? 2 : 4;
-            h->s.schur_warps = std::max(1, std::min(4, w2));
-            h->s.schur_ctas = std::max(1, c2);
-        }
-    }
     if (const char* w = getenv("B200_LBA_WAIT")) h->s.wait_mode = w[0] == 'b' ? 1 : (w[0] == 'y' ? 2 : (w[0] == 'n' ? 3 : 0));  // spin | block | yield | nap
     if (e != cudaSuccess) {
         delete h;

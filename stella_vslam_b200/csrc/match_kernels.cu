@@ -8,7 +8,7 @@
 // brute_force_match is sequential in the reference: keyframe keypoints idx_2 are visited in order and every accepted
 // match removes its frame keypoint idx_1 from all later searches.  Restated here as
 //   (1) a fully parallel pass that keeps, per idx_2, the K smallest (distance, idx_1) keys over the orientation-gated
-//       frame keypoints (uint4 loads of the descriptors, __popc on the XOR), and
+//       frame keypoints (an int8 GEMM on the tensor cores, listing only distances that can still decide a match), and
 //   (2) an in-order resolve (one warp per problem) that walks each list skipping taken idx_1; when a list cannot decide
 //       the outcome exactly (too many of its entries were taken) the warp recomputes that row against the live set.
 // Both steps are exact, so the match pairs equal the reference's bit for bit.
@@ -28,8 +28,7 @@ namespace b200 {
 namespace match {
 
 constexpr int kTopK = 8;            // candidates kept per keyframe keypoint
-constexpr int kRowsPerBlock = 64;   // one keyframe keypoint per thread (small CTAs: a 2000-row problem still yields 32 of them)
-constexpr int kChunk = 256;         // frame descriptors staged per shared-memory tile (8 KB)
+constexpr int kListRowAlign = 64;   // a problem's candidate lists are padded to a multiple of this many keyframe rows
 constexpr unsigned kInfKey = 0xFFFFFFFFu;
 constexpr unsigned kSentinelIdx = 0x3FFFFFu;  // index no keypoint can have (frames hold < 2^22 - 1 keypoints)
 constexpr int kThrLow = 50;         // HAMMING_DIST_THR_LOW  (match/base.h:15)
@@ -74,7 +73,7 @@ __global__ void __launch_bounds__(256) hamming_matrix_kernel(const uint4* __rest
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// (1) top-K candidate lists.  grid = (ceil(max_n2 / 128), n_problems); thread = one keyframe keypoint idx_2.
+// the two sides of a batch of matching problems
 // ---------------------------------------------------------------------------------------------------------------
 struct Side {                       // one side of the problems: descriptors, strided angles, per-problem (offset, count)
     const uint4* desc;
@@ -87,70 +86,16 @@ __device__ __forceinline__ float side_angle(const Side& s, int i) {
     return *reinterpret_cast<const float*>(s.angle + (long long)i * s.angle_stride);
 }
 
-__global__ void __launch_bounds__(kRowsPerBlock) topk_kernel(Side S1, Side S2, const unsigned char* __restrict__ valid2,
-                                                            int check_orientation, unsigned* __restrict__ lists) {
-    __shared__ uint4 s1[kChunk * 2];
-    __shared__ float sa[kChunk];
-    const uint4* __restrict__ desc1 = S1.desc;
-    const uint4* __restrict__ desc2 = S2.desc;
-    const int p = blockIdx.y;
-    const int b1 = S1.off[p], n1 = S1.cnt[p];
-    const int b2 = S2.off[p], n2 = S2.cnt[p];
-    if ((int)(blockIdx.x * kRowsPerBlock) >= n2) return;
-    const int row = blockIdx.x * kRowsPerBlock + threadIdx.x;
-    const bool active = row < n2 && (!valid2 || valid2[b2 + row]);
-    uint4 q0 = make_uint4(0, 0, 0, 0), q1 = q0;
-    float qa = 0.f;
-    if (active) {
-        q0 = desc2[(size_t)(b2 + row) * 2];
-        q1 = desc2[(size_t)(b2 + row) * 2 + 1];
-        qa = side_angle(S2, b2 + row);
-    }
-    unsigned top[kTopK];
-#pragma unroll
-    for (int k = 0; k < kTopK; ++k) top[k] = kInfKey;
-    for (int c0 = 0; c0 < n1; c0 += kChunk) {
-        const int cn = min(kChunk, n1 - c0);
-        __syncthreads();
-        for (int t = threadIdx.x; t < cn * 2; t += blockDim.x) s1[t] = desc1[(size_t)(b1 + c0) * 2 + t];
-        for (int t = threadIdx.x; t < cn; t += blockDim.x) sa[t] = side_angle(S1, b1 + c0 + t);
-        __syncthreads();
-        if (!active) continue;
-#pragma unroll 4
-        for (int j = 0; j < cn; ++j) {
-            const unsigned dist = hamming256(q0, q1, s1[2 * j], s1[2 * j + 1]);
-            const unsigned key = make_key(dist, (unsigned)(c0 + j));
-            if (key < top[kTopK - 1]) {
-                if (check_orientation && orientation_rejects(sa[j], qa)) continue;
-                top[kTopK - 1] = key;
-#pragma unroll
-                for (int k = kTopK - 1; k > 0; --k) {
-                    if (top[k] < top[k - 1]) {
-                        const unsigned t = top[k];
-                        top[k] = top[k - 1];
-                        top[k - 1] = t;
-                    }
-                }
-            }
-        }
-    }
-    if (row < n2) {
-        unsigned* o = lists + ((size_t)p * gridDim.x * kRowsPerBlock + row) * kTopK;
-#pragma unroll
-        for (int k = 0; k < kTopK; ++k) o[k] = top[k];
-    }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
-// (1b) top-K candidate lists on the Hopper tensor cores.  The Hamming distance of two 256-bit descriptors is a dot product in
+// (1) top-K candidate lists on the Hopper tensor cores.  The Hamming distance of two 256-bit descriptors is a dot product in
 //      disguise: with the bits mapped to +-1,  popcount(a ^ b) = (256 - <a, b>) / 2  -- exact in int32 -- so the all-pairs distance
 //      matrix of a (frame, keyframe) pair is a 2000 x 2000 x 256 int8 GEMM.  One CTA owns 128 keyframe rows (the A operand, expanded
 //      once into shared memory in the K-major no-swizzle core-matrix layout: 8 rows x 16 bytes per core matrix) and walks the frame's
 //      keypoints in chunks of 128 (the B operand, expanded by the same threads into one of two buffers).  Each of the two warpgroups
 //      issues wgmma.mma_async.m64n128k32.s32.s8.s8 (8 per chunk) for its 64 rows with the accumulators in registers; while the tensor
 //      core works on chunk c the threads expand chunk c+1 into the other buffer, then every thread scans its accumulator fragment (two
-//      rows x 32 columns) and keeps, per row, the smallest (distance, index) keys that pass the orientation gate -- the selection of
-//      topk_kernel up to a distance cap that cannot change a decision.  The four lanes of a quad hold the same two rows; their lists
+//      rows x 32 columns) and keeps, per row, the kTopK smallest (distance, index) keys that pass the orientation gate, among the
+//      distances up to a cap that cannot change a decision.  The four lanes of a quad hold the same two rows; their lists
 //      are merged at the end.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kTcRows = 128;        // keyframe rows per CTA (two m64 tiles); two CTAs share an SM: one stages / waits while the other selects
@@ -1296,8 +1241,6 @@ struct Matcher {
     cudaEvent_t ev_t[3] = {nullptr, nullptr, nullptr};
     cudaEvent_t ev_track[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // b200_track_local_map stage boundaries
     bool track_timed = false;
-    // all-pairs distances + top-K on the tensor cores (wgmma, int8 +-1 GEMM) or on the POPC pipe (B200_MATCH_TOPK=popc)
-    bool use_tensor_core = true;
     int join() {  // the main stream waits for the side stream's resolve
         if (resolve_pending) {
             B200_CUDA(cudaStreamWaitEvent(stream, ev_resolved, 0));
@@ -1361,20 +1304,16 @@ struct Matcher {
             return B200_ERR_CAPACITY;
         }
         const int taken_words = ceil_div(max_n1, 32);
-        const int row_blocks = std::max(1, ceil_div(max_n2, kRowsPerBlock)), list_rows = row_blocks * kRowsPerBlock;
+        const int list_rows = std::max(1, ceil_div(max_n2, kListRowAlign)) * kListRowAlign;
         if ((rc = grow((void**)&d_lists, &lists_cap, sizeof(unsigned) * kTopK * (size_t)list_rows * n_problems))) return rc;
         if ((rc = grow((void**)&d_matched, &matched_cap, sizeof(int) * (size_t)max_n1 * n_problems))) return rc;
         if ((rc = grow((void**)&d_taken, &taken_cap, sizeof(unsigned) * (size_t)taken_words * n_problems))) return rc;
         if (timing) B200_CUDA(cudaEventRecord(ev_t[0], stream));
-        if (use_tensor_core) {
-            const float need = lowe > 0.f ? std::ceil((float)kThrLow / lowe) + 1.f : (float)kMaxDist;
-            const unsigned cap = (unsigned)std::min((float)kMaxDist, std::max((float)kThrLow, need));
-            B200_CUDA(cudaFuncSetAttribute(topk_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcSmem) + 1024));
-            topk_tc_kernel<<<dim3(ceil_div(std::max(max_n2, 1), kTcRows), n_problems), kTcThreads, sizeof(TcSmem) + 1024, stream>>>(
-                S1, S2, (const unsigned char*)valid2, check_ori, d_lists, list_rows, cap);
-        } else {
-            topk_kernel<<<dim3(row_blocks, n_problems), kRowsPerBlock, 0, stream>>>(S1, S2, (const unsigned char*)valid2, check_ori, d_lists);
-        }
+        const float need = lowe > 0.f ? std::ceil((float)kThrLow / lowe) + 1.f : (float)kMaxDist;
+        const unsigned cap = (unsigned)std::min((float)kMaxDist, std::max((float)kThrLow, need));
+        B200_CUDA(cudaFuncSetAttribute(topk_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcSmem) + 1024));
+        topk_tc_kernel<<<dim3(ceil_div(std::max(max_n2, 1), kTcRows), n_problems), kTcThreads, sizeof(TcSmem) + 1024, stream>>>(
+            S1, S2, (const unsigned char*)valid2, check_ori, d_lists, list_rows, cap);
         if (timing) B200_CUDA(cudaEventRecord(ev_t[1], stream));
         const size_t state_bytes = sizeof(unsigned) * ((size_t)taken_words + 2 * (size_t)max_n1);  // taken bitmap, idx_1 -> idx_2 table, claim table
         const size_t stage_bytes = sizeof(unsigned) * 9 * (size_t)max_n1;
@@ -1429,7 +1368,6 @@ int b200_matcher_create(int device, b200_matcher_t* out) {
         return b200::cuda_fail(e, "stream creation", __FILE__, __LINE__);
     }
     h->m.stream = h->m.own_stream;
-    if (const char* tk = getenv("B200_MATCH_TOPK")) h->m.use_tensor_core = !(tk[0] == 'p');
     *out = h;
     return B200_OK;
 }

@@ -37,19 +37,15 @@ def case_orb():
 
 def case_match():
     total = 0
-    for topk in ("tc", "popc"):                      # both top-K kernels (wgmma and XOR/POPC), then the same resolve
-        os.environ["B200_MATCH_TOPK"] = topk
-        match._tls.matchers = {}                    # the env knob is read when a matcher handle is created
-        for n1, n2, seed in [(300, 280, 1), (129, 517, 2), (1, 1, 3)]:
-            d1, a1, d2, a2, v2 = synth.make_descriptor_pair(n1, n2, seed=seed)
-            m = match.robust(0.8, True)
-            got = m.brute_force_match(d1, a1, d2, a2, v2)
-            want = O.brute_force_match(d1, a1, d2, a2, v2, 0.8, True)
-            assert np.array_equal(got, want), (topk, n1, n2)
-            total += len(got)
-        D = match.hamming_matrix(d1, d2)
-        assert D.shape == (len(d1), len(d2))
-    os.environ.pop("B200_MATCH_TOPK", None)
+    for n1, n2, seed in [(300, 280, 1), (129, 517, 2), (1, 1, 3)]:
+        d1, a1, d2, a2, v2 = synth.make_descriptor_pair(n1, n2, seed=seed)
+        m = match.robust(0.8, True)
+        got = m.brute_force_match(d1, a1, d2, a2, v2)
+        want = O.brute_force_match(d1, a1, d2, a2, v2, 0.8, True)
+        assert np.array_equal(got, want), (n1, n2)
+        total += len(got)
+    D = match.hamming_matrix(d1, d2)
+    assert D.shape == (len(d1), len(d2))
     return total
 
 
