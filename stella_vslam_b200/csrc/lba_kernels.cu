@@ -359,7 +359,9 @@ __global__ void __launch_bounds__(128) plan_sort_kernel(const WinDev* __restrict
         ord[j + 1] = v;
     }
     const int lc = W.pt_col[l];
-    unsigned long long mask[3] = {0ull, 0ull, 0ull};  // free keyframe columns that observe this landmark (Kf <= 166)
+    // this thread owns the landmark's mask row: bit j of it says free keyframe column j observes the landmark
+    unsigned long long* __restrict__ mask = W.lm_mask + (size_t)l * W.mask_words;
+    for (int w2 = 0; w2 < W.mask_words; ++w2) mask[w2] = 0ull;
     for (int s = a; s < b; ++s) {
         const int e = ord[s];
         EdgeS d;
@@ -384,7 +386,6 @@ __global__ void __launch_bounds__(128) plan_sort_kernel(const WinDev* __restrict
             if (lc >= 0) mask[d.pcol >> 6] |= 1ull << (d.pcol & 63);
         }
     }
-    for (int w2 = 0; w2 < W.mask_words; ++w2) W.lm_mask[(size_t)l * W.mask_words + w2] = mask[w2];
 }
 // P5: one CTA per free keyframe lists its edges in ascending sorted-edge order (= landmark order) by an ordered compaction
 //     over the window's edges

@@ -37,7 +37,8 @@ def case_orb():
 
 def case_match():
     total = 0
-    for n1, n2, seed in [(300, 280, 1), (129, 517, 2), (1, 1, 3)]:
+    # (15000, 64): resolve state in shared memory, descriptors from L2; (26000, 64): state in global scratch (Matcher::run)
+    for n1, n2, seed in [(300, 280, 1), (129, 517, 2), (15000, 64, 4), (26000, 64, 5), (1, 1, 3)]:
         d1, a1, d2, a2, v2 = synth.make_descriptor_pair(n1, n2, seed=seed)
         m = match.robust(0.8, True)
         got = m.brute_force_match(d1, a1, d2, a2, v2)

@@ -63,6 +63,39 @@ def test_large_map_off_chip_cholesky(K, L, seed):
         optimize.local_bundle_adjuster().optimize(pr)
 
 
+def _free_columns(pr):
+    """The reduced system's keyframe column of every edge (-1: fixed keyframe), numbered as the host plan numbers them."""
+    fixed = pr["pose_fixed"].astype(bool)
+    col = np.where(fixed, -1, np.cumsum(~fixed) - 1)
+    return col[pr["e_pose"]]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("Kf", [64, 65, 128, 129, 166, 167, 192, 193, 257])
+def test_free_keyframe_count_thresholds(Kf, monkeypatch):
+    # The plan keeps one 64-bit mask word per 64 free keyframe columns for every landmark (lba_kernels.cu:2153: mask_words =
+    # ceil(Kf / 64)); these counts sit on both sides of each word boundary.  6 * Kf <= kCholOnChipMax (1000, :1350) is factored on
+    # chip, above that panel by panel (:2340: `large = max_n > kCholOnChipMax`): 166 and 167 straddle that switch.
+    from stella_vslam_b200 import optimize
+    pr = synth.make_ba_problem(Kf + 1, 1, 3000, seed=100 + Kf, model="stereo")
+    assert (pr["pose_fixed"] == 0).sum() == Kf
+    col = _free_columns(pr)
+    for b in range(64, Kf, 64):                                 # a landmark seen on both sides of every word boundary
+        lo = np.zeros(len(pr["points"]), bool)
+        hi = np.zeros(len(pr["points"]), bool)
+        lo[pr["e_point"][(col >= 0) & (col < b)]] = True
+        hi[pr["e_point"][col >= b]] = True
+        assert (lo & hi).sum() > 10, (b, (lo & hi).sum())
+    got = optimize.global_bundle_adjuster(4).optimize(pr)
+    _check(got, O.global_ba_solve(pr, 4), pr)
+    if 6 * Kf > 1000:
+        assert got["launches"] > 2 * (6 * Kf // 24)             # the panel-by-panel path ran
+    else:                                                       # the on-chip path ran: forcing the panels adds their launches
+        monkeypatch.setenv("B200_LBA_FORCE_OFFCHIP", "1")
+        off = optimize.global_bundle_adjuster(4).optimize(pr)
+        assert off["iterations"] == got["iterations"] and off["launches"] > got["launches"]
+
+
 @pytest.mark.gpu
 def test_force_stop_protocol():
     from stella_vslam_b200 import optimize

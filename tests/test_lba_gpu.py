@@ -177,6 +177,26 @@ def test_many_fixed_keyframes(mods):
         ba.optimize(big)
 
 
+def test_on_chip_limit_alone_and_in_a_batch(mods):
+    # 166 free keyframes is the largest window the on-chip Cholesky takes (6 * Kf <= kCholOnChipMax = 1000, lba_kernels.cu): n = 996,
+    # the largest dynamic shared-memory plan.  Alone it runs in a cluster of 8 CTAs, in a batch of three windows in clusters of 4
+    # (lba_kernels.cu: `nw <= 2 ? 8 : 4`); 167 free keyframes is refused.
+    O, optimize, synth = mods
+    pr = synth.make_ba_problem(176, 10, 3000, seed=51, model="stereo")
+    assert (pr["pose_fixed"] == 0).sum() == 166
+    ba = optimize.local_bundle_adjuster()
+    one = ba.optimize(pr)
+    check_same(one, O.lba_solve(pr), pr)
+    small = [synth.make_ba_problem(12, 3, 600, seed=52, model="mono"), synth.make_ba_problem(8, 2, 300, seed=53, model="stereo")]
+    got = ba.optimize_batch([small[0], pr, small[1]])
+    assert np.array_equal(got[1]["pose_cw"], one["pose_cw"]) and np.array_equal(got[1]["points"], one["points"])
+    assert np.array_equal(got[1]["outliers"], one["outliers"]) and got[1]["iterations"] == one["iterations"]
+    for g, p in zip((got[0], got[2]), small):
+        check_same(g, O.lba_solve(p), p)
+    with pytest.raises(RuntimeError):
+        ba.optimize(synth.make_ba_problem(177, 10, 400, seed=54, model="stereo"))
+
+
 def test_batch_force_stop_flags_and_bad_edges(mods):
     O, optimize, synth = mods
     prs = [synth.make_ba_problem(8, 3, 200, seed=2, model="mono"), synth.make_ba_problem(6, 2, 100, seed=3, model="stereo"),

@@ -36,7 +36,11 @@ def test_hamming_matrix_vs_oracle(mods):
 
 
 @pytest.mark.parametrize("n1,n2,lowe,ori,seed", [(2000, 2000, 0.8, True, 7), (2000, 2000, 0.95, False, 8), (500, 1300, 0.7, True, 9),
-                                                 (1, 1, 0.8, True, 10), (37, 5, 0.6, False, 11), (3000, 2500, 0.75, True, 12)])
+                                                 (1, 1, 0.8, True, 10), (37, 5, 0.6, False, 11), (3000, 2500, 0.75, True, 12),
+                                                 # both sides of resolve_kernel's two placement switches (4641 | 4642, 25206 | 25207,
+                                                 # test_size_paths_gpu.bf_resolve_mode) and the 3840x1920 golden frame's 15 168
+                                                 (4641, 4641, 0.8, True, 13), (4642, 4642, 0.8, True, 14), (15168, 15168, 0.8, True, 15),
+                                                 (25206, 25206, 0.8, True, 16), (25207, 25207, 0.8, True, 17)])
 def test_brute_force_vs_oracle(mods, n1, n2, lowe, ori, seed):
     O, match, synth = mods
     d1, a1, d2, a2, v2 = synth.make_descriptor_pair(n1, n2, seed=seed)
