@@ -698,6 +698,57 @@ uint32_t b200_mt19937_next(b200_mt19937_t* engine);
 /* max_num_iter minimal sets (out: max_num_iter x 4) from one engine, continuing its state; n_matches >= 4. */
 int b200_pnp_draw_min_sets(b200_mt19937_t* engine, uint32_t n_matches, uint32_t max_num_iter, int32_t* out);
 
+/* ----------------------------------------------------------------------------------------------------------------
+ * Pose-graph optimisation (optimize::graph_optimizer, optimize/graph_optimizer.cc:254-302): the Sim3 essential graph of a loop
+ * closure, g2o's Levenberg-Marquardt with numeric central-difference Jacobians (delta 1e-9) and the terminate action, on the handle's
+ * stream.  The vertices and edges are built by the caller as :45-250 does (stella_vslam_b200.optimize.build_essential_graph restates
+ * it).  The linear solve is an envelope (skyline) Cholesky over 32x32 tiles in a reverse Cuthill-McKee ordering of the free vertices
+ * instead of CSparse: both are exact SPD solves and differ in rounding only (DESIGN.md section 8).
+ * ---------------------------------------------------------------------------------------------------------------- */
+typedef struct b200_sim3 {
+    double q[4];                    /* g2o::Sim3::rotation().coeffs(): x y z w */
+    double t[3];                    /* translation() */
+    double s;                       /* scale() */
+} b200_sim3_t;
+typedef struct b200_pose_graph {
+    int32_t n_vertices, n_edges, fix_scale;   /* fix_scale: shot_vertex::fix_scale_ (stereo / RGBD) */
+    const b200_sim3_t* estimate;    /* n_vertices: Sim3_cw before the optimisation, in the reference's vertex order */
+    const uint8_t* fixed;           /* n_vertices: loop keyframe, current keyframe and spanning root are fixed */
+    const int32_t* e_v1;            /* n_edges, insertion order: vertex 0 (id1) */
+    const int32_t* e_v2;            /* vertex 1 (id2) */
+    const b200_sim3_t* e_meas;      /* Sim3_21 = Sim3_2w * Sim3_w1; information I_7, no robust kernel */
+    int32_t n_points;               /* landmarks to correct (may be 0) */
+    const double* points;           /* n_points x 3: pos_w */
+    const int32_t* point_ref;       /* n_points: vertex index of found_lm_to_ref_keyfrm_id[lm] or lm->get_ref_keyframe() */
+    b200_sim3_t* estimate_out;      /* n_vertices: corrected Sim3_cw (fixed vertices bit-unchanged) */
+    double* pose_cw_out;            /* n_vertices x 16 row-major: [R | t / s] with s rounded to float (:265-268) */
+    double* points_out;             /* n_points x 3 or NULL: corrected_Sim3_wc[ref].map(Sim3_cw[ref].map(pos_w)) (:283-300) */
+} b200_pose_graph_t;
+typedef struct b200_pgo_stats {
+    int32_t iterations;             /* LM iterations run */
+    int32_t trials;                 /* linear solves over all iterations */
+    double chi2_init, chi2_final, lambda_init, lambda_final;
+    int64_t envelope_doubles;       /* size of the envelope factor (32x32 tiles) */
+    int64_t factor_flops;           /* floating-point operations of one envelope factorisation, counted from the structure */
+    int32_t launches;               /* kernel launches of the whole call (graph nodes counted per replay) */
+    float lin_ms, factor_ms, solve_ms, total_ms; /* device time of the linearisations, of envelope assembly + factorisation and of
+                                                    substitution + trial oplus + chi2, summed over the call; host wall time of the call */
+} b200_pgo_stats_t;
+/* Bound on the envelope, in doubles (2 GiB).  A chain-like essential graph (spanning tree plus covisibilities of neighbouring
+ * keyframes) needs roughly 2 000 doubles per keyframe and fits up to about 100 000 keyframes; a map that revisits its ground once
+ * needs about twice that.  Measured sizes are in DESIGN.md section 8. */
+#define B200_PGO_MAX_ENVELOPE_DOUBLES ((int64_t)1 << 28)
+/* graph_optimizer::optimize steps 4-5: optimize(max_iter) (50 in the reference) with terminate_action(gain_threshold) (1e-3), then
+ * the write-back of the poses and the landmark correction.  The caller still runs update_mean_normal_and_obs_scale_variance().
+ * B200_ERR_INVALID (nothing written): a null required pointer, a negative count, an edge with an endpoint out of range or v1 == v2, a
+ * point_ref out of range, a non-finite value, a scale <= 0 or a quaternion whose norm is not within [0.5, 2] in an estimate or a
+ * measurement, a non-finite point, no free vertex.
+ * B200_ERR_CAPACITY (nothing written, nothing allocated): the envelope exceeds B200_PGO_MAX_ENVELOPE_DOUBLES (checked on the host). */
+int b200_graph_optimize(b200_lba_t h, const b200_pose_graph_t* g, int max_iter, double gain_threshold, b200_pgo_stats_t* stats);
+/* Host only: the reverse Cuthill-McKee order of the free vertices (order_out: n_free vertex indices, position 0 first; may be NULL),
+ * the number of free vertices and the envelope b200_graph_optimize would factor.  Same validation as b200_graph_optimize. */
+int b200_pgo_envelope(const b200_pose_graph_t* g, int32_t* n_free, int32_t* order_out, int64_t* envelope_doubles);
+
 /* Profiling mode: an event after every launch of the following solves (adds a few microseconds per launch; off by default).
  * b200_lba_kernel_ms reports, for the LAST batch, the summed device time and the number of intervals of
  *   kernel 0 plan (5 launches, one interval), 1 landmark pass / build, 2 keyframe rows, 3 Schur rows, 4 reduced-system Cholesky,

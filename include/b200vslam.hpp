@@ -409,6 +409,46 @@ private:
     b200_lba_t h_ = nullptr;
 };
 
+class graph_optimizer {  // optimize/graph_optimizer.h:20-45: steps 4-5 on a graph built as graph_optimizer.cc:43-250 builds it
+public:
+    explicit graph_optimizer(bool fix_scale, unsigned int min_num_shared_lms = 100, int device = 0)
+        : fix_scale_(fix_scale), min_num_shared_lms_(min_num_shared_lms) {
+        check(b200_lba_create(device, &h_), "b200_lba_create");
+    }
+    ~graph_optimizer() { b200_lba_destroy(h_); }
+    graph_optimizer(const graph_optimizer&) = delete;
+    // estimate / fixed per vertex, e_v1 / e_v2 / e_meas per edge, landmarks (points, point_ref) to correct; fills the outputs
+    void optimize(const std::vector<b200_sim3_t>& estimate, const std::vector<uint8_t>& fixed, const std::vector<int32_t>& e_v1,
+                  const std::vector<int32_t>& e_v2, const std::vector<b200_sim3_t>& e_meas, const std::vector<double>& points,
+                  const std::vector<int32_t>& point_ref, std::vector<b200_sim3_t>& estimate_out, std::vector<double>& pose_cw_out,
+                  std::vector<double>& points_out, b200_pgo_stats_t* stats = nullptr, int max_iter = 50, double gain_threshold = 1e-3) const {
+        estimate_out.resize(estimate.size());
+        pose_cw_out.resize(16 * estimate.size());
+        points_out.resize(points.size());
+        b200_pose_graph_t g{};
+        g.n_vertices = (int32_t)estimate.size();
+        g.n_edges = (int32_t)e_v1.size();
+        g.fix_scale = fix_scale_ ? 1 : 0;
+        g.estimate = estimate.data();
+        g.fixed = fixed.data();
+        g.e_v1 = e_v1.data();
+        g.e_v2 = e_v2.data();
+        g.e_meas = e_meas.data();
+        g.n_points = (int32_t)point_ref.size();
+        g.points = points.data();
+        g.point_ref = point_ref.data();
+        g.estimate_out = estimate_out.data();
+        g.pose_cw_out = pose_cw_out.data();
+        g.points_out = points_out.empty() ? nullptr : points_out.data();
+        check(b200_graph_optimize(h_, &g, max_iter, gain_threshold, stats), "b200_graph_optimize");
+    }
+    const bool fix_scale_;
+    const unsigned int min_num_shared_lms_;
+
+private:
+    b200_lba_t h_ = nullptr;
+};
+
 }  // namespace optimize
 
 namespace tracking {

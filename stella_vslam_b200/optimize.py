@@ -6,6 +6,7 @@ edges (steps 1-4) and writes the result back under the map mutex (step 8); both 
 flattened problem (the layout of b200_lba_problem_t) and runs steps 5-7 on the GPU.
 """
 import ctypes as C
+import math
 
 import numpy as np
 
@@ -40,6 +41,8 @@ def _bind():
     L.b200_lba_last_profile.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.b200_pose_optimize.argtypes = [vp, C.c_int, C.POINTER(LbaProblem), C.c_int, C.c_int, C.c_int, vp, vp, vp]
     L.b200_global_ba_solve.argtypes = [vp, C.POINTER(LbaProblem), C.c_int, C.c_double, vp, vp, vp, C.POINTER(LbaStats)]
+    L.b200_graph_optimize.argtypes = [vp, C.POINTER(PoseGraph), C.c_int, C.c_double, C.POINTER(PgoStats)]
+    L.b200_pgo_envelope.argtypes = [C.POINTER(PoseGraph), C.POINTER(C.c_int32), vp, C.POINTER(C.c_int64)]
     return L
 
 
@@ -260,3 +263,254 @@ def create(yaml_node=None, device=0):
     if backend != "b200":
         raise RuntimeError(f"Invalid backend: {backend}")
     return local_bundle_adjuster(node.get("num_first_iter", 5), node.get("num_second_iter", 10), device)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# optimize::graph_optimizer (optimize/graph_optimizer.{h,cc}): the Sim3 pose-graph optimisation of a loop closure
+# ---------------------------------------------------------------------------------------------------------------------------------
+class Sim3(C.Structure):
+    """b200_sim3_t: g2o::Sim3 as rotation().coeffs() (x y z w), translation(), scale()."""
+    _fields_ = [("q", C.c_double * 4), ("t", C.c_double * 3), ("s", C.c_double)]
+
+
+class PoseGraph(C.Structure):
+    """b200_pose_graph_t (include/b200vslam.h)."""
+    _fields_ = [("n_vertices", C.c_int32), ("n_edges", C.c_int32), ("fix_scale", C.c_int32), ("estimate", C.c_void_p), ("fixed", C.c_void_p),
+                ("e_v1", C.c_void_p), ("e_v2", C.c_void_p), ("e_meas", C.c_void_p), ("n_points", C.c_int32), ("points", C.c_void_p),
+                ("point_ref", C.c_void_p), ("estimate_out", C.c_void_p), ("pose_cw_out", C.c_void_p), ("points_out", C.c_void_p)]
+
+
+class PgoStats(C.Structure):
+    """b200_pgo_stats_t (include/b200vslam.h)."""
+    _fields_ = [("iterations", C.c_int32), ("trials", C.c_int32), ("chi2_init", C.c_double), ("chi2_final", C.c_double),
+                ("lambda_init", C.c_double), ("lambda_final", C.c_double), ("envelope_doubles", C.c_int64), ("factor_flops", C.c_int64),
+                ("launches", C.c_int32), ("lin_ms", C.c_float), ("factor_ms", C.c_float), ("solve_ms", C.c_float), ("total_ms", C.c_float)]
+
+
+PGO_MAX_ENVELOPE_DOUBLES = 1 << 28   # B200_PGO_MAX_ENVELOPE_DOUBLES
+
+
+# g2o::Sim3 on the host, as 8-vectors (q x y z w, t, s), in the evaluation order of csrc/sim3.cuh: what build_essential_graph needs
+def _quat_rotate(q, v):
+    uv = [q[1] * v[2] - q[2] * v[1], q[2] * v[0] - q[0] * v[2], q[0] * v[1] - q[1] * v[0]]
+    uv = [u + u for u in uv]
+    c = [q[1] * uv[2] - q[2] * uv[1], q[2] * uv[0] - q[0] * uv[2], q[0] * uv[1] - q[1] * uv[0]]
+    return [v[i] + q[3] * uv[i] + c[i] for i in range(3)]
+
+
+def _quat_normalize(q):
+    if q[3] < 0:
+        q = [-x for x in q]
+    n = math.sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3])
+    return [x / n for x in q]
+
+
+def sim3_from_rts(R, t, s=1.0):
+    """g2o::Sim3(const Matrix3& R, const Vector3& t, double s): Quaternion(R), normalised."""
+    R = [float(x) for x in np.asarray(R, np.float64).reshape(9)]
+    tr = R[0] + R[4] + R[8]
+    if tr > 0:
+        tr = math.sqrt(tr + 1.0)
+        w = 0.5 * tr
+        tr = 0.5 / tr
+        q = [(R[7] - R[5]) * tr, (R[2] - R[6]) * tr, (R[3] - R[1]) * tr, w]
+    else:
+        i = 0
+        if R[4] > R[0]:
+            i = 1
+        if R[8] > R[i * 3 + i]:
+            i = 2
+        j, k = (i + 1) % 3, (i + 2) % 3
+        tr = math.sqrt(R[i * 3 + i] - R[j * 3 + j] - R[k * 3 + k] + 1.0)
+        q = [0.0] * 4
+        q[i] = 0.5 * tr
+        tr = 0.5 / tr
+        q[3] = (R[k * 3 + j] - R[j * 3 + k]) * tr
+        q[j] = (R[j * 3 + i] + R[i * 3 + j]) * tr
+        q[k] = (R[k * 3 + i] + R[i * 3 + k]) * tr
+    t = [float(x) for x in np.asarray(t, np.float64).reshape(3)]
+    return np.array(_quat_normalize(q) + t + [float(s)])
+
+
+def sim3_mul(a, b):
+    """g2o::Sim3::operator*."""
+    a, b = [float(x) for x in a], [float(x) for x in b]
+    q = [a[3] * b[0] + a[0] * b[3] + a[1] * b[2] - a[2] * b[1],
+         a[3] * b[1] + a[1] * b[3] + a[2] * b[0] - a[0] * b[2],
+         a[3] * b[2] + a[2] * b[3] + a[0] * b[1] - a[1] * b[0],
+         a[3] * b[3] - a[0] * b[0] - a[1] * b[1] - a[2] * b[2]]
+    rt = _quat_rotate(a[:4], b[4:7])
+    return np.array(q + [a[7] * rt[i] + a[4 + i] for i in range(3)] + [a[7] * b[7]])
+
+
+def sim3_inverse(a):
+    """g2o::Sim3::inverse() (its constructor normalises the rotation)."""
+    a = [float(x) for x in a]
+    qc = [-a[0], -a[1], -a[2], a[3]]
+    f = -1. / a[7]
+    t = _quat_rotate(qc, [f * a[4], f * a[5], f * a[6]])
+    return np.array(_quat_normalize(qc) + t + [1. / a[7]])
+
+
+def build_essential_graph(keyframes, curr_id, loop_id, loop_connections, non_corrected_Sim3s=None, pre_corrected_Sim3s=None,
+                          min_num_shared_lms=100, fix_scale=False, landmarks=None, found_lm_to_ref_keyfrm_id=None):
+    """graph_optimizer::optimize steps 1-3 (graph_optimizer.cc:43-250) from a flat description of the map.
+
+    keyframes: curr_keyfrm->graph_node_->get_keyframes_from_root() in order, each a dict with
+        id, rot_cw (3x3), trans_cw (3), erased (will_be_erased), parent (spanning parent id or None for the root), children (spanning
+        children ids), loop_edges (ids), covisibilities ([(id, num_shared_lms)] in the order of ordered_covisibilities_: descending).
+    loop_connections: [(id1, [id2, ...])] in the order of the caller's std::map.
+    non_corrected_Sim3s / pre_corrected_Sim3s: {id: Sim3 8-vector}.
+    landmarks: optional [(lm_id, pos_w (3), ref_keyfrm_id)] of the non-erased landmarks in all_lms order; found_lm_to_ref_keyfrm_id:
+        {lm_id: keyframe id}.
+    Returns the graph dict of graph_optimizer.optimize (plus vertex_ids, the keyframe id of every vertex)."""
+    non_corrected_Sim3s = non_corrected_Sim3s or {}
+    pre_corrected_Sim3s = pre_corrected_Sim3s or {}
+    found = found_lm_to_ref_keyfrm_id or {}
+    kf_by_id = {k["id"]: k for k in keyframes}
+    Sim3s_cw, vidx, est, fixed, vertex_ids = {}, {}, [], [], []
+    for k in keyframes:                                              # 2. vertices (:70-106)
+        if k.get("erased", False):
+            continue
+        kid = k["id"]
+        if kid in pre_corrected_Sim3s:
+            s = np.asarray(pre_corrected_Sim3s[kid], np.float64)
+        else:
+            s = sim3_from_rts(k["rot_cw"], k["trans_cw"], 1.0)
+        Sim3s_cw[kid] = s
+        vidx[kid] = len(est)
+        est.append(s)
+        fixed.append(kid == loop_id or kid == curr_id or k.get("parent") is None)
+        vertex_ids.append(kid)
+    e_v1, e_v2, meas = [], [], []
+    inserted = set()
+
+    def insert_edge(id1, id2, S21):
+        e_v1.append(vidx[id1])
+        e_v2.append(vidx[id2])
+        meas.append(S21)
+        inserted.add((min(id1, id2), max(id1, id2)))
+
+    def shared(k, other):
+        return dict(k.get("covisibilities", ())).get(other, 0)
+
+    for id1, connected in loop_connections:                          # loop edges over the threshold (:130-160)
+        S_w1 = sim3_inverse(Sim3s_cw[id1])
+        for id2 in connected:
+            if not (id1 == curr_id and id2 == loop_id) and shared(kf_by_id[id1], id2) < min_num_shared_lms:
+                continue
+            insert_edge(id1, id2, sim3_mul(Sim3s_cw[id2], S_w1))
+
+    def sim3_2w(id2):
+        return np.asarray(non_corrected_Sim3s[id2], np.float64) if id2 in non_corrected_Sim3s else Sim3s_cw[id2]
+
+    for k in keyframes:                                              # non-loop edges (:162-250)
+        if k.get("erased", False):                                   # no vertex: the reference's Sim3s_cw.at(id1) would throw
+            continue
+        id1 = k["id"]
+        S_w1 = sim3_inverse(np.asarray(non_corrected_Sim3s[id1], np.float64) if id1 in non_corrected_Sim3s else Sim3s_cw[id1])
+        parent = k.get("parent")
+        if parent is not None:
+            if id1 <= parent:                                        # :166-172 skips the rest of this keyframe, not only the edge
+                continue
+            insert_edge(id1, parent, sim3_mul(sim3_2w(parent), S_w1))
+        loop_edges = set(k.get("loop_edges", ()))
+        for id2 in k.get("loop_edges", ()):
+            if id1 > id2:
+                insert_edge(id1, id2, sim3_mul(sim3_2w(id2), S_w1))
+        children = set(k.get("children", ()))
+        for id2, w in k.get("covisibilities", ()):
+            if w < min_num_shared_lms or parent is None:
+                continue
+            if id2 == parent or id2 in children or id2 in loop_edges:
+                continue
+            if kf_by_id[id2].get("erased", False):
+                continue
+            if id1 <= id2 or (min(id1, id2), max(id1, id2)) in inserted:
+                continue
+            insert_edge(id1, id2, sim3_mul(sim3_2w(id2), S_w1))
+    graph = dict(estimate=np.array(est).reshape(-1, 8), fixed=np.array(fixed, np.uint8), e_v1=np.array(e_v1, np.int32),
+                 e_v2=np.array(e_v2, np.int32), e_meas=np.array(meas).reshape(-1, 8), fix_scale=bool(fix_scale), vertex_ids=vertex_ids,
+                 points=np.zeros((0, 3)), point_ref=np.zeros(0, np.int32))
+    if landmarks:                                                    # 5. landmark references (:283-300)
+        graph["points"] = np.array([lm[1] for lm in landmarks], np.float64).reshape(-1, 3)
+        graph["point_ref"] = np.array([vidx[found.get(lm[0], lm[2])] for lm in landmarks], np.int32)
+    return graph
+
+
+def pack_pose_graph(graph):
+    """graph dict -> (PoseGraph with output buffers, keep-alive dict holding estimate_out / pose_cw_out / points_out)."""
+    keep = {}
+
+    def arr(name, x, dt, shape=None):
+        a = np.ascontiguousarray(x, dt)
+        if shape is not None:
+            a = a.reshape(shape)
+        keep[name] = a
+        return a.ctypes.data
+
+    nv, ne = len(graph["estimate"]), len(graph["e_v1"])
+    pts = np.asarray(graph.get("points", np.zeros((0, 3))), np.float64).reshape(-1, 3)
+    G = PoseGraph()
+    G.n_vertices, G.n_edges, G.fix_scale = nv, ne, int(bool(graph.get("fix_scale", False)))
+    G.estimate = arr("estimate", graph["estimate"], np.float64, (-1, 8))
+    G.fixed = arr("fixed", graph["fixed"], np.uint8)
+    G.e_v1 = arr("e_v1", graph["e_v1"], np.int32)
+    G.e_v2 = arr("e_v2", graph["e_v2"], np.int32)
+    G.e_meas = arr("e_meas", np.asarray(graph["e_meas"], np.float64).reshape(-1, 8), np.float64)
+    G.n_points = len(pts)
+    G.points = arr("points", pts, np.float64)
+    G.point_ref = arr("point_ref", graph.get("point_ref", np.zeros(0)), np.int32)
+    keep["estimate_out"], keep["pose_cw_out"], keep["points_out"] = np.zeros((nv, 8)), np.zeros((nv, 4, 4)), np.zeros((len(pts), 3))
+    G.estimate_out, G.pose_cw_out = keep["estimate_out"].ctypes.data, keep["pose_cw_out"].ctypes.data
+    G.points_out = keep["points_out"].ctypes.data if len(pts) else None
+    return G, keep
+
+
+def pgo_envelope(graph):
+    """b200_pgo_envelope (host only): (reverse Cuthill-McKee order of the free vertices, envelope doubles)."""
+    L = _bind()
+    G, keep = pack_pose_graph(graph)
+    nf, env = C.c_int32(), C.c_int64()
+    order = np.zeros(max(len(graph["estimate"]), 1), np.int32)
+    check(L.b200_pgo_envelope(C.byref(G), C.byref(nf), ptr(order), C.byref(env)))
+    return order[:nf.value].copy(), env.value
+
+
+class graph_optimizer:
+    """optimize::graph_optimizer (optimize/graph_optimizer.h:20-45): the loop closure's Sim3 essential-graph optimisation on the GPU.
+    build_essential_graph() restates how the reference builds the vertices and edges; optimize() runs steps 4-5."""
+
+    def __init__(self, min_num_shared_lms=100, fix_scale=False, device=0, max_iter=50, gain_threshold=1e-3):
+        self.min_num_shared_lms_, self.fix_scale_ = int(min_num_shared_lms), bool(fix_scale)   # GraphOptimizer.min_num_shared_lms
+        self.max_iter_, self.gain_threshold_ = int(max_iter), float(gain_threshold)
+        self._L = _bind()
+        self._h = C.c_void_p()
+        check(self._L.b200_lba_create(device, C.byref(self._h)))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.b200_lba_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def build_essential_graph(self, keyframes, curr_id, loop_id, loop_connections, non_corrected_Sim3s=None, pre_corrected_Sim3s=None,
+                              landmarks=None, found_lm_to_ref_keyfrm_id=None):
+        return build_essential_graph(keyframes, curr_id, loop_id, loop_connections, non_corrected_Sim3s, pre_corrected_Sim3s,
+                                     self.min_num_shared_lms_, self.fix_scale_, landmarks, found_lm_to_ref_keyfrm_id)
+
+    def optimize(self, graph):
+        """graph: dict(estimate (n,8), fixed (n,), e_v1, e_v2, e_meas (m,8), fix_scale, points (k,3), point_ref (k,)).
+        Returns dict(estimate, pose_cw (n,4,4), points (k,3), iterations, trials, chi2_init, chi2_final, lambda_init, lambda_final,
+        envelope_doubles, factor_flops, launches, lin_ms, factor_ms, solve_ms, total_ms)."""
+        G, keep = pack_pose_graph(graph)
+        st = PgoStats()
+        check(self._L.b200_graph_optimize(self._h, C.byref(G), self.max_iter_, self.gain_threshold_, C.byref(st)))
+        out = dict(estimate=keep["estimate_out"], pose_cw=keep["pose_cw_out"], points=keep["points_out"])
+        out.update({name: getattr(st, name) for name, _ in PgoStats._fields_})
+        return out

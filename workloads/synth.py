@@ -748,3 +748,92 @@ def make_pnp_problem(seed=0, n=300, inlier_frac=0.5, model="perspective", case=N
         o[~far] = turned[~far]
         bear[out] = o
     return dict(bearings=bear, points=pw, octaves=octaves, scale_factors=sf, gt_rot_cw=Rcw, gt_trans_cw=tcw, gt_inlier=inl)
+
+
+def make_pose_graph(n_keyframes=500, seed=0, fix_scale=False, laps=1.5, window=8, rot_noise=2e-3, trans_noise=0.01, scale_noise=2e-3,
+                    lm_per_keyframe=4, min_num_shared_lms=100, return_description=False):
+    """A loop-closure pose graph for optimize.graph_optimizer, built by optimize.build_essential_graph.
+
+    The camera drives `laps` times around a circle of keyframes (laps > 1 revisits the ground of the first lap), facing along the
+    track.  The keyframe poses are dead reckoning from noisy relative motions (rotation, translation and, unless fix_scale, scale drift
+    as a monocular map drifts).  Covisibility weights (shared landmarks) come from the overlap of the true views: keyframes within about
+    `window` steps, and the keyframes of other laps at the same place.  The spanning tree is the chain of keyframes (the root is keyframe
+    0).  The last keyframe closes a loop with the first-lap keyframe at its place; its neighbours are pre-corrected through it as
+    correct_loop does, and the loop connections join them to the loop keyframe's neighbours.  Landmarks: `lm_per_keyframe` per keyframe,
+    in front of their reference keyframe; every third landmark of the current keyframe's neighbourhood is re-referenced to the loop
+    keyframe (found_lm_to_ref_keyfrm_id).  Returns the graph dict (and the flat description with return_description)."""
+    from stella_vslam_b200.optimize import build_essential_graph, sim3_from_rts, sim3_inverse, sim3_mul
+
+    rng = np.random.default_rng(seed)
+    n = int(n_keyframes)
+    per_lap = max(8, int(round(n / laps)))
+    radius = per_lap * 1.0 / (2 * np.pi)                      # 1 m between keyframes
+    ang = 2 * np.pi * np.arange(n) / per_lap
+    # true camera: at (r cos a, 0, r sin a), optical axis (z) along the track
+    R_true, t_true = [], []
+    for a in ang:
+        Rwc = _rot_y(-a)                                       # camera z axis rotates with the heading
+        c = np.array([radius * np.cos(a), 0.0, radius * np.sin(a)])
+        R_true.append(Rwc.T)
+        t_true.append(-Rwc.T @ c)
+    R_true, t_true = np.array(R_true), np.array(t_true)
+    # dead reckoning with drift
+    R_est, t_est, sc = [R_true[0]], [t_true[0]], 1.0
+    for i in range(1, n):
+        R_rel = R_true[i] @ R_true[i - 1].T
+        t_rel = t_true[i] - R_rel @ t_true[i - 1]
+        if not fix_scale:
+            sc *= 1.0 + scale_noise * rng.standard_normal()
+        R_rel = _rodrigues(rot_noise * rng.standard_normal(3)) @ R_rel
+        t_rel = sc * t_rel + trans_noise * rng.standard_normal(3)
+        R_est.append(R_rel @ R_est[-1])
+        t_est.append(R_rel @ t_est[-1] + t_rel)
+    # covisibility weights from the overlap of the true views
+    pos = np.stack([radius * np.cos(ang), np.zeros(n), radius * np.sin(ang)], 1)
+    weights = []
+    for i in range(n):
+        d = np.linalg.norm(pos - pos[i], axis=1)
+        dh = np.abs((ang - ang[i] + np.pi) % (2 * np.pi) - np.pi)
+        w = (400 * np.clip(1 - d / (window * 1.25), 0, 1) * np.clip(np.cos(dh), 0, 1)).astype(int)
+        w[i] = 0
+        nz = np.nonzero(w > 0)[0]
+        order = nz[np.argsort(-w[nz], kind="stable")]
+        weights.append([(int(j), int(w[j])) for j in order])
+    curr, loop = n - 1, int((n - 1) % per_lap)
+    if loop >= curr - window:
+        loop = 0
+    kfs = []
+    for i in range(n):
+        kfs.append(dict(id=i, rot_cw=R_est[i], trans_cw=t_est[i], erased=False, parent=(i - 1 if i else None), children=([i + 1] if i + 1 < n else []),
+                        loop_edges=[], covisibilities=weights[i]))
+    # correct_loop: the current keyframe's Sim3 from the loop keyframe, its neighbours pre-corrected through it
+    E = {i: sim3_from_rts(R_est[i], t_est[i], 1.0) for i in range(n)}
+    R_cl = R_true[curr] @ R_true[loop].T
+    t_cl = t_true[curr] - R_cl @ t_true[loop]
+    corr_c = sim3_mul(sim3_from_rts(R_cl, t_cl, 1.0), E[loop])
+    if not fix_scale:
+        corr_c[7] = 1.0 / sc                                   # undo the scale the dead reckoning drifted by
+    neigh = [curr] + [j for j, w in weights[curr] if w >= min_num_shared_lms and j > loop + window][:window]
+    non_corrected = {j: E[j] for j in neigh}
+    pre_corrected = {j: (corr_c if j == curr else sim3_mul(sim3_mul(E[j], sim3_inverse(E[curr])), corr_c)) for j in neigh}
+    loop_side = [loop] + [j for j, w in weights[loop] if w >= min_num_shared_lms and j < loop + window][:window]
+    loop_connections = []
+    for j in neigh:
+        conn = [k for k in loop_side if dict(weights[j]).get(k, 0) >= min_num_shared_lms or (j == curr and k == loop)]
+        if conn:
+            loop_connections.append((j, conn))
+    # landmarks in front of their reference keyframe, in the drifted map
+    landmarks, found, lid = [], {}, 0
+    for i in range(n):
+        for _ in range(lm_per_keyframe):
+            pc = np.array([rng.uniform(-3, 3), rng.uniform(-2, 2), rng.uniform(2, 10)])
+            pw = R_est[i].T @ (pc - t_est[i])
+            landmarks.append((lid, pw, i))
+            if i in pre_corrected and lid % 3 == 0:
+                found[lid] = loop
+            lid += 1
+    desc = dict(keyframes=kfs, curr_id=curr, loop_id=loop, loop_connections=loop_connections, non_corrected_Sim3s=non_corrected,
+                pre_corrected_Sim3s=pre_corrected, min_num_shared_lms=min_num_shared_lms, fix_scale=fix_scale, landmarks=landmarks,
+                found_lm_to_ref_keyfrm_id=found)
+    graph = build_essential_graph(**desc)
+    return (graph, desc) if return_description else graph
