@@ -147,10 +147,13 @@ __device__ __forceinline__ double block_sum(double v, double* sh) {  // determin
 }
 
 
-// The 6x3 block Hpl of an edge is a 160-byte record (18 doubles + 2 of padding), 32-byte aligned: a thread that reads a whole record
-// does it in whole 32-byte sectors, each as a pair of 128-bit accesses (Hopper has no 256-bit load; with 144-byte records half of
-// every sector fetched from L2 was wasted, and the Schur kernel runs at the L2 bandwidth).
-constexpr int kHplStride = 20;
+// Factored Hpl record.  All three edge models factor their Jacobians through the camera-frame point pc = R P + t:
+//     Jj = Jpi [-[pc]x | I]  (rotation columns first),   Ji = Jpi R,
+// so with A = ww Jpi^T Ji (3x3; rows 3..5 of Hpl)  the 6x3 block is  Hpl = ww Jj^T Ji = [ [pc]x A ; A ].
+// A record holds A (row-major, 9 doubles) and pc (3): 96 bytes = three whole 32-byte sectors, read and written as pairs of 128-bit
+// accesses (Hopper has no 256-bit access).  The Schur kernel, which runs at the L2 bandwidth, gathers 40 % fewer bytes than with the
+// 18 entries padded to 160 bytes.  An edge that contributes no Hpl (inactive, fixed landmark or fixed keyframe) has an all-zero record.
+constexpr int kHplStride = 12;
 __device__ __forceinline__ void ld256(const double* p, double& a, double& b, double& c, double& d) {
     const double2 lo = reinterpret_cast<const double2*>(p)[0], hi = reinterpret_cast<const double2*>(p)[1];
     a = lo.x, b = lo.y, c = hi.x, d = hi.y;
@@ -159,11 +162,24 @@ __device__ __forceinline__ void st256(double* p, double a, double b, double c, d
     reinterpret_cast<double2*>(p)[0] = make_double2(a, b);
     reinterpret_cast<double2*>(p)[1] = make_double2(c, d);
 }
-__device__ __forceinline__ void load18(const double* __restrict__ p, double* out) {
-    double pad0, pad1;
+// out = {A (9), pc (3)}
+__device__ __forceinline__ void load_hpl_record(const double* __restrict__ p, double* out) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) ld256(p + 4 * i, out[4 * i], out[4 * i + 1], out[4 * i + 2], out[4 * i + 3]);
-    ld256(p + 16, out[16], out[17], pad0, pad1);
+    for (int i = 0; i < 3; ++i) ld256(p + 4 * i, out[4 * i], out[4 * i + 1], out[4 * i + 2], out[4 * i + 3]);
+}
+// the 6x3 block (row-major) from a record: rows 0..2 = [pc]x A, rows 3..5 = A
+__device__ __forceinline__ void expand_hpl(const double* r, double* h) {
+    const double* A = r;
+    const double x = r[9], y = r[10], z = r[11];
+#pragma unroll
+    for (int b = 0; b < 3; ++b) {
+        h[b] = y * A[6 + b] - z * A[3 + b];
+        h[3 + b] = z * A[b] - x * A[6 + b];
+        h[6 + b] = x * A[3 + b] - y * A[b];
+        h[9 + b] = A[b];
+        h[12 + b] = A[3 + b];
+        h[15 + b] = A[6 + b];
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -698,7 +714,7 @@ __global__ void __launch_bounds__(256) lm_round_end_kernel(const WinDev* __restr
 // ---------------------------------------------------------------------------------------------------------------
 // K1: landmark pass.  Eight lanes share a landmark and split its edges; sixteen landmarks per 128-thread CTA.
 //   kBuild : computeActiveErrors + the landmark side of buildSystem at the CURRENT state -- per edge the residual, chi2, Huber
-//            weight, the 6x3 block Hpl (144-byte record) and the landmark's Hll (6 unique) / bl (3), reduced over the
+//            weight, the factored Hpl record (96 bytes: A and pc) and the landmark's Hll (6 unique) / bl (3), reduced over the
 //            landmark's contiguous edge range in a fixed order; chi2 and max |diag| partials per CTA
 //   kTrial : chi2 of the TRIAL state (inactive edges carry the chi2 of their last activation over); the last CTA of the window
 //            runs the accept / reject bookkeeping
@@ -763,22 +779,24 @@ __global__ void __launch_bounds__(kLmThreads, 4) landmark_kernel(const WinDev* _
                     h[7] += -ww * (Ji[1] * err[0] + Ji[4] * err[1] + Ji[7] * err[2]);
                     h[8] += -ww * (Ji[2] * err[0] + Ji[5] * err[1] + Ji[8] * err[2]);
                 }
-                // Hpl = Jj^T W Ji (6x3)
-                double hp[18];
+                // factored Hpl record {A = ww Jpi^T Ji, pc}; the translation columns of Jj are Jpi
+                const bool both = lfree && pfree;
+                double hr[12];
 #pragma unroll
-                for (int a = 0; a < 6; ++a)
+                for (int a = 0; a < 3; ++a)
 #pragma unroll
                     for (int b = 0; b < 3; ++b) {
-                        const double s = ww * (Jj[a] * Ji[b] + Jj[6 + a] * Ji[3 + b] + Jj[12 + a] * Ji[6 + b]);
-                        hp[a * 3 + b] = (lfree && pfree) ? s : 0.0;
+                        const double s = ww * (Jj[3 + a] * Ji[b] + Jj[9 + a] * Ji[3 + b] + Jj[15 + a] * Ji[6 + b]);
+                        hr[a * 3 + b] = both ? s : 0.0;
                     }
 #pragma unroll
-                for (int i = 0; i < 4; ++i) st256(rec + 4 * i, hp[4 * i], hp[4 * i + 1], hp[4 * i + 2], hp[4 * i + 3]);
-                st256(rec + 16, hp[16], hp[17], 0.0, 0.0);
+                for (int i = 0; i < 3; ++i) hr[9 + i] = both ? pc[i] : 0.0;
+#pragma unroll
+                for (int i = 0; i < 3; ++i) st256(rec + 4 * i, hr[4 * i], hr[4 * i + 1], hr[4 * i + 2], hr[4 * i + 3]);
             }
         } else if (MODE == kBuild) {
 #pragma unroll
-            for (int i = 0; i < 5; ++i) st256(rec + 4 * i, 0.0, 0.0, 0.0, 0.0);
+            for (int i = 0; i < 3; ++i) st256(rec + 4 * i, 0.0, 0.0, 0.0, 0.0);
         } else if (MODE == kTrial) {
             chi[e] = chi_carry[e];  // inactive edges keep the chi2 of their last activation across the current/trial swap
         }
@@ -1206,8 +1224,9 @@ __global__ void __launch_bounds__(kCholThreads) chol_solve_kernel(const WinDev* 
 
 // K5 (pair-list chunks, one warp per chunk): a chunk's block partial is formed as a small GEMM on the fp64 tensor cores:
 //        S (6 x 6 | rhs) = [T_1 ... T_P] (6 x 3P) . [H_1 | b_1 ... H_P | b_P]^T (3P x 7),   T_p = Hpl(a_p) Dinv(l_p),  H_p = Hpl(c_p)
-//     Phase 1 (lane = pair, 32 pairs per pass): load the two 160-byte records and Dinv, form T, park T and H (and bl for diagonal
-//     blocks) in the warp's shared-memory operand tiles, r-major with a row stride of 100 doubles (conflict-free fragment loads).
+//     Phase 1 (lane = pair, 32 pairs per pass): load the two 96-byte records and Dinv, expand the records to Hpl, form T, park T and
+//     H (and bl for diagonal blocks) in the warp's shared-memory operand tiles, r-major with a row stride of 100 doubles (conflict-free
+//     fragment loads).
 //     Phase 2: 24 x mma.sync.m8n8k4.f64 (DMMA) per pass, two LDS + one DMMA per lane and step; the 8 x 8 accumulator tile lives in two
 //     registers per lane for the whole chunk, so no per-lane accumulators have to be reduced across the warp.  Summation order is
 //     fixed => deterministic.
@@ -1246,9 +1265,11 @@ __global__ void __launch_bounds__(128) schur_mma_kernel(const WinDev* __restrict
             double t[18], hc[18], b3[3];
             if (k < ch.end) {
                 const int4 pr = W.pairs[k];
-                double ha[18];
-                load18(Hpl + (size_t)pr.x * kHplStride, ha);
-                load18(Hpl + (size_t)pr.y * kHplStride, hc);
+                double ra[12], rc[12], ha[18];
+                load_hpl_record(Hpl + (size_t)pr.x * kHplStride, ra);
+                load_hpl_record(Hpl + (size_t)pr.y * kHplStride, rc);
+                expand_hpl(ra, ha);
+                expand_hpl(rc, hc);
                 const int lc = pr.z;
                 const double D0 = Dinv[lc], D1 = Dinv[(size_t)Lf + lc], D2 = Dinv[(size_t)2 * Lf + lc];
                 const double D4 = Dinv[(size_t)3 * Lf + lc], D5 = Dinv[(size_t)4 * Lf + lc], D8 = Dinv[(size_t)5 * Lf + lc];
@@ -1519,7 +1540,7 @@ __global__ void __launch_bounds__(kGfinThreads) gchol_finish_kernel(const WinDev
 }
 
 // K7: back-substitution x_l = Dinv (bl - sum_e Hpl(e)^T x_p), trial landmark, scale partials.  Eight lanes share a landmark
-//     (they split its edges), sixteen landmarks per 128-thread CTA.
+//     (they split its edges), sixteen landmarks per 128-thread CTA.  Hpl^T x_p is formed from the factored record without expanding it.
 __global__ void __launch_bounds__(128) backsub_kernel(const WinDev* __restrict__ wins) {
     __shared__ double sh[128];
     const WinDev& W = wins[blockIdx.y];
@@ -1547,14 +1568,17 @@ __global__ void __launch_bounds__(128) backsub_kernel(const WinDev* __restrict__
         for (int e = a0 + sub; e < b0; e += 8) {
             const int pcol = v.edges[e].pcol;
             if (pcol < 0) continue;
-            double h[18];
-            load18(Hpl + (size_t)e * kHplStride, h);
+            double r[12];
+            load_hpl_record(Hpl + (size_t)e * kHplStride, r);
+            // Hpl^T [w; v] = A^T (v - [pc]x w) = A^T (v + w x pc)
+            const double* x = xp + 6 * pcol;
+            const double w0 = x[0], w1 = x[1], w2 = x[2];
+            const double u[3] = {x[3] + (w1 * r[11] - w2 * r[10]), x[4] + (w2 * r[9] - w0 * r[11]), x[5] + (w0 * r[10] - w1 * r[9])};
 #pragma unroll
-            for (int r = 0; r < 6; ++r) {
-                const double x = xp[6 * pcol + r];
-                c0 -= h[r * 3] * x;
-                c1 -= h[r * 3 + 1] * x;
-                c2 -= h[r * 3 + 2] * x;
+            for (int k = 0; k < 3; ++k) {
+                c0 -= r[k * 3] * u[k];
+                c1 -= r[k * 3 + 1] * u[k];
+                c2 -= r[k * 3 + 2] * u[k];
             }
         }
     }
