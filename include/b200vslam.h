@@ -749,6 +749,43 @@ int b200_graph_optimize(b200_lba_t h, const b200_pose_graph_t* g, int max_iter, 
  * the number of free vertices and the envelope b200_graph_optimize would factor.  Same validation as b200_graph_optimize. */
 int b200_pgo_envelope(const b200_pose_graph_t* g, int32_t* n_free, int32_t* order_out, int64_t* envelope_doubles);
 
+/* ----------------------------------------------------------------------------------------------------------------
+ * Sim3 refinement of a loop candidate (optimize::transform_optimizer::optimize, optimize/transform_optimizer.cc:20-158): one Sim3_12
+ * vertex, a forward and a backward reprojection edge per matched pair (internal/sim3/mutual_reproj_edge_wrapper.h) with Huber delta
+ * sqrt(chi_sq), g2o's Levenberg-Marquardt with numeric central-difference Jacobians (delta 1e-9) and no terminate action:
+ * optimize(5), the outlier test, optimize(num_iter) on the surviving pairs, the inlier count.  One CTA per problem, the whole protocol in
+ * one launch on the handle's stream.  The caller gathers the pairs as :58-94 does (stella_vslam_b200.optimize.gather_mutual_edges
+ * restates it).  The 7x7 system is solved by a dense Cholesky instead of SimplicialLDLT (DESIGN.md section 8).
+ * ---------------------------------------------------------------------------------------------------------------- */
+typedef struct b200_transform_problem {
+    int32_t n_matches;              /* gathered pairs, in ascending idx1 */
+    int32_t fix_scale;              /* transform_vertex::fix_scale_ (stereo / RGBD) */
+    b200_sim3_t sim3_12;            /* initial Sim3_12 as the caller built it: g2o::Sim3(rot_12, trans_12, scale_12) */
+    double rot_1w[9], trans_1w[3];  /* keyfrm_1->get_rot_cw() row-major, get_trans_cw() */
+    double rot_2w[9], trans_2w[3];  /* keyfrm_2 */
+    b200_camera_t cam_1, cam_2;     /* model 0 (perspective / fisheye / radial division) or 1 (equirectangular); fxb unused */
+    const float* obs_1;             /* n x 2: keyfrm_1's undistorted keypoint idx1 (observation of edge_12) */
+    const float* inv_sigma_sq_1;    /* n: keyfrm_1's inv_level_sigma_sq_[octave] */
+    const double* pos_w_2;          /* n x 3: lm_2->get_pos_in_world() (point of edge_12) */
+    const float* obs_2;             /* n x 2: keyfrm_2's undistorted keypoint idx2 (observation of edge_21) */
+    const float* inv_sigma_sq_2;    /* n */
+    const double* pos_w_1;          /* n x 3: lm_1->get_pos_in_world() (point of edge_21) */
+    /* out */
+    b200_sim3_t sim3_12_out;        /* optimised Sim3_12; the input when the second round did not run */
+    uint8_t* keep;                  /* n: 1 = the entry stays non-null in matched_lms_in_keyfrm_2 */
+    uint32_t num_inliers;           /* return value of optimize() */
+    int32_t n_outliers_round1;      /* pairs nulled by the first outlier test */
+    int32_t iterations[2];          /* LM iterations of optimize(5) and optimize(num_iter) */
+    int32_t trials[2];              /* linear solves of each round */
+    double chi2[2];                 /* active robust chi2 of the state each round leaves */
+    double lambda_init[2];          /* computeLambdaInit of each round */
+} b200_transform_problem_t;
+/* transform_optimizer(fix_scale, num_iter)::optimize(..., chi_sq) for every problem.  Results are independent of the batch.
+ * B200_ERR_INVALID (nothing written): a null handle or required pointer, a negative count, chi_sq <= 0 or non-finite, num_iter < 0,
+ * a non-finite value, a scale <= 0 or a quaternion whose norm is not within [0.5, 2] in sim3_12, a camera model other than 0 or 1, an
+ * inv_sigma_sq <= 0. */
+int b200_transform_optimize(b200_lba_t h, int n_problems, b200_transform_problem_t* problems, float chi_sq, int num_iter);
+
 /* Profiling mode: an event after every launch of the following solves (adds a few microseconds per launch; off by default).
  * b200_lba_kernel_ms reports, for the LAST batch, the summed device time and the number of intervals of
  *   kernel 0 plan (5 launches, one interval), 1 landmark pass / build, 2 keyframe rows, 3 Schur rows, 4 reduced-system Cholesky,

@@ -9,6 +9,7 @@
 //   b200::match::projection / fuse / area / bow_tree / stereo  <->  match/projection.h, fuse.h, area.h, bow_tree.h, stereo.h
 //   b200::optimize::local_bundle_adjuster <-> stella_vslam::optimize::local_bundle_adjuster (optimize/local_bundle_adjuster.h:15-24)
 //   b200::optimize::pose_optimizer        <-> stella_vslam::optimize::pose_optimizer        (optimize/pose_optimizer.h:24-40)
+//   b200::optimize::transform_optimizer   <-> stella_vslam::optimize::transform_optimizer   (optimize/transform_optimizer.h:17-48)
 //   b200::util::stereo_rectifier          <-> stella_vslam::util::stereo_rectifier          (util/stereo_rectifier.h:14-46)
 //   b200::solve::pnp_solver               <-> stella_vslam::solve::pnp_solver               (solve/pnp_solver.h:13-142)
 #pragma once
@@ -446,6 +447,32 @@ public:
     const unsigned int min_num_shared_lms_;
 
 private:
+    b200_lba_t h_ = nullptr;
+};
+
+class transform_optimizer {  // optimize/transform_optimizer.h:17-48: optimize() on pairs gathered as transform_optimizer.cc:58-94 does
+public:
+    explicit transform_optimizer(bool fix_scale, unsigned int num_iter = 10, int device = 0) : fix_scale_(fix_scale), num_iter_(num_iter) {
+        check(b200_lba_create(device, &h_), "b200_lba_create");
+    }
+    ~transform_optimizer() { b200_lba_destroy(h_); }
+    transform_optimizer(const transform_optimizer&) = delete;
+    // problems: inputs filled by the caller (n_matches, sim3_12, poses, cameras, the pair arrays, keep); fix_scale is set here.
+    // Writes the outputs of every problem; returns nothing (each problem's num_inliers is optimize()'s return value).
+    void optimize_batch(std::vector<b200_transform_problem_t>& problems, float chi_sq = 10.0f) const {
+        for (auto& p : problems) p.fix_scale = fix_scale_ ? 1 : 0;
+        check(b200_transform_optimize(h_, (int)problems.size(), problems.data(), chi_sq, (int)num_iter_), "b200_transform_optimize");
+    }
+    unsigned int optimize(b200_transform_problem_t& problem, float chi_sq = 10.0f) const {
+        problem.fix_scale = fix_scale_ ? 1 : 0;
+        check(b200_transform_optimize(h_, 1, &problem, chi_sq, (int)num_iter_), "b200_transform_optimize");
+        return problem.num_inliers;
+    }
+    b200_lba_t handle() const { return h_; }
+
+private:
+    const bool fix_scale_;
+    const unsigned int num_iter_;
     b200_lba_t h_ = nullptr;
 };
 

@@ -24,6 +24,8 @@ SOURCES = {
     "pnp_kernels.cu": [],
     # the pose-graph Jacobian is a central difference at delta 1e-9: no contraction on either side, as in tests/pgo_oracle.c
     "pgo_kernels.cu": ["-fmad=false", "-Xcompiler", "-ffp-contract=off"],
+    # the transform optimiser's Jacobian is the same central difference (tests/transform_oracle.c)
+    "transform_kernels.cu": ["-fmad=false", "-Xcompiler", "-ffp-contract=off"],
 }
 
 

@@ -29,6 +29,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "lm_common.cuh"
 #include "quat.cuh"
 #include "track_chain.cuh"
 
@@ -129,9 +130,8 @@ __device__ __forceinline__ void edge_jacobians(const EdgeS& e, const Cam& c, con
     }
 }
 
-// RobustKernelHuber: rho[1] weight and rho[0] cost
-__device__ __forceinline__ double huber_weight(double e2, double delta) { return (e2 <= delta * delta) ? 1.0 : delta / sqrt(e2); }
-__device__ __forceinline__ double huber_cost(double e2, double delta) { return (e2 <= delta * delta) ? e2 : 2 * sqrt(e2) * delta - delta * delta; }
+using b200::huber_cost;  // lm_common.cuh
+using b200::huber_weight;
 
 __device__ __forceinline__ double block_sum(double v, double* sh) {  // deterministic tree reduction, blockDim.x power of two <= 1024
     const int tid = threadIdx.x;
@@ -1715,28 +1715,6 @@ __device__ __forceinline__ void pose_rt(const double* q, const double* t, double
     Rt[10] = t[1];
     Rt[11] = t[2];
 }
-// sum of v over the CTA in a fixed order: warp shuffle tree, then the warp leaders in index order
-template <int N>
-__device__ __forceinline__ void cta_sum(double (&v)[N], double* out, double* scratch) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int i = 0; i < N; ++i) {
-#pragma unroll
-        for (int s2 = 16; s2 > 0; s2 >>= 1) v[i] += __shfl_down_sync(0xFFFFFFFFu, v[i], s2);
-    }
-    __syncthreads();
-    if (lane == 0)
-#pragma unroll
-        for (int i = 0; i < N; ++i) scratch[warp * N + i] = v[i];
-    __syncthreads();
-    if (threadIdx.x < N) {
-        double r = 0.0;
-        for (int w = 0; w < kPoseThreads / 32; ++w) r += scratch[w * N + threadIdx.x];
-        out[threadIdx.x] = r;
-    }
-    __syncthreads();
-}
-
 __global__ void __launch_bounds__(kPoseThreads) pose_optimize_kernel(const PoseProb* __restrict__ probs, const PoseEdge* __restrict__ edges_all,
                                                                      unsigned char* __restrict__ level_all, unsigned char* __restrict__ flags_all,
                                                                      int trials_robust, int trials, int each_iter, double* __restrict__ pose_out,
@@ -1813,7 +1791,7 @@ __global__ void __launch_bounds__(kPoseThreads) pose_optimize_kernel(const PoseP
             __syncthreads();
             double acc[28];
             accumulate(Rt, true, acc);
-            cta_sum<28>(acc, red, scratch);
+            cta_sum<kPoseThreads>(acc, red, scratch);
             if (tid == 0) {
                 if (s_it == 0) {  // computeLambdaInit
                     s_cur_chi = red[27];
@@ -1885,7 +1863,7 @@ __global__ void __launch_bounds__(kPoseThreads) pose_optimize_kernel(const PoseP
                 double tacc[28];
                 accumulate(Rt_trial, false, tacc);
                 double chi1[1] = {tacc[27]};
-                cta_sum<1>(chi1, red + 27, scratch);  // red[0..26] (H, b of the current state) stay valid for the next trial
+                cta_sum<kPoseThreads>(chi1, red + 27, scratch);  // red[0..26] (H, b of the current state) stay valid for the next trial
                 if (tid == 0) {
                     const bool ok2 = s_ok2 != 0;
                     const double temp_chi = ok2 ? red[27] : 1.7976931348623157e308;

@@ -56,15 +56,7 @@ struct Plan {
     long long flops = 0;
 };
 
-static bool finite_sim3(const b200_sim3_t& x) {
-    for (int k = 0; k < 4; ++k)
-        if (!std::isfinite(x.q[k])) return false;
-    for (int k = 0; k < 3; ++k)
-        if (!std::isfinite(x.t[k])) return false;
-    // a quaternion far from unit norm (zero, denormal) would divide by ~0 in Sim3::inverse's normalisation
-    const double n2 = x.q[0] * x.q[0] + x.q[1] * x.q[1] + x.q[2] * x.q[2] + x.q[3] * x.q[3];
-    return std::isfinite(x.s) && x.s > 0 && n2 > 0.25 && n2 < 4.0;
-}
+static bool finite_sim3(const b200_sim3_t& x) { return sim3::well_formed(x.q, x.t, x.s); }
 
 static int validate(const b200_pose_graph_t* g, const char* who) {
     if (!g || g->n_vertices <= 0 || g->n_edges < 0 || g->n_points < 0 || !g->estimate || !g->fixed

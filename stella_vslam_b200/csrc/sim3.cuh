@@ -236,7 +236,18 @@ __host__ __device__ inline void log7(const Sim3& g, double* res) {
     res[6] = sigma;
 }
 
-// shot_vertex::oplusImpl: estimate <- Sim3(update) * estimate, update(6) zeroed under fix_scale
+// Host-side input check of the optimisers: finite, scale > 0, and a quaternion near unit norm (a zero or denormal one would divide
+// by ~0 in inverse()'s normalisation).
+inline bool well_formed(const double* q, const double* t, double s) {
+    for (int k = 0; k < 4; ++k)
+        if (!std::isfinite(q[k])) return false;
+    for (int k = 0; k < 3; ++k)
+        if (!std::isfinite(t[k])) return false;
+    const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+    return std::isfinite(s) && s > 0 && n2 > 0.25 && n2 < 4.0;
+}
+
+// shot_vertex::oplusImpl and transform_vertex::oplusImpl: estimate <- Sim3(update) * estimate, update(6) zeroed under fix_scale
 __host__ __device__ inline Sim3 oplus(const Sim3& est, const double* upd, bool fix_scale) {
     double u[7] = {upd[0], upd[1], upd[2], upd[3], upd[4], upd[5], fix_scale ? 0.0 : upd[6]};
     return mul(exp7(u), est);

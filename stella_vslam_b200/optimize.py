@@ -43,6 +43,7 @@ def _bind():
     L.b200_global_ba_solve.argtypes = [vp, C.POINTER(LbaProblem), C.c_int, C.c_double, vp, vp, vp, C.POINTER(LbaStats)]
     L.b200_graph_optimize.argtypes = [vp, C.POINTER(PoseGraph), C.c_int, C.c_double, C.POINTER(PgoStats)]
     L.b200_pgo_envelope.argtypes = [C.POINTER(PoseGraph), C.POINTER(C.c_int32), vp, C.POINTER(C.c_int64)]
+    L.b200_transform_optimize.argtypes = [vp, C.c_int, C.POINTER(TransformProblem), C.c_float, C.c_int]
     return L
 
 
@@ -514,3 +515,138 @@ class graph_optimizer:
         out = dict(estimate=keep["estimate_out"], pose_cw=keep["pose_cw_out"], points=keep["points_out"])
         out.update({name: getattr(st, name) for name, _ in PgoStats._fields_})
         return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# optimize::transform_optimizer (optimize/transform_optimizer.{h,cc}): the Sim3 refinement of a loop candidate
+# ---------------------------------------------------------------------------------------------------------------------------------
+class TransformProblem(C.Structure):
+    """b200_transform_problem_t (include/b200vslam.h)."""
+    _fields_ = [("n_matches", C.c_int32), ("fix_scale", C.c_int32), ("sim3_12", Sim3), ("rot_1w", C.c_double * 9), ("trans_1w", C.c_double * 3),
+                ("rot_2w", C.c_double * 9), ("trans_2w", C.c_double * 3), ("cam_1", Camera), ("cam_2", Camera), ("obs_1", C.c_void_p),
+                ("inv_sigma_sq_1", C.c_void_p), ("pos_w_2", C.c_void_p), ("obs_2", C.c_void_p), ("inv_sigma_sq_2", C.c_void_p),
+                ("pos_w_1", C.c_void_p), ("sim3_12_out", Sim3), ("keep", C.c_void_p), ("num_inliers", C.c_uint32),
+                ("n_outliers_round1", C.c_int32), ("iterations", C.c_int32 * 2), ("trials", C.c_int32 * 2), ("chi2", C.c_double * 2),
+                ("lambda_init", C.c_double * 2)]
+
+
+def _camera(c):
+    return Camera(int(c["model"]), *[float(c.get(k, 0.0)) for k in ("fx", "fy", "cx", "cy", "fxb", "cols", "rows")])
+
+
+def gather_mutual_edges(keyfrm_1, keyfrm_2, matched_lms_in_keyfrm_2):
+    """transform_optimizer::optimize step 3 (transform_optimizer.cc:58-94): the pairs that get a forward and a backward edge.
+
+    keyfrm_1 / keyfrm_2: dict(id, rot_cw (3x3), trans_cw (3), camera (b200_camera_t fields), undist_keypts (n, 2), octaves (n,),
+        inv_level_sigma_sq (per octave), landmarks (keyframe 1: get_landmarks(), a list of landmarks or None per keypoint)).
+    A landmark: dict(pos_w (3), will_be_erased (bool), observations {keyframe id: keypoint index}).
+    matched_lms_in_keyfrm_2: a landmark or None per keypoint of keyframe 1.
+    Returns (problem dict in the layout of transform_optimizer.optimize without sim3_12, idx1 of every pair in ascending order)."""
+    lms_1 = keyfrm_1["landmarks"]
+    idx1s, idx2s, lm1s, lm2s = [], [], [], []
+    for idx1, lm_2 in enumerate(matched_lms_in_keyfrm_2):
+        if lm_2 is None:
+            continue
+        lm_1 = lms_1[idx1]
+        if lm_1 is None:
+            continue
+        if lm_1.get("will_be_erased", False) or lm_2.get("will_be_erased", False):
+            continue
+        idx2 = lm_2.get("observations", {}).get(keyfrm_2["id"], -1)   # get_index_in_keyframe
+        if idx2 < 0:
+            continue
+        idx1s.append(idx1)
+        idx2s.append(idx2)
+        lm1s.append(lm_1)
+        lm2s.append(lm_2)
+
+    def obs(kf, idx):
+        kp = np.asarray(kf["undist_keypts"], np.float32).reshape(-1, 2)
+        sig = np.asarray(kf["inv_level_sigma_sq"], np.float32)
+        octv = np.asarray(kf["octaves"], np.int64)
+        idx = np.asarray(idx, np.int64)
+        return kp[idx].reshape(-1, 2), sig[octv[idx]]
+
+    obs_1, w1 = obs(keyfrm_1, idx1s)
+    obs_2, w2 = obs(keyfrm_2, idx2s)
+    prob = dict(n_matches=len(idx1s), rot_1w=np.asarray(keyfrm_1["rot_cw"], np.float64), trans_1w=np.asarray(keyfrm_1["trans_cw"], np.float64),
+                rot_2w=np.asarray(keyfrm_2["rot_cw"], np.float64), trans_2w=np.asarray(keyfrm_2["trans_cw"], np.float64),
+                cam_1=keyfrm_1["camera"], cam_2=keyfrm_2["camera"], obs_1=obs_1, inv_sigma_sq_1=w1,
+                pos_w_2=np.array([lm["pos_w"] for lm in lm2s], np.float64).reshape(-1, 3), obs_2=obs_2, inv_sigma_sq_2=w2,
+                pos_w_1=np.array([lm["pos_w"] for lm in lm1s], np.float64).reshape(-1, 3))
+    return prob, np.array(idx1s, np.int64)
+
+
+def pack_transform_problem(problem, fix_scale):
+    """problem dict -> (TransformProblem, keep-alive dict holding the keep output)."""
+    keep = {}
+
+    def arr(name, x, dt, shape):
+        a = np.ascontiguousarray(np.asarray(x, dt).reshape(shape))
+        keep[name] = a
+        return a.ctypes.data
+
+    n = len(problem["obs_1"])
+    P = TransformProblem()
+    P.n_matches, P.fix_scale = n, int(bool(fix_scale))
+    s = np.asarray(problem["sim3_12"], np.float64).reshape(8)
+    P.sim3_12 = Sim3((C.c_double * 4)(*s[:4]), (C.c_double * 3)(*s[4:7]), float(s[7]))
+    P.rot_1w = (C.c_double * 9)(*np.asarray(problem["rot_1w"], np.float64).reshape(9))
+    P.trans_1w = (C.c_double * 3)(*np.asarray(problem["trans_1w"], np.float64).reshape(3))
+    P.rot_2w = (C.c_double * 9)(*np.asarray(problem["rot_2w"], np.float64).reshape(9))
+    P.trans_2w = (C.c_double * 3)(*np.asarray(problem["trans_2w"], np.float64).reshape(3))
+    P.cam_1, P.cam_2 = _camera(problem["cam_1"]), _camera(problem["cam_2"])
+    P.obs_1 = arr("obs_1", problem["obs_1"], np.float32, (n, 2))
+    P.inv_sigma_sq_1 = arr("inv_sigma_sq_1", problem["inv_sigma_sq_1"], np.float32, n)
+    P.pos_w_2 = arr("pos_w_2", problem["pos_w_2"], np.float64, (n, 3))
+    P.obs_2 = arr("obs_2", problem["obs_2"], np.float32, (n, 2))
+    P.inv_sigma_sq_2 = arr("inv_sigma_sq_2", problem["inv_sigma_sq_2"], np.float32, n)
+    P.pos_w_1 = arr("pos_w_1", problem["pos_w_1"], np.float64, (n, 3))
+    keep["keep"] = np.zeros(max(n, 1), np.uint8)
+    P.keep = keep["keep"].ctypes.data
+    return P, keep
+
+
+def _transform_result(P, keep):
+    o = P.sim3_12_out
+    return dict(sim3_12=np.array(list(o.q) + list(o.t) + [o.s]), keep=keep["keep"][:P.n_matches].copy(), num_inliers=int(P.num_inliers),
+                n_outliers_round1=int(P.n_outliers_round1), iterations=list(P.iterations), trials=list(P.trials), chi2=list(P.chi2),
+                lambda_init=list(P.lambda_init))
+
+
+class transform_optimizer:
+    """optimize::transform_optimizer (optimize/transform_optimizer.h:17-48): the Sim3 refinement of loop candidates on the GPU, one
+    launch for a whole batch.  gather_mutual_edges() restates how the reference picks the pairs; optimize() runs the rest of
+    transform_optimizer::optimize on them."""
+
+    def __init__(self, fix_scale, num_iter=10, device=0):
+        self.fix_scale_, self.num_iter_ = bool(fix_scale), int(num_iter)
+        self._L = _bind()
+        self._h = C.c_void_p()
+        check(self._L.b200_lba_create(device, C.byref(self._h)))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.b200_lba_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def optimize_batch(self, problems, chi_sq=10.0):
+        """problems: dicts (workloads.synth.make_sim3_pair layout; sim3_12 is the initial Sim3_12 as an 8-vector q x y z w, t, s).
+        Returns per problem dict(sim3_12: the refined Sim3_12, or the input when the second round did not run; keep (n,) uint8: 1 where
+        the entry stays in matched_lms_in_keyfrm_2; num_inliers: the return value; n_outliers_round1, iterations, trials, chi2,
+        lambda_init)."""
+        if not problems:
+            return []
+        packed = [pack_transform_problem(pr, self.fix_scale_) for pr in problems]
+        arr = (TransformProblem * len(packed))(*[pk[0] for pk in packed])
+        check(self._L.b200_transform_optimize(self._h, len(packed), arr, float(chi_sq), self.num_iter_))
+        return [_transform_result(arr[i], pk[1]) for i, pk in enumerate(packed)]
+
+    def optimize(self, problem, chi_sq=10.0):
+        return self.optimize_batch([problem], chi_sq)[0]

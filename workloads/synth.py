@@ -837,3 +837,88 @@ def make_pose_graph(n_keyframes=500, seed=0, fix_scale=False, laps=1.5, window=8
                 found_lm_to_ref_keyfrm_id=found)
     graph = build_essential_graph(**desc)
     return (graph, desc) if return_description else graph
+
+
+def make_sim3_pair(seed=0, n_matches=300, models=("perspective", "perspective"), fix_scale=False, outlier_frac=0.2, pixel_sigma=1.0,
+                   init_noise=(0.02, 0.05, 0.02)):
+    """A loop candidate for optimize.transform_optimizer: keyframe 1 of the map and keyframe 2 of a drifted map see the same physical
+    points, and the gathered pairs are already matched (gather_mutual_edges' output layout).
+
+    The drifted map is the true one under a Sim3 (scale 1 under fix_scale): its landmarks (pos_w_2) and keyframe 2's pose are expressed
+    in it, so the true Sim3_12 maps keyframe 2's camera frame, at the drifted scale, into keyframe 1's.  models: camera of keyframe 1 and
+    2, "perspective" or "equirect".  Observations carry level-dependent noise (pixel_sigma * 1.2^octave); a fraction outlier_frac of
+    the pairs has a gross error of 20-80 px on one of its two observations.  The initial Sim3 is the truth perturbed by init_noise =
+    (rotation rad, translation m, log scale), as the loop detector's estimate would be.  Returns the problem dict plus gt_sim3_12 and
+    gt_outlier."""
+    from stella_vslam_b200.optimize import sim3_from_rts
+
+    rng = np.random.default_rng(seed)
+    n = int(n_matches)
+
+    def camera(model):
+        if model == "equirect":
+            return dict(model=1, fx=0.0, fy=0.0, cx=0.0, cy=0.0, fxb=0.0, cols=3840.0, rows=1920.0)
+        return dict(model=0, fx=KITTI["fx"], fy=KITTI["fy"], cx=KITTI["cx"], cy=KITTI["cy"], fxb=0.0, cols=float(KITTI["cols"]),
+                    rows=float(KITTI["rows"]))
+
+    cam1, cam2 = camera(models[0]), camera(models[1])
+    # true poses (camera from world): keyframe 2 is a nearby view of keyframe 1's scene
+    R1 = _rot_y(0.3 * rng.standard_normal()) @ _rodrigues(0.03 * rng.standard_normal(3))
+    t1 = rng.normal(0, 1.0, 3)
+    R21 = _rot_y(0.05 * rng.standard_normal()) @ _rodrigues(0.02 * rng.standard_normal(3))
+    R2 = R21 @ R1
+    t2 = R21 @ t1 + np.array([rng.uniform(-0.8, 0.8), 0.1 * rng.standard_normal(), 0.2 * rng.standard_normal()])
+
+    def proj(cam, pc):
+        if cam["model"] == 1:
+            th, ph = np.arctan2(pc[:, 0], pc[:, 2]), -np.arcsin(pc[:, 1] / np.linalg.norm(pc, axis=1))
+            return np.stack([cam["cols"] * (0.5 + th / (2 * np.pi)), cam["rows"] * (0.5 - ph / np.pi)], 1)
+        return np.stack([cam["fx"] * pc[:, 0] / pc[:, 2] + cam["cx"], cam["fy"] * pc[:, 1] / pc[:, 2] + cam["cy"]], 1)
+
+    def visible(cam, pc):
+        if cam["model"] == 1:
+            return np.linalg.norm(pc, axis=1) > 1.0
+        uv = proj(cam, np.where(pc[:, 2:3] > 0.5, pc, 1.0))
+        return (pc[:, 2] > 0.5) & (uv[:, 0] > 10) & (uv[:, 0] < cam["cols"] - 10) & (uv[:, 1] > 10) & (uv[:, 1] < cam["rows"] - 10)
+
+    X = np.zeros((0, 3))
+    while len(X) < n:                                        # points seen by both keyframes, 4-40 m from keyframe 1
+        m = 4 * n + 64
+        depth = rng.uniform(4, 40, m)
+        if cam1["model"] == 1:
+            d = rng.standard_normal((m, 3))
+            pc1 = d / np.linalg.norm(d, axis=1, keepdims=True) * depth[:, None]
+        else:
+            u, v = rng.uniform(20, cam1["cols"] - 20, m), rng.uniform(20, cam1["rows"] - 20, m)
+            pc1 = np.stack([(u - cam1["cx"]) / cam1["fx"] * depth, (v - cam1["cy"]) / cam1["fy"] * depth, depth], 1)
+        Xw = (pc1 - t1) @ R1
+        ok = visible(cam2, Xw @ R2.T + t2)
+        X = np.concatenate([X, Xw[ok]])[:n]
+    # the drifted map: P_B = s_d R_d X + t_d; keyframe 2's pose in it
+    s_d = 1.0 if fix_scale else float(np.exp(0.2 * rng.standard_normal()))
+    R_d = _rodrigues(0.1 * rng.standard_normal(3))
+    t_d = rng.normal(0, 2.0, 3)
+    pos_w_1 = X.copy()
+    pos_w_2 = s_d * X @ R_d.T + t_d
+    rot_2w = R2 @ R_d.T
+    trans_2w = s_d * t2 - rot_2w @ t_d
+    R12 = R1 @ R2.T
+    gt = sim3_from_rts(R12, t1 - R12 @ t2, 1.0 / s_d)
+    # observations with octave-dependent noise
+    inv_sigma = (np.float32(1.0) / np.cumprod(np.concatenate([[np.float32(1.0)], np.full(7, np.float32(1.2))])).astype(np.float32) ** 2).astype(np.float32)
+    lv1, lv2 = rng.integers(0, 8, n), rng.integers(0, 8, n)
+    obs_1 = proj(cam1, X @ R1.T + t1) + (pixel_sigma / np.sqrt(inv_sigma[lv1].astype(np.float64)))[:, None] * rng.standard_normal((n, 2))
+    obs_2 = proj(cam2, X @ R2.T + t2) + (pixel_sigma / np.sqrt(inv_sigma[lv2].astype(np.float64)))[:, None] * rng.standard_normal((n, 2))
+    bad = rng.random(n) < outlier_frac
+    which = rng.integers(0, 2, n)
+    for o, side in ((obs_1, 0), (obs_2, 1)):
+        sel = bad & (which == side)
+        o[sel] += rng.choice([-1, 1], (sel.sum(), 2)) * rng.uniform(20, 80, (sel.sum(), 2))
+    # initial estimate: the truth perturbed
+    dR = _rodrigues(init_noise[0] * rng.standard_normal(3) / np.sqrt(3))
+    s0 = 1.0 / s_d if fix_scale else float(np.exp(init_noise[2] * rng.standard_normal())) / s_d
+    t0 = dR @ (t1 - R12 @ t2) + init_noise[1] * rng.standard_normal(3) / np.sqrt(3)
+    init = sim3_from_rts(dR @ R12, t0, s0)
+    return dict(n_matches=n, fix_scale=bool(fix_scale), sim3_12=init, rot_1w=R1, trans_1w=t1, rot_2w=rot_2w, trans_2w=trans_2w, cam_1=cam1,
+                cam_2=cam2, obs_1=obs_1.astype(np.float32), inv_sigma_sq_1=inv_sigma[lv1], pos_w_2=pos_w_2, obs_2=obs_2.astype(np.float32),
+                inv_sigma_sq_2=inv_sigma[lv2], pos_w_1=pos_w_1, gt_sim3_12=gt, gt_outlier=bad)
