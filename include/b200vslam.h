@@ -697,6 +697,40 @@ int b200_mt19937_seed(b200_mt19937_t* engine, const uint32_t* seed_seq, int n_se
 uint32_t b200_mt19937_next(b200_mt19937_t* engine);
 /* max_num_iter minimal sets (out: max_num_iter x 4) from one engine, continuing its state; n_matches >= 4. */
 int b200_pnp_draw_min_sets(b200_mt19937_t* engine, uint32_t n_matches, uint32_t max_num_iter, int32_t* out);
+/* max_num_iter calls of util::create_random_array(set_size, 0, n_matches - 1, engine) (out: max_num_iter x set_size), continuing the
+ * engine's state.  B200_ERR_INVALID for a null engine, set_size outside [1, 65535] or n_matches < set_size. */
+int b200_draw_min_sets(b200_mt19937_t* engine, uint32_t set_size, uint32_t n_matches, uint32_t max_num_iter, int32_t* out);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * Robust matching's essential matrix: solve::essential_solver::find_via_ransac (src/stella_vslam/solve/essential_solver.cc) with the
+ * five-point minimal set (Stewenius et al.), for many problems (frame x keyframe, or an equirectangular initialisation) in one launch
+ * sequence on the b200_lba_t handle's stream.  fp64 in the CPU restatement's evaluation order; the pieces of Eigen it uses (FullPivLU,
+ * EigenSolver, JacobiSVD with its QR preconditioners) restated.  Deviations (DESIGN.md section 8): Eigen's vectorised summation and
+ * blocked triangular-solve order are not reproduced; a RealSchur that does not converge gives no candidates (the reference reads
+ * uninitialised eigenvalues) and sets status; Jacobi sweeps are bounded.
+ * ---------------------------------------------------------------------------------------------------------------- */
+typedef struct b200_essential_problem {
+    int32_t n_matches;
+    const double* bearings_1;       /* n x 3: bearings_1[matches_12[i].first] */
+    const double* bearings_2;       /* n x 3: bearings_2[matches_12[i].second] */
+    uint32_t min_set_size;          /* must be 5 (every caller in the reference passes the default) */
+    uint32_t max_num_iter;          /* robust matcher: 1000 */
+    int32_t recompute;              /* find_via_ransac's recompute */
+    const int32_t* min_sets;        /* max_num_iter x min_set_size: util::create_random_array's draws in draw order (b200_draw_min_sets) */
+    /* out */
+    int32_t status;                 /* B200_OK, or B200_ERR_INVALID when a RealSchur did not converge or a Jacobi SVD hit its sweep bound */
+    int32_t valid;                  /* solution_is_valid() */
+    int32_t best_iter;              /* iteration of the RANSAC winner (-1 none) */
+    int32_t best_candidate;         /* its candidate, in eigenvalue order (-1 none) */
+    int32_t num_inliers;            /* of the RANSAC winner (before the recompute) */
+    float best_cost;                /* get_best_cost(): FLT_MAX when no winner; 0 on the early return (the member's initial value) */
+    double E_21[9];                 /* row-major get_best_E_21(); written only when valid */
+    uint8_t* inlier_flags;          /* n: get_inlier_matches(); all 0 when not valid; untouched on the early return (n < min_set_size) */
+} b200_essential_problem_t;
+/* find_via_ransac(max_num_iter, recompute, 5) for every problem: one upload, the hypothesis, scoring and selection launches, one
+ * download.  B200_ERR_INVALID (nothing written) for a negative count, a null required pointer, min_set_size != 5 or a min_sets index
+ * outside [0, n) of a problem that runs RANSAC. */
+int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t* problems);
 
 /* ----------------------------------------------------------------------------------------------------------------
  * Pose-graph optimisation (optimize::graph_optimizer, optimize/graph_optimizer.cc:254-302): the Sim3 essential graph of a loop

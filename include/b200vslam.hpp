@@ -12,6 +12,7 @@
 //   b200::optimize::transform_optimizer   <-> stella_vslam::optimize::transform_optimizer   (optimize/transform_optimizer.h:17-48)
 //   b200::util::stereo_rectifier          <-> stella_vslam::util::stereo_rectifier          (util/stereo_rectifier.h:14-46)
 //   b200::solve::pnp_solver               <-> stella_vslam::solve::pnp_solver               (solve/pnp_solver.h:13-142)
+//   b200::solve::essential_solver         <-> stella_vslam::solve::essential_solver         (solve/essential_solver.h)
 #pragma once
 
 #include <cmath>
@@ -702,6 +703,98 @@ private:
     bool solution_is_valid_ = false;
     int status_ = B200_OK;
     double best_rot_cw_[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, best_trans_cw_[3] = {0, 0, 0};
+    std::vector<bool> is_inlier_match_;
+};
+
+
+// util::create_random_array(set_size, 0, n - 1, engine), max_num_iter times from one engine (b200_draw_min_sets), max_num_iter x set_size
+inline std::vector<int32_t> draw_min_sets(b200_mt19937_t& engine, uint32_t set_size, uint32_t n_matches, uint32_t max_num_iter) {
+    std::vector<int32_t> out((size_t)set_size * max_num_iter);
+    check(b200_draw_min_sets(&engine, set_size, n_matches, max_num_iter, out.data()), "b200_draw_min_sets");
+    return out;
+}
+
+// essential_solver::find_via_ransac for many problems in one call (b200_essential_ransac); the problems' out fields are filled
+inline void essential_ransac_batch(b200_lba_t h, std::vector<b200_essential_problem_t>& problems) {
+    check(b200_essential_ransac(h, (int)problems.size(), problems.data()), "b200_essential_ransac");
+}
+
+// solve::essential_solver (solve/essential_solver.h).  bearings: n x 3 row-major; matches_12: (first, second) index pairs; E_21
+// row-major.  The engine is the solver's member: find_via_ransac continues its state across calls.  The solver owns a b200_lba_t
+// handle unless one is given.  Only the five-point minimal set (min_set_size = 5, every caller's value) is supported.
+class essential_solver {
+public:
+    essential_solver(const std::vector<double>& bearings_1, const std::vector<double>& bearings_2,
+                     const std::vector<std::pair<int, int>>& matches_12, bool use_fixed_seed = false, b200_lba_t handle = nullptr)
+        : num_matches_((unsigned int)matches_12.size()), h_(handle) {
+        b1_.reserve(3 * matches_12.size());
+        b2_.reserve(3 * matches_12.size());
+        for (const auto& m : matches_12) {
+            if (m.first < 0 || 3 * (size_t)m.first + 3 > bearings_1.size() || m.second < 0 || 3 * (size_t)m.second + 3 > bearings_2.size())
+                throw std::out_of_range("essential_solver: match index outside the bearings");
+            b1_.insert(b1_.end(), bearings_1.begin() + 3 * m.first, bearings_1.begin() + 3 * m.first + 3);
+            b2_.insert(b2_.end(), bearings_2.begin() + 3 * m.second, bearings_2.begin() + 3 * m.second + 3);
+        }
+        if (use_fixed_seed) {  // util::create_random_engine
+            check(b200_mt19937_seed(&engine_, nullptr, 0), "b200_mt19937_seed");
+        } else {
+            std::random_device rd;
+            uint32_t words[10];
+            for (auto& w : words) w = rd();
+            check(b200_mt19937_seed(&engine_, words, 10), "b200_mt19937_seed");
+        }
+    }
+    ~essential_solver() {
+        if (own_) b200_lba_destroy(h_);
+    }
+    essential_solver(const essential_solver&) = delete;
+    essential_solver& operator=(const essential_solver&) = delete;
+
+    void find_via_ransac(unsigned int max_num_iter, bool recompute = true, unsigned int min_set_size = 5) {
+        if (min_set_size != 5) throw std::invalid_argument("essential_solver: only the five-point minimal set is supported");
+        if (num_matches_ < min_set_size) {  // before any draw (essential_solver.cc:23-26)
+            solution_is_valid_ = false;
+            return;
+        }
+        if (!h_) {
+            check(b200_lba_create(0, &h_), "b200_lba_create");
+            own_ = true;
+        }
+        const std::vector<int32_t> sets = draw_min_sets(engine_, 5, num_matches_, max_num_iter);
+        std::vector<uint8_t> flags(num_matches_);
+        b200_essential_problem_t P{};
+        P.n_matches = (int32_t)num_matches_;
+        P.bearings_1 = b1_.data();
+        P.bearings_2 = b2_.data();
+        P.min_set_size = 5;
+        P.max_num_iter = max_num_iter;
+        P.recompute = recompute ? 1 : 0;
+        P.min_sets = sets.data();
+        P.inlier_flags = flags.data();
+        check(b200_essential_ransac(h_, 1, &P), "b200_essential_ransac");
+        status_ = P.status;
+        solution_is_valid_ = P.valid != 0;
+        best_cost_ = P.best_cost;
+        if (solution_is_valid_)
+            for (int k = 0; k < 9; ++k) best_E_21_[k] = P.E_21[k];
+        is_inlier_match_.assign(flags.begin(), flags.end());
+    }
+    bool solution_is_valid() const { return solution_is_valid_; }
+    float get_best_cost() const { return best_cost_; }
+    const double* get_best_E_21() const { return best_E_21_; }
+    std::vector<bool> get_inlier_matches() const { return is_inlier_match_; }
+    int status() const { return status_; }  // B200_ERR_INVALID when a RealSchur or a Jacobi SVD of the last call did not converge
+
+private:
+    unsigned int num_matches_;
+    std::vector<double> b1_, b2_;
+    b200_mt19937_t engine_;
+    b200_lba_t h_ = nullptr;
+    bool own_ = false;
+    bool solution_is_valid_ = false;
+    int status_ = B200_OK;
+    float best_cost_ = 0.0f;
+    double best_E_21_[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     std::vector<bool> is_inlier_match_;
 };
 

@@ -22,6 +22,7 @@ SOURCES = {
     # the rectification maps are built on the host in double; keep the host compiler from contracting them to FMA
     "rectify_kernels.cu": ["-Xcompiler", "-ffp-contract=off"],
     "pnp_kernels.cu": [],
+    "essential_kernels.cu": [],
     # the pose-graph Jacobian is a central difference at delta 1e-9: no contraction on either side, as in tests/pgo_oracle.c
     "pgo_kernels.cu": ["-fmad=false", "-Xcompiler", "-ffp-contract=off"],
     # the transform optimiser's Jacobian is the same central difference (tests/transform_oracle.c)

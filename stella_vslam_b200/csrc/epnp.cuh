@@ -6,7 +6,8 @@
 //   HouseholderQR<6 x 4>::solve (gauss_newton).
 // fp64 with explicit round-to-nearest intrinsics, sums left to right in index order: operation for operation the CPU restatement
 // tests/pnp_oracle.c.  Eigen's vectorised reductions are not reproduced (DESIGN.md section 8).  One thread runs one problem; the
-// 12 x 12 work matrices live in the thread's local memory (L1-resident).
+// 12 x 12 work matrices live in the thread's local memory (L1-resident).  The out-of-line functions have internal linkage, so more than
+// one translation unit can include this header (essential_kernels.cu uses its SVD and Householder pieces).
 #pragma once
 
 #include "jacobi.cuh"
@@ -24,7 +25,7 @@ __device__ __forceinline__ double dot3(const double* a, const double* b) { retur
 // Sweeps of JacobiSVD on the n x n row-major W; U has m rows (row-major, stride m; columns p, q rotated), V is n x n or null.  Then
 // the singular values (scaled back), the sign flip of U's columns and the descending sort.  Returns the number of nonzero singular
 // values, or -1 when the sweeps did not converge.
-__device__ __noinline__ int svd_core(int n, double* W, int m, double* U, double* V, double scale, double* sv) {
+static __device__ __noinline__ int svd_core(int n, double* W, int m, double* U, double* V, double scale, double* sv) {
     double max_diag = 0.0;
     for (int i = 0; i < n; ++i)
         if (fabs(W[i * n + i]) > max_diag || i == 0) max_diag = fabs(W[i * n + i]);
@@ -154,7 +155,7 @@ __device__ __forceinline__ double col_norm(const double* A, int ld, int r0, int 
 }
 
 // JacobiSVD<MatX_t>(A (6 x k row-major), ComputeFullU | ComputeFullV).solve(rhs).  Returns the rank, or -1 (no convergence).
-__device__ __noinline__ int svd_solve_6xk(int k, const double* A, const double* rhs, double* x) {
+static __device__ __noinline__ int svd_solve_6xk(int k, const double* A, const double* rhs, double* x) {
     double S[30], U[36], W[25], V[25], sv[5], htau[5], cn_upd[5], cn_dir[5];
     int perm[5];
     const double scale = max_abs_or_one(A, 6 * k);
@@ -279,7 +280,7 @@ __device__ __forceinline__ double pcs_coord(const double a[4], const double ccs[
 }
 
 // estimate_R_and_t, with compute_pcs' local points rebuilt on the fly from the alphas and ccs (flip = -1 inverts them)
-__device__ __noinline__ int estimate_R_and_t(const Pts& s, const Basis& E, const double (&ccs)[4][3], double flip, double* R, double* t) {
+static __device__ __noinline__ int estimate_R_and_t(const Pts& s, const Basis& E, const double (&ccs)[4][3], double flip, double* R, double* t) {
     const int n = s.n;
     double pc0[3] = {0, 0, 0}, pw0[3] = {0, 0, 0};
     for (int j = 0; j < n; ++j) {
@@ -371,7 +372,7 @@ __device__ __forceinline__ void find_initial_betas(const double* L, const double
     betas[3] = 0.0;
 }
 
-__device__ __noinline__ void gauss_newton(const double* L, const double* rho, double* betas, unsigned num_iter) {
+static __device__ __noinline__ void gauss_newton(const double* L, const double* rho, double* betas, unsigned num_iter) {
     for (unsigned it = 0; it < num_iter; ++it) {
         double A[24], B[6], x[4];
         const double* b = betas;
@@ -400,7 +401,7 @@ __device__ __noinline__ void gauss_newton(const double* L, const double* rho, do
 
 // pnp_solver::compute_pose.  R, t are written only when a candidate N has reproj_error < the running minimum (from DBL_MAX); `wrote`
 // says whether they were.  Returns the minimum; status = -1 when an SVD did not converge.
-__device__ __noinline__ double compute_pose(const Pts& s, unsigned num_iter, double* R, double* t, bool& wrote, int& status) {
+static __device__ __noinline__ double compute_pose(const Pts& s, unsigned num_iter, double* R, double* t, bool& wrote, int& status) {
     const int n = s.n;
     Basis E;
     wrote = false;

@@ -1,0 +1,322 @@
+// essential_kernels.cu -- solve::essential_solver (src/stella_vslam/solve/essential_solver.cc) on the device: find_via_ransac with the
+// five-point minimal set for many problems in one launch sequence on the b200_lba_t handle's stream, and the host-side restatement of
+// util::create_random_array for any set size.
+//
+// find_via_ransac is split in three launches:
+//   essential_hypothesis_kernel  one thread per (problem, iteration): compute_E_21_minimal on the minimal set (essential_core.h),
+//                                up to ten candidates written to scratch in eigenvalue order;
+//   essential_score_kernel       one thread per (problem, iteration, candidate slot): check_inliers, the float cost accumulated over
+//                                the matches in ascending order (a tree sum could change which candidate wins);
+//   essential_select_kernel      one thread per problem: the first-wins selection in (iteration, candidate) order
+//                                (num_inliers > min_set_size and best_cost > cost), the winner's inlier flags and, with recompute and
+//                                at least 8 inliers, compute_E_21_nonminimal over the inliers and check_inliers again.
+// The arithmetic is fp64 with explicit round-to-nearest intrinsics; tests/essential_oracle.c compiles the same essential_core.h as C.
+#include <cfloat>
+#include <climits>
+#include <cmath>
+#include <cstring>
+#include <vector>
+
+#include "common.cuh"
+#include "epnp.cuh"
+#include "util_trig.cuh"
+
+namespace b200 {
+namespace lba {
+int borrow_buffers(b200_lba_t h, size_t dev_bytes, size_t host_bytes, cudaStream_t* stream, unsigned char** d, unsigned char** hst);
+}
+namespace pnp {
+uint32_t uniform_below(b200_mt19937_t* e, uint32_t range);
+}
+
+namespace ess {
+
+using pnp::apply_householder_left;
+using pnp::svd_core;
+using tri::da;
+using tri::dd;
+using tri::dm;
+using tri::ds;
+
+#define ES_FN __device__
+#define ES_BIG __device__ __noinline__
+#define ES_SQRT(x) __dsqrt_rn(x)
+#define ES_MAKE_HOUSEHOLDER(v, len, stride, tau, beta) pnp::make_householder((v), (len), (stride), (tau), (beta))
+#include "essential_core.h"
+#undef ES_FN
+#undef ES_BIG
+#undef ES_SQRT
+#undef ES_MAKE_HOUSEHOLDER
+
+constexpr int kMinSet = 5;
+constexpr int kMaxCand = 10;
+
+struct ProblemDev {
+    int n;          // matches
+    int match_off;  // first row in the concatenated bearings / flags
+    int hyp_off;    // first iteration in the concatenated minimal sets
+    int n_hyp;      // max_num_iter (0 on the early return)
+    int runs;       // 0: find_via_ransac returns before drawing (n < min_set_size)
+    int recompute;
+};
+
+struct HypDev {
+    int count;  // candidates written
+    int flags;  // ES_STATUS_* bits
+};
+
+struct ScoreDev {
+    float cost;
+    unsigned num_inliers;
+};
+
+struct ResultDev {
+    double E[9];
+    float best_cost;
+    int valid, best_iter, best_candidate, num_inliers, status;
+};
+
+__global__ void __launch_bounds__(32) essential_hypothesis_kernel(int n_hyp_total, const int* __restrict__ hyp_problem,
+                                                                   const ProblemDev* __restrict__ probs, const double* __restrict__ b1,
+                                                                   const double* __restrict__ b2, const int32_t* __restrict__ min_sets,
+                                                                   double* __restrict__ cand, HypDev* __restrict__ hyps) {
+    const int h = blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= n_hyp_total) return;
+    const ProblemDev P = probs[hyp_problem[h]];
+    HypDev out;
+    out.flags = 0;
+    out.count = es_minimal(b1 + 3 * (size_t)P.match_off, b2 + 3 * (size_t)P.match_off, min_sets + kMinSet * (size_t)h,
+                           cand + 9 * kMaxCand * (size_t)h, &out.flags);
+    hyps[h] = out;
+}
+
+__global__ void __launch_bounds__(64) essential_score_kernel(long long n_slots, const int* __restrict__ hyp_problem,
+                                                              const ProblemDev* __restrict__ probs, const double* __restrict__ b1,
+                                                              const double* __restrict__ b2, const double* __restrict__ cand,
+                                                              const HypDev* __restrict__ hyps, ScoreDev* __restrict__ scores) {
+    const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_slots) return;
+    const long long h = s / kMaxCand;
+    if ((int)(s - h * kMaxCand) >= hyps[h].count) return;
+    const ProblemDev P = probs[hyp_problem[h]];
+    ScoreDev out;
+    out.num_inliers = es_check_inliers(b1 + 3 * (size_t)P.match_off, b2 + 3 * (size_t)P.match_off, P.n, cand + 9 * (size_t)s,
+                                       es_cos_angle_thr(), nullptr, &out.cost);
+    scores[s] = out;
+}
+
+__global__ void __launch_bounds__(64) essential_select_kernel(int n_problems, const ProblemDev* __restrict__ probs,
+                                                              const double* __restrict__ b1, const double* __restrict__ b2,
+                                                              const double* __restrict__ cand, const HypDev* __restrict__ hyps,
+                                                              const ScoreDev* __restrict__ scores, int32_t* __restrict__ idx_scratch,
+                                                              double* __restrict__ mat_scratch, uint8_t* __restrict__ flags,
+                                                              ResultDev* __restrict__ results) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= n_problems) return;
+    const ProblemDev P = probs[q];
+    ResultDev r;
+    r.valid = 0;
+    r.best_iter = -1;
+    r.best_candidate = -1;
+    r.num_inliers = 0;
+    r.best_cost = 0.0f;  // the member's initial value, kept on the early return
+    r.status = 0;
+    if (!P.runs) {
+        results[q] = r;
+        return;
+    }
+    r.best_cost = FLT_MAX;
+    for (int it = 0; it < P.n_hyp; ++it) {
+        const HypDev H = hyps[P.hyp_off + it];
+        r.status |= H.flags & (ES_STATUS_SCHUR | ES_STATUS_SVD);
+        for (int k = 0; k < H.count; ++k) {
+            const ScoreDev S = scores[(size_t)(P.hyp_off + it) * kMaxCand + k];
+            if (S.num_inliers > (unsigned)kMinSet && r.best_cost > S.cost) {
+                r.best_cost = S.cost;
+                r.best_iter = it;
+                r.best_candidate = k;
+                r.num_inliers = (int)S.num_inliers;
+            }
+        }
+    }
+    r.valid = r.best_cost < FLT_MAX;
+    const double* pb1 = b1 + 3 * (size_t)P.match_off;
+    const double* pb2 = b2 + 3 * (size_t)P.match_off;
+    uint8_t* fl = flags + P.match_off;
+    if (!r.valid) {
+        for (int j = 0; j < P.n; ++j) fl[j] = 0;
+        results[q] = r;
+        return;
+    }
+    const double* W = cand + 9 * ((size_t)(P.hyp_off + r.best_iter) * kMaxCand + r.best_candidate);
+    for (int k = 0; k < 9; ++k) r.E[k] = W[k];
+    const float thr = es_cos_angle_thr();
+    float cost;
+    es_check_inliers(pb1, pb2, P.n, r.E, thr, fl, &cost);
+    if (P.recompute && r.num_inliers >= 8) {
+        int32_t* idx = idx_scratch + P.match_off;
+        int m = 0;
+        for (int j = 0; j < P.n; ++j)
+            if (fl[j]) idx[m++] = j;
+        r.status |= es_nonminimal(pb1, pb2, idx, m, mat_scratch + 9 * (size_t)P.match_off, r.E);
+        es_check_inliers(pb1, pb2, P.n, r.E, thr, fl, &r.best_cost);
+    }
+    results[q] = r;
+}
+
+// util::create_random_array(set_size, 0, n - 1, engine) as libstdc++ evaluates it: make_size = size_t(set_size * 1.2) draws of
+// uniform_int_distribution<unsigned>, sort + unique (truncated to set_size), repeated until set_size remain, then std::shuffle.
+void create_random_array(b200_mt19937_t* e, uint32_t set_size, uint32_t n, uint32_t* v, int32_t* out) {
+    const size_t make_size = (size_t)(set_size * 1.2);
+    size_t size = 0;
+    while (size != set_size) {
+        while (size < make_size) v[size++] = pnp::uniform_below(e, n);
+        for (size_t i = 1; i < size; ++i)
+            for (size_t j = i; j > 0 && v[j - 1] > v[j]; --j) {
+                const uint32_t t = v[j];
+                v[j] = v[j - 1];
+                v[j - 1] = t;
+            }
+        size_t u = 0;
+        for (size_t i = 0; i < size; ++i)
+            if (u == 0 || v[u - 1] != v[i]) v[u++] = v[i];
+        size = u < set_size ? u : set_size;
+    }
+    // std::shuffle: with a 32-bit engine and set_size^2 <= 2^32 - 1, swap positions come in pairs from one draw
+    uint32_t t;
+    size_t i = 1;
+    if (set_size % 2 == 0) {
+        const uint32_t d = pnp::uniform_below(e, 2);
+        t = v[i], v[i] = v[d], v[d] = t;
+        ++i;
+    }
+    while (i < set_size) {
+        const uint32_t r = (uint32_t)i + 1;
+        const uint32_t x = pnp::uniform_below(e, r * (r + 1));
+        t = v[i], v[i] = v[x / (r + 1)], v[x / (r + 1)] = t;
+        ++i;
+        t = v[i], v[i] = v[x % (r + 1)], v[x % (r + 1)] = t;
+        ++i;
+    }
+    for (uint32_t k = 0; k < set_size; ++k) out[k] = (int32_t)v[k];
+}
+
+}  // namespace ess
+}  // namespace b200
+
+extern "C" {
+
+int b200_draw_min_sets(b200_mt19937_t* e, uint32_t set_size, uint32_t n_matches, uint32_t max_num_iter, int32_t* out) {
+    // set_size <= 65535 keeps set_size^2 within the engine's range (the paired shuffle) and the products below in 32 bits
+    if (!e || set_size < 1 || set_size > 65535u || n_matches < set_size || (max_num_iter > 0 && !out)) return B200_ERR_INVALID;
+    std::vector<uint32_t> v((size_t)(set_size * 1.2) + set_size);
+    for (uint32_t it = 0; it < max_num_iter; ++it) b200::ess::create_random_array(e, set_size, n_matches, v.data(), out + (size_t)set_size * it);
+    return B200_OK;
+}
+
+int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t* problems) {
+    B200_RANGE("b200:essential:ransac");
+    using namespace b200::ess;
+    if (!h || n_problems < 0) return B200_ERR_INVALID;
+    if (n_problems == 0) return B200_OK;
+    if (!problems) return B200_ERR_INVALID;
+    std::vector<ProblemDev> pd(n_problems);
+    long long total = 0, total_hyp = 0;
+    for (int q = 0; q < n_problems; ++q) {
+        const b200_essential_problem_t& P = problems[q];
+        const int n = P.n_matches;
+        if (P.min_set_size != (uint32_t)kMinSet) {
+            b200::set_error("b200_essential_ransac: problem %d: min_set_size %u (only the five-point minimal set is supported)", q, P.min_set_size);
+            return B200_ERR_INVALID;
+        }
+        if (n < 0 || (n > 0 && (!P.bearings_1 || !P.bearings_2 || !P.inlier_flags))) {
+            b200::set_error("b200_essential_ransac: problem %d: negative count or null buffer", q);
+            return B200_ERR_INVALID;
+        }
+        const bool runs = n >= kMinSet;
+        const int n_hyp = runs ? (int)P.max_num_iter : 0;
+        if (runs && (P.max_num_iter > (uint32_t)INT_MAX || (n_hyp > 0 && !P.min_sets))) {
+            b200::set_error("b200_essential_ransac: problem %d: bad max_num_iter or null min_sets", q);
+            return B200_ERR_INVALID;
+        }
+        for (long long k = 0; k < (long long)kMinSet * n_hyp; ++k)
+            if (P.min_sets[k] < 0 || P.min_sets[k] >= n) {
+                b200::set_error("b200_essential_ransac: problem %d: min_sets entry %lld = %d outside [0, %d)", q, k, P.min_sets[k], n);
+                return B200_ERR_INVALID;
+            }
+        pd[q] = ProblemDev{n, (int)total, (int)total_hyp, n_hyp, runs, P.recompute != 0};
+        total += n;
+        total_hyp += n_hyp;
+        if (total > INT_MAX / 16 || total_hyp > INT_MAX / 16) {
+            b200::set_error("b200_essential_ransac: too many matches or iterations in one call");
+            return B200_ERR_INVALID;
+        }
+    }
+    const size_t T = (size_t)std::max(total, 1LL), NH = (size_t)std::max(total_hyp, 1LL);
+    auto al = [](size_t& o, size_t bytes) {
+        const size_t r = o;
+        o = b200::round_up(o + bytes, (size_t)256);
+        return r;
+    };
+    size_t o = 0;
+    const size_t o_probs = al(o, sizeof(ProblemDev) * n_problems), o_b1 = al(o, 24 * T), o_b2 = al(o, 24 * T);
+    const size_t o_ms = al(o, 4 * kMinSet * NH), o_hp = al(o, 4 * NH);
+    const size_t in_bytes = o;
+    const size_t o_res = al(o, sizeof(ResultDev) * n_problems), o_fl = al(o, T);
+    const size_t out_end = o;
+    const size_t o_cand = al(o, 8 * 9 * kMaxCand * NH), o_hyp = al(o, sizeof(HypDev) * NH), o_sc = al(o, sizeof(ScoreDev) * kMaxCand * NH);
+    const size_t o_idx = al(o, 4 * T), o_mat = al(o, 72 * T);
+    cudaStream_t st;
+    unsigned char *db, *hb;
+    int rc = b200::lba::borrow_buffers(h, o, out_end, &st, &db, &hb);
+    if (rc) return rc;
+    std::memcpy(hb + o_probs, pd.data(), sizeof(ProblemDev) * n_problems);
+    int* hyp_problem = reinterpret_cast<int*>(hb + o_hp);
+    for (int q = 0; q < n_problems; ++q) {
+        const b200_essential_problem_t& P = problems[q];
+        const size_t off = (size_t)pd[q].match_off, n = (size_t)P.n_matches;
+        if (n) {
+            std::memcpy(hb + o_b1 + 24 * off, P.bearings_1, 24 * n);
+            std::memcpy(hb + o_b2 + 24 * off, P.bearings_2, 24 * n);
+        }
+        if (pd[q].n_hyp) std::memcpy(hb + o_ms + 4 * kMinSet * (size_t)pd[q].hyp_off, P.min_sets, 4 * kMinSet * (size_t)pd[q].n_hyp);
+        for (int k = 0; k < pd[q].n_hyp; ++k) hyp_problem[pd[q].hyp_off + k] = q;
+    }
+    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    const double* d_b1 = (const double*)(db + o_b1);
+    const double* d_b2 = (const double*)(db + o_b2);
+    if (total_hyp > 0) {
+        // 32-thread blocks: one problem of 1 000 iterations spreads over 32 SMs rather than 8 (the tracker's fallback is one problem)
+        essential_hypothesis_kernel<<<b200::ceil_div((int)total_hyp, 32), 32, 0, st>>>(
+            (int)total_hyp, (const int*)(db + o_hp), (const ProblemDev*)(db + o_probs), d_b1, d_b2, (const int32_t*)(db + o_ms),
+            (double*)(db + o_cand), (HypDev*)(db + o_hyp));
+        B200_CUDA(cudaGetLastError());
+        const long long slots = total_hyp * kMaxCand;
+        essential_score_kernel<<<(unsigned)((slots + 63) / 64), 64, 0, st>>>(slots, (const int*)(db + o_hp), (const ProblemDev*)(db + o_probs),
+                                                                                d_b1, d_b2, (const double*)(db + o_cand),
+                                                                                (const HypDev*)(db + o_hyp), (ScoreDev*)(db + o_sc));
+        B200_CUDA(cudaGetLastError());
+    }
+    essential_select_kernel<<<b200::ceil_div(n_problems, 64), 64, 0, st>>>(
+        n_problems, (const ProblemDev*)(db + o_probs), d_b1, d_b2, (const double*)(db + o_cand), (const HypDev*)(db + o_hyp),
+        (const ScoreDev*)(db + o_sc), (int32_t*)(db + o_idx), (double*)(db + o_mat), db + o_fl, (ResultDev*)(db + o_res));
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaMemcpyAsync(hb + o_res, db + o_res, out_end - o_res, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    const ResultDev* res = reinterpret_cast<const ResultDev*>(hb + o_res);
+    for (int q = 0; q < n_problems; ++q) {
+        b200_essential_problem_t& P = problems[q];
+        const ResultDev& r = res[q];
+        P.status = r.status ? B200_ERR_INVALID : B200_OK;
+        P.valid = r.valid;
+        P.best_iter = r.best_iter;
+        P.best_candidate = r.best_candidate;
+        P.num_inliers = r.num_inliers;
+        P.best_cost = r.best_cost;
+        if (r.valid) std::memcpy(P.E_21, r.E, sizeof r.E);
+        if (pd[q].runs) std::memcpy(P.inlier_flags, hb + o_fl + pd[q].match_off, (size_t)P.n_matches);
+    }
+    return B200_OK;
+}
+
+}  // extern "C"

@@ -1,8 +1,11 @@
-"""Host-side mirror of solve::pnp_solver (src/stella_vslam/solve/pnp_solver.{h,cc}): EPnP inside RANSAC on the device
+"""Host-side mirrors of solve::pnp_solver (src/stella_vslam/solve/pnp_solver.{h,cc}): EPnP inside RANSAC on the device
 (b200_pnp_ransac / b200_epnp_compute_pose on a b200_lba_t handle), with the minimal sets drawn on the host exactly as
 util::create_random_array draws them from the solver's std::mt19937 (b200_pnp_draw_min_sets).
 
 Arrays: bearings and points are (n, 3) float64, octaves (n,) int, scale_factors the ORB pyramid's float32 scale factors.
+
+And of solve::essential_solver (src/stella_vslam/solve/essential_solver.{h,cc}): the five-point minimal solver inside RANSAC on the
+device (b200_essential_ransac), the minimal sets drawn on the host by util::create_random_array(5, ...) (b200_draw_min_sets).
 """
 import ctypes as C
 
@@ -27,6 +30,14 @@ class EpnpProblem(C.Structure):
                 ("status", C.c_int32)]
 
 
+class EssentialProblem(C.Structure):
+    """b200_essential_problem_t (include/b200vslam.h)."""
+    _fields_ = [("n_matches", C.c_int32), ("bearings_1", C.c_void_p), ("bearings_2", C.c_void_p), ("min_set_size", C.c_uint32),
+                ("max_num_iter", C.c_uint32), ("recompute", C.c_int32), ("min_sets", C.c_void_p),
+                ("status", C.c_int32), ("valid", C.c_int32), ("best_iter", C.c_int32), ("best_candidate", C.c_int32),
+                ("num_inliers", C.c_int32), ("best_cost", C.c_float), ("E_21", C.c_double * 9), ("inlier_flags", C.c_void_p)]
+
+
 class Mt19937(C.Structure):
     """b200_mt19937_t: std::mt19937's state."""
     _fields_ = [("state", C.c_uint32 * 624), ("index", C.c_uint32)]
@@ -43,6 +54,8 @@ def _L():
         L.b200_mt19937_next.argtypes = [C.POINTER(Mt19937)]
         L.b200_mt19937_next.restype = C.c_uint32
         L.b200_pnp_draw_min_sets.argtypes = [C.POINTER(Mt19937), C.c_uint32, C.c_uint32, C.POINTER(C.c_int32)]
+        L.b200_draw_min_sets.argtypes = [C.POINTER(Mt19937), C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_int32)]
+        L.b200_essential_ransac.argtypes = [vp, C.c_int, C.POINTER(EssentialProblem)]
         L._pnp_bound = True
     return L
 
@@ -67,12 +80,17 @@ def mt19937(seed_seq=None):
     return e
 
 
-def draw_min_sets(n_matches, max_num_iter, engine=None):
-    """max_num_iter calls of util::create_random_array(4, 0, n_matches - 1, engine), (max_num_iter, 4) int32.  engine: an Mt19937
-    (advanced in place) or None for a default-constructed one."""
+def draw_min_sets(n_matches, max_num_iter, engine=None, set_size=4):
+    """max_num_iter calls of util::create_random_array(set_size, 0, n_matches - 1, engine), (max_num_iter, set_size) int32.  engine: an
+    Mt19937 (advanced in place) or None for a default-constructed one.  set_size 4 is PnP's minimal set, 5 the essential solver's."""
     e = mt19937() if engine is None else engine
-    out = np.zeros((max(int(max_num_iter), 1), 4), np.int32)
-    check(_L().b200_pnp_draw_min_sets(C.byref(e), int(n_matches), int(max_num_iter), out.ctypes.data_as(C.POINTER(C.c_int32))))
+    k = int(set_size)
+    out = np.zeros((max(int(max_num_iter), 1), max(k, 1)), np.int32)
+    ptr = out.ctypes.data_as(C.POINTER(C.c_int32))
+    if k == 4:
+        check(_L().b200_pnp_draw_min_sets(C.byref(e), int(n_matches), int(max_num_iter), ptr))
+    else:
+        check(_L().b200_draw_min_sets(C.byref(e), k, int(n_matches), int(max_num_iter), ptr))
     return out[:int(max_num_iter)]
 
 
@@ -199,3 +217,94 @@ class pnp_solver:
         r = compute_pose_batch([dict(bearings=bearing_vectors, points=pos_ws, num_iter=num_iter, rot_cw=rot_cw, trans_cw=trans_cw)], device)[0]
         check(r["status"])
         return r["reproj_error"], r["rot_cw"], r["trans_cw"]
+
+
+def _pack_essential(prob, keep):
+    S = EssentialProblem()
+    b1 = np.ascontiguousarray(np.asarray(prob["bearings_1"], np.float64).reshape(-1, 3))
+    b2 = np.ascontiguousarray(np.asarray(prob["bearings_2"], np.float64).reshape(-1, 3))
+    if len(b1) != len(b2):
+        raise ValueError("bearings_1 and bearings_2 must have one row per match")
+    k = int(prob.get("min_set_size", 5))
+    ms = np.ascontiguousarray(np.asarray(prob.get("min_sets", np.zeros((0, k))), np.int32).reshape(-1, max(k, 1)))
+    fl = np.zeros(max(len(b1), 1), np.uint8)
+    keep += [b1, b2, ms, fl]
+    S.n_matches = len(b1)
+    S.bearings_1, S.bearings_2 = b1.ctypes.data, b2.ctypes.data
+    S.min_set_size = k
+    S.max_num_iter = len(ms)
+    S.recompute = int(bool(prob.get("recompute", True)))
+    S.min_sets = ms.ctypes.data
+    S.inlier_flags = fl.ctypes.data
+    return S, fl
+
+
+def essential_ransac_batch(problems, device=0):
+    """b200_essential_ransac over dicts(bearings_1, bearings_2 (n x 3, gathered through matches_12), min_sets (max_num_iter x 5),
+    recompute=True, min_set_size=5).  Returns per problem dict(status, valid, best_iter, best_candidate, num_inliers, best_cost (float32),
+    E_21 (None unless valid), inlier_flags (None on the early return))."""
+    keep, flags = [], []
+    arr = (EssentialProblem * max(len(problems), 1))()
+    for i, pr in enumerate(problems):
+        arr[i], fl = _pack_essential(pr, keep)
+        flags.append(fl)
+    check(_L().b200_essential_ransac(_handle(device), len(problems), arr))
+    out = []
+    for i in range(len(problems)):
+        S, n = arr[i], arr[i].n_matches
+        out.append(dict(status=S.status, valid=bool(S.valid), best_iter=S.best_iter, best_candidate=S.best_candidate,
+                        num_inliers=S.num_inliers, best_cost=np.float32(S.best_cost),
+                        E_21=np.array(S.E_21).reshape(3, 3) if S.valid else None,
+                        inlier_flags=None if n < S.min_set_size else flags[i][:n].astype(bool)))
+    return out
+
+
+class essential_solver:
+    """solve::essential_solver.  matches_12: (first, second) index pairs into bearings_1 / bearings_2.  The engine is the solver's
+    member: find_via_ransac continues its state across calls."""
+
+    def __init__(self, bearings_1, bearings_2, matches_12, use_fixed_seed=False, device=0):
+        b1 = np.asarray(bearings_1, np.float64).reshape(-1, 3)
+        b2 = np.asarray(bearings_2, np.float64).reshape(-1, 3)
+        m = np.asarray(matches_12, np.int64).reshape(-1, 2)
+        if len(m) and (m.min() < 0 or m[:, 0].max() >= len(b1) or m[:, 1].max() >= len(b2)):
+            raise IndexError("match index outside the bearings")  # std::vector::at throws in the reference
+        self.bearings_1_ = np.ascontiguousarray(b1[m[:, 0]])
+        self.bearings_2_ = np.ascontiguousarray(b2[m[:, 1]])
+        self.num_matches_ = len(m)
+        self.device = device
+        self.random_engine_ = mt19937(None if use_fixed_seed else np.frombuffer(np.random.bytes(40), np.uint32))
+        self.solution_is_valid_ = False
+        self.best_cost_ = np.float32(0.0)
+        self.best_E_21_ = np.zeros((3, 3))
+        self.is_inlier_match_ = []
+        self.status_ = 0
+
+    def find_via_ransac(self, max_num_iter, recompute=True, min_set_size=5):
+        if int(min_set_size) != 5:
+            raise ValueError("essential_solver: only the five-point minimal set (min_set_size = 5) is supported")
+        n = self.num_matches_
+        if n < min_set_size:
+            self.solution_is_valid_ = False
+            return
+        ms = draw_min_sets(n, max_num_iter, self.random_engine_, set_size=5)
+        r = essential_ransac_batch([dict(bearings_1=self.bearings_1_, bearings_2=self.bearings_2_, min_sets=ms, recompute=recompute)],
+                                   self.device)[0]
+        self.status_ = r["status"]
+        self.solution_is_valid_ = r["valid"]
+        self.best_cost_ = r["best_cost"]
+        if r["valid"]:
+            self.best_E_21_ = r["E_21"]
+        self.is_inlier_match_ = [bool(v) for v in r["inlier_flags"]]
+
+    def solution_is_valid(self):
+        return self.solution_is_valid_
+
+    def get_best_cost(self):
+        return self.best_cost_
+
+    def get_best_E_21(self):
+        return self.best_E_21_.copy()
+
+    def get_inlier_matches(self):
+        return list(self.is_inlier_match_)

@@ -339,7 +339,8 @@ def make_keyframe_pair(seed, n1=2000, n2=2000, stereo=False, n_nodes=150, num_le
     """Two keyframes looking at the same synthetic points, for the all-pairs matchers with greedy state (bow_tree::*,
     robust::match_for_triangulation).  Returns (keyfrm_1, keyfrm_2, geometry): dicts with desc, angle, octave, bearings (unit,
     f64), node (BoW node id), no_landmark / has_landmark (u8), stereo (u8 | None), scale_factors; geometry holds E_12 with
-    bearing_1 . (E_12 bearing_2) = 0 for true correspondences, the epipole of keyframe 1 in keyframe 2, and the pair list.
+    bearing_1 . (E_12 bearing_2) = 0 for true correspondences, the epipole of keyframe 1 in keyframe 2, the pair list (perm1[k],
+    perm2[k]) and its mask `wrong` of the correspondences moved off their epipolar plane.
     Corresponding keypoints share descriptors up to noise of varied strength; some rows have two look-alike candidates (ratio
     test), some correspondences violate the epipolar constraint, some sit next to the epipole."""
     rng = np.random.default_rng(seed)
@@ -398,7 +399,8 @@ def make_keyframe_pair(seed, n1=2000, n2=2000, stereo=False, n_nodes=150, num_le
         return dict(desc=desc, angle=angle, octave=octave, bearings=np.ascontiguousarray(bearings), node=node, has_landmark=has_lm,
                     no_landmark=(1 - has_lm).astype(np.uint8), stereo=(rng.random(n) < 0.4).astype(np.uint8) if stereo else None, scale_factors=sf)
 
-    geometry = dict(E_12=E_12, epiplane_in_keyfrm_2=c1_in_2 / np.linalg.norm(c1_in_2), valid_epiplane=True, perm1=perm1, perm2=perm2)
+    geometry = dict(E_12=E_12, epiplane_in_keyfrm_2=c1_in_2 / np.linalg.norm(c1_in_2), valid_epiplane=True, perm1=perm1, perm2=perm2,
+                    wrong=wrong)
     return kf(desc1, angle1, octave1, bearings1, node1, has_lm1, n1), kf(desc2, angle2, octave2, bearings2, node2, has_lm2, n2), geometry
 
 
@@ -748,6 +750,66 @@ def make_pnp_problem(seed=0, n=300, inlier_frac=0.5, model="perspective", case=N
         o[~far] = turned[~far]
         bear[out] = o
     return dict(bearings=bear, points=pw, octaves=octaves, scale_factors=sf, gt_rot_cw=Rcw, gt_trans_cw=tcw, gt_inlier=inl)
+
+
+def make_essential_problem(seed=0, n=500, inlier_frac=0.6, model="perspective", case=None, noise=5e-4):
+    """Matched bearings of two views for solve::essential_solver: a true R_21 / t_21 (unit translation), points at 2-30 m, inlier
+    bearings of view 2 turned off their true ray by up to `noise` rad, outliers with view-2 bearings at least 3 deg away from their
+    epipolar plane.  model: "perspective" (z > 0, KITTI frustum) or "equirect" (all directions, backward bearings included).
+    case: None; "pure_rotation" (|t_21| = 1e-4 m); "planar" (all points on one plane); "duplicated" (a fifth of the matches are copies
+    of others, so minimal sets with repeated bearings occur); "n5" (five noise-free inliers); "inliers8" / "inliers9" / "inliers10"
+    (exactly 8, 9 or 10 noise-free inliers among 10, 11 or 14 matches, so RANSAC keeps exactly that many).
+    Returns dict(bearings_1, bearings_2 (n x 3, in match order), E_21 (= [t_21]x R_21), R_21, t_21, gt_inlier)."""
+    rng = np.random.default_rng(seed)
+    equirect = model == "equirect"
+    fixed = {"n5": (5, 5), "inliers8": (10, 8), "inliers9": (11, 9), "inliers10": (14, 10)}
+    if case in fixed:
+        n, n_in = fixed[case]
+        noise = 0.0
+    else:
+        n_in = int(round(inlier_frac * n))
+    R = _rodrigues(0.15 * rng.standard_normal(3))
+    t = rng.standard_normal(3)
+    t /= np.linalg.norm(t)
+    if case == "pure_rotation":
+        t *= 1e-4
+    depth = rng.uniform(2, 30, n)
+    if equirect:
+        d = rng.standard_normal((n, 3))
+        P = d / np.linalg.norm(d, axis=1, keepdims=True) * depth[:, None]
+    else:
+        u, v = rng.uniform(20, KITTI["cols"] - 20, n), rng.uniform(20, KITTI["rows"] - 20, n)
+        P = np.stack([(u - KITTI["cx"]) / KITTI["fx"] * depth, (v - KITTI["cy"]) / KITTI["fy"] * depth, depth], 1)
+    if case == "planar":  # the plane z = 8 + 0.2 x - 0.1 y (perspective) or x = 4 + 0.3 z (equirect)
+        if equirect:
+            P[:, 0] = 4.0 + 0.3 * P[:, 2]
+        else:
+            P[:, 2] = 8.0 + 0.2 * P[:, 0] - 0.1 * P[:, 1]
+    unit = lambda a: a / np.linalg.norm(a, axis=-1, keepdims=True)
+    b1 = unit(P)
+    b2 = unit(P @ R.T + t)
+    tx = np.array([[0, -t[2], t[1]], [t[2], 0, -t[0]], [-t[1], t[0], 0]])
+    E = tx @ R
+    if noise > 0:
+        perp = unit(np.cross(b2, rng.standard_normal((n, 3))))
+        ang = rng.uniform(0, noise, n)
+        b2 = np.cos(ang)[:, None] * b2 + np.sin(ang)[:, None] * perp
+    inl = np.zeros(n, bool)
+    inl[rng.permutation(n)[:n_in]] = True
+    for j in np.flatnonzero(~inl):
+        nrm = unit(E @ b1[j])
+        while True:
+            o = rng.standard_normal(3) if equirect else np.array([(rng.uniform(20, KITTI["cols"] - 20) - KITTI["cx"]) / KITTI["fx"],
+                                                                   (rng.uniform(20, KITTI["rows"] - 20) - KITTI["cy"]) / KITTI["fy"], 1.0])
+            o = unit(o)
+            if abs(o @ nrm) > np.sin(np.deg2rad(3.0)):
+                break
+        b2[j] = o
+    if case == "duplicated":
+        k = n // 5
+        src, dst = rng.choice(n, k, replace=False), rng.choice(n, k, replace=False)
+        b1[dst], b2[dst], inl[dst] = b1[src], b2[src], inl[src]
+    return dict(bearings_1=np.ascontiguousarray(b1), bearings_2=np.ascontiguousarray(b2), E_21=E, R_21=R, t_21=t, gt_inlier=inl)
 
 
 def make_pose_graph(n_keyframes=500, seed=0, fix_scale=False, laps=1.5, window=8, rot_noise=2e-3, trans_noise=0.01, scale_noise=2e-3,
