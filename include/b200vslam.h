@@ -732,6 +732,44 @@ typedef struct b200_essential_problem {
  * outside [0, n) of a problem that runs RANSAC. */
 int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t* problems);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Monocular initialisation's two-view RANSAC: solve::homography_solver::find_via_ransac (src/stella_vslam/solve/homography_solver.cc)
+ * and solve::fundamental_solver::find_via_ransac (fundamental_solver.cc), with solve::normalize (solve/common.cc) over all keypoints of
+ * each frame, for many problems of either model in one launch sequence on the b200_lba_t handle's stream.  initialize::perspective
+ * runs one H and one F problem per attempt (recompute = false); both go into one call.  Float exactly where the reference stores
+ * float, fp64 elsewhere, in the CPU restatement's evaluation order (csrc/twoview_core.h).  Deviations (DESIGN.md section 8): sums run
+ * left to right (Eigen's vectorised reductions are not reproduced); Jacobi sweeps are bounded, and an H coefficient matrix whose sweeps
+ * hit the bound counts as degenerate and sets status.
+ * ---------------------------------------------------------------------------------------------------------------- */
+#define B200_TWOVIEW_H 0
+#define B200_TWOVIEW_F 1
+typedef struct b200_twoview_problem {
+    int32_t model;                  /* B200_TWOVIEW_H (minimal set 4) or B200_TWOVIEW_F (minimal set 8) */
+    int32_t n_keypts_1;             /* all undistorted keypoints of frame 1: normalize runs over every one, matched or not */
+    const float* keypts_1;          /* n_keypts_1 x 2: undist_keypts_1[i].pt (x, y) */
+    int32_t n_keypts_2;
+    const float* keypts_2;          /* n_keypts_2 x 2 */
+    int32_t n_matches;
+    const int32_t* matches_12;      /* n_matches x 2: (index into keypts_1, index into keypts_2) in the reference's order */
+    float sigma;                    /* initialize::perspective passes 1.0f */
+    uint32_t max_num_iter;          /* initialize::perspective: num_ransac_iterations (default 100) */
+    int32_t recompute;              /* find_via_ransac's recompute (initialize::perspective passes false) */
+    const int32_t* min_sets;        /* max_num_iter x (4 or 8): util::create_random_array's draws in draw order (b200_draw_min_sets) */
+    /* out */
+    int32_t status;                 /* B200_OK, or B200_ERR_INVALID when a Jacobi SVD hit its sweep bound */
+    int32_t valid;                  /* solution_is_valid() */
+    int32_t best_iter;              /* iteration of the RANSAC winner (-1 none) */
+    int32_t num_inliers;            /* of the RANSAC winner (before the recompute) */
+    float best_cost;                /* get_best_cost(): FLT_MAX when no winner; 0 on the early return (the member's initial value) */
+    double M_21[9];                 /* row-major get_best_H_21() / get_best_F_21(); written only when valid */
+    uint8_t* inlier_flags;          /* n_matches: get_inlier_matches(); all 0 when not valid; untouched on the early return (n < 8) */
+} b200_twoview_problem_t;
+/* find_via_ransac(max_num_iter, recompute) for every problem: one upload, the normalisation, hypothesis, scoring and selection
+ * launches, one download.  Early return (nothing drawn, flags untouched) when n_matches < 8 for either model.  B200_ERR_INVALID
+ * (nothing written) for a negative count, a null required pointer, a model other than H / F, a match index outside its frame's
+ * keypoints or a min_sets entry outside [0, n_matches) of a problem that runs RANSAC. */
+int b200_twoview_ransac(b200_lba_t h, int n_problems, b200_twoview_problem_t* problems);
+
 /* ----------------------------------------------------------------------------------------------------------------
  * Pose-graph optimisation (optimize::graph_optimizer, optimize/graph_optimizer.cc:254-302): the Sim3 essential graph of a loop
  * closure, g2o's Levenberg-Marquardt with numeric central-difference Jacobians (delta 1e-9) and the terminate action, on the handle's

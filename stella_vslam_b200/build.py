@@ -23,6 +23,7 @@ SOURCES = {
     "rectify_kernels.cu": ["-Xcompiler", "-ffp-contract=off"],
     "pnp_kernels.cu": [],
     "essential_kernels.cu": [],
+    "twoview_kernels.cu": [],
     # the pose-graph Jacobian is a central difference at delta 1e-9: no contraction on either side, as in tests/pgo_oracle.c
     "pgo_kernels.cu": ["-fmad=false", "-Xcompiler", "-ffp-contract=off"],
     # the transform optimiser's Jacobian is the same central difference (tests/transform_oracle.c)

@@ -755,23 +755,25 @@ ES_BIG void es_colpiv_qr(int rows, int cols, double* S, double* htau, int* perm)
     }
 }
 
-/* compute_E_21_nonminimal over the m >= 8 pairs idx[0..m-1]; S is m x 9 scratch.  Returns 0, or ES_STATUS_SVD. */
-ES_BIG int es_nonminimal(const double* b1, const double* b2, const int32_t* idx, int m, double* S, double* E) {
+/* The singular values of the wide path's 8 x 8 work matrix, R^T of the adjoint's QR (At: 9 x 8 after es_colpiv_qr).  U and V are not
+ * formed: the callers need neither.  Returns svd_core's count. */
+ES_BIG int es_wide_sv(const double* At, double scale, double* sv) {
+    double W[64];
+    for (int i = 0; i < 8; ++i)
+        for (int j = 0; j < 8; ++j) W[i * 8 + j] = j <= i ? At[j * 8 + i] : 0.0;
+    return svd_core(8, W, 0, NULL, NULL, scale, sv);
+}
+
+/* JacobiSVD<Matrix<double, Dynamic, 9>> (ComputeFullV) of the m x 9 S (row-major, m >= 8; overwritten on the tall path), scale its
+ * max |entry| (1 when all are zero): V's last column into v9.  With sv non-null also the min(m, 9) singular values in descending order
+ * and *nonzero, svd_core's count (m_nonzeroSingularValues; -1 when the sweeps hit their bound).  The wide path then also sweeps its
+ * 8 x 8 work matrix, which V's last column does not depend on.  Returns 0, or ES_STATUS_SVD.
+ *   wide (m = 8): ColPivHouseholderQR of the adjoint (9 x 8); V = its full Q, whose last column no sweep touches;
+ *   square (m = 9): no preconditioner;
+ *   tall (m >= 10): ColPivHouseholderQR; the work matrix is R, V the column permutation. */
+ES_BIG int es_svd_n9(int m, double* S, double scale, double* v9, double* sv, int* nonzero) {
     int status = 0;
-    double scale = 0.0;
-    for (int i = 0; i < m; ++i) {
-        const double* x1 = b1 + 3 * (size_t)idx[i];
-        const double* x2 = b2 + 3 * (size_t)idx[i];
-        for (int a = 0; a < 3; ++a)
-            for (int c = 0; c < 3; ++c) {
-                const double v = dm(x2[a], x1[c]);
-                S[(size_t)i * 9 + 3 * a + c] = v;
-                scale = es_max(scale, fabs(v));
-            }
-    }
-    if (scale == 0.0) scale = 1.0;
-    double v9[9];
-    if (m == 8) {  /* wide: ColPivHouseholderQR of the adjoint (9 x 8); V = its full Q, whose last column no sweep touches */
+    if (m == 8) {
         double At[72], htau[8], Q[81];
         int perm[8];
         for (int i = 0; i < 8; ++i)
@@ -780,14 +782,18 @@ ES_BIG int es_nonminimal(const double* b1, const double* b2, const int32_t* idx,
         for (int k = 0; k < 81; ++k) Q[k] = (k % 10 == 0) ? 1.0 : 0.0;
         for (int c = 7; c >= 0; --c) apply_householder_left(&Q[c * 9 + c], 9 - c, 9 - c, 9, &At[(c + 1) * 8 + c], 8, htau[c]);
         for (int r = 0; r < 9; ++r) v9[r] = Q[r * 9 + 8];
+        if (sv) {
+            *nonzero = es_wide_sv(At, scale, sv);
+            if (*nonzero < 0) status = ES_STATUS_SVD;
+        }
     } else {
-        double W[81], V[81], sv[9];
-        if (m == 9) {  /* square: no preconditioner */
+        double W[81], V[81], s9[9];
+        if (m == 9) {
             for (int k = 0; k < 81; ++k) {
                 W[k] = dd(S[k], scale);
                 V[k] = (k % 10 == 0) ? 1.0 : 0.0;
             }
-        } else {  /* tall: ColPivHouseholderQR; W = R, V = the column permutation */
+        } else {
             double htau[9];
             int perm[9];
             for (size_t k = 0; k < (size_t)m * 9; ++k) S[k] = dd(S[k], scale);
@@ -798,10 +804,31 @@ ES_BIG int es_nonminimal(const double* b1, const double* b2, const int32_t* idx,
                     V[i * 9 + j] = (i == perm[j]) ? 1.0 : 0.0;
                 }
         }
-        if (svd_core(9, W, 0, NULL, V, scale, sv) < 0) status = ES_STATUS_SVD;
+        const int nz = svd_core(9, W, 0, NULL, V, scale, s9);
+        if (nz < 0) status = ES_STATUS_SVD;
         for (int r = 0; r < 9; ++r) v9[r] = V[r * 9 + 8];
+        if (sv) {
+            for (int k = 0; k < 9; ++k) sv[k] = s9[k];
+            *nonzero = nz;
+        }
     }
-    /* init_E_21 = Mat33_t(v.data()).transpose(): row-major v; then JacobiSVD<Mat33_t>, lambda(2) = 0, U diag(lambda) V^T */
+    return status;
+}
+
+/* JacobiSVD::rank() at its default threshold: the singular values >= max(s0 * diag * eps, DBL_MIN), counted down from the last
+ * nonzero one (diag = min(rows, cols)).  A sweep that hit its bound (nonzero < 0) counts as rank 0. */
+ES_FN int es_svd_rank(int diag, const double* sv, int nonzero) {
+    if (nonzero <= 0) return 0;
+    const double thr = es_max(dm(sv[0], dm((double)diag, DBL_EPSILON)), DBL_MIN);
+    int i = nonzero - 1;
+    while (i >= 0 && sv[i] < thr) --i;
+    return i + 1;
+}
+
+/* Mat33_t(v.data()).transpose() (row-major v9), then JacobiSVD<Mat33_t>, lambda(2) = 0, U diag(lambda) V^T into E: the rank-2
+ * projection shared by compute_E_21_nonminimal and fundamental_solver::compute_F_21.  Returns 0, or ES_STATUS_SVD. */
+ES_BIG int es_rank2(const double* v9, double* E) {
+    int status = 0;
     double W3[9], U3[9], V3[9], s3[3];
     double sc = 0.0;
     for (int k = 0; k < 9; ++k) sc = es_max(sc, fabs(v9[k]));
@@ -816,5 +843,25 @@ ES_BIG int es_nonminimal(const double* b1, const double* b2, const int32_t* idx,
         for (int c = 0; c < 3; ++c)
             E[r * 3 + c] = da(da(dm(dm(U3[r * 3], s3[0]), V3[c * 3]), dm(dm(U3[r * 3 + 1], s3[1]), V3[c * 3 + 1])),
                               dm(dm(U3[r * 3 + 2], s3[2]), V3[c * 3 + 2]));
+    return status;
+}
+
+/* compute_E_21_nonminimal over the m >= 8 pairs idx[0..m-1]; S is m x 9 scratch.  Returns 0, or ES_STATUS_SVD. */
+ES_BIG int es_nonminimal(const double* b1, const double* b2, const int32_t* idx, int m, double* S, double* E) {
+    double scale = 0.0;
+    for (int i = 0; i < m; ++i) {
+        const double* x1 = b1 + 3 * (size_t)idx[i];
+        const double* x2 = b2 + 3 * (size_t)idx[i];
+        for (int a = 0; a < 3; ++a)
+            for (int c = 0; c < 3; ++c) {
+                const double v = dm(x2[a], x1[c]);
+                S[(size_t)i * 9 + 3 * a + c] = v;
+                scale = es_max(scale, fabs(v));
+            }
+    }
+    if (scale == 0.0) scale = 1.0;
+    double v9[9];
+    int status = es_svd_n9(m, S, scale, v9, NULL, NULL);
+    status |= es_rank2(v9, E);
     return status;
 }

@@ -6,6 +6,10 @@ Arrays: bearings and points are (n, 3) float64, octaves (n,) int, scale_factors 
 
 And of solve::essential_solver (src/stella_vslam/solve/essential_solver.{h,cc}): the five-point minimal solver inside RANSAC on the
 device (b200_essential_ransac), the minimal sets drawn on the host by util::create_random_array(5, ...) (b200_draw_min_sets).
+
+And of solve::homography_solver and solve::fundamental_solver (homography_solver.{h,cc}, fundamental_solver.{h,cc}), monocular
+initialisation's two RANSAC solvers, H and F problems together in one call (b200_twoview_ransac), the minimal sets of 4 and 8 drawn
+by b200_draw_min_sets.
 """
 import ctypes as C
 
@@ -56,6 +60,7 @@ def _L():
         L.b200_pnp_draw_min_sets.argtypes = [C.POINTER(Mt19937), C.c_uint32, C.c_uint32, C.POINTER(C.c_int32)]
         L.b200_draw_min_sets.argtypes = [C.POINTER(Mt19937), C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_int32)]
         L.b200_essential_ransac.argtypes = [vp, C.c_int, C.POINTER(EssentialProblem)]
+        L.b200_twoview_ransac.argtypes = [vp, C.c_int, C.POINTER(TwoviewProblem)]
         L._pnp_bound = True
     return L
 
@@ -308,3 +313,135 @@ class essential_solver:
 
     def get_inlier_matches(self):
         return list(self.is_inlier_match_)
+
+
+# ---- solve::homography_solver / solve::fundamental_solver (src/stella_vslam/solve/homography_solver.cc, fundamental_solver.cc) ----
+
+MODEL_H, MODEL_F = 0, 1
+_SET_SIZE = {MODEL_H: 4, MODEL_F: 8}
+
+
+class TwoviewProblem(C.Structure):
+    """b200_twoview_problem_t (include/b200vslam.h)."""
+    _fields_ = [("model", C.c_int32), ("n_keypts_1", C.c_int32), ("keypts_1", C.c_void_p), ("n_keypts_2", C.c_int32),
+                ("keypts_2", C.c_void_p), ("n_matches", C.c_int32), ("matches_12", C.c_void_p), ("sigma", C.c_float),
+                ("max_num_iter", C.c_uint32), ("recompute", C.c_int32), ("min_sets", C.c_void_p),
+                ("status", C.c_int32), ("valid", C.c_int32), ("best_iter", C.c_int32), ("num_inliers", C.c_int32),
+                ("best_cost", C.c_float), ("M_21", C.c_double * 9), ("inlier_flags", C.c_void_p)]
+
+
+def _model_id(model):
+    m = {"H": MODEL_H, "F": MODEL_F, MODEL_H: MODEL_H, MODEL_F: MODEL_F}.get(model)
+    if m is None:
+        raise ValueError(f"two-view model must be 'H' or 'F', not {model!r}")
+    return m
+
+
+def _keypts(k):
+    """(n, 2) float32 pixel coordinates: an array, or a sequence of objects with .pt / (x, y) pairs."""
+    return np.ascontiguousarray(np.asarray(k, np.float32).reshape(-1, 2))
+
+
+def _pack_twoview(prob, keep):
+    S = TwoviewProblem()
+    m = _model_id(prob["model"])
+    k1, k2 = _keypts(prob["keypts_1"]), _keypts(prob["keypts_2"])
+    mt = np.ascontiguousarray(np.asarray(prob["matches_12"], np.int32).reshape(-1, 2))
+    k = _SET_SIZE[m]
+    ms = np.ascontiguousarray(np.asarray(prob.get("min_sets", np.zeros((0, k))), np.int32).reshape(-1, k))
+    fl = np.zeros(max(len(mt), 1), np.uint8)
+    keep += [k1, k2, mt, ms, fl]
+    S.model = m
+    S.n_keypts_1, S.keypts_1 = len(k1), k1.ctypes.data
+    S.n_keypts_2, S.keypts_2 = len(k2), k2.ctypes.data
+    S.n_matches, S.matches_12 = len(mt), mt.ctypes.data
+    S.sigma = float(prob.get("sigma", 1.0))
+    S.max_num_iter = len(ms)
+    S.recompute = int(bool(prob.get("recompute", True)))
+    S.min_sets = ms.ctypes.data
+    S.inlier_flags = fl.ctypes.data
+    return S, fl
+
+
+def twoview_ransac_batch(problems, device=0):
+    """b200_twoview_ransac over dicts(model ("H" or "F"), keypts_1, keypts_2 (all undistorted keypoints of each frame, (n, 2) pixels),
+    matches_12 ((n, 2) keypoint index pairs), min_sets (max_num_iter x 4 for H, x 8 for F), sigma=1.0, recompute=True).  H and F
+    problems mix freely in one call.  Returns per problem dict(status, valid, best_iter, num_inliers, best_cost (float32), M_21 (None
+    unless valid), inlier_flags (None on the early return, n < 8))."""
+    keep, flags = [], []
+    arr = (TwoviewProblem * max(len(problems), 1))()
+    for i, pr in enumerate(problems):
+        arr[i], fl = _pack_twoview(pr, keep)
+        flags.append(fl)
+    check(_L().b200_twoview_ransac(_handle(device), len(problems), arr))
+    out = []
+    for i in range(len(problems)):
+        S, n = arr[i], arr[i].n_matches
+        out.append(dict(status=S.status, valid=bool(S.valid), best_iter=S.best_iter, num_inliers=S.num_inliers,
+                        best_cost=np.float32(S.best_cost), M_21=np.array(S.M_21).reshape(3, 3) if S.valid else None,
+                        inlier_flags=None if n < 8 else flags[i][:n].astype(bool)))
+    return out
+
+
+class _twoview_solver:
+    """The shared surface of homography_solver and fundamental_solver.  undist_keypts_*: every undistorted keypoint of each frame
+    ((n, 2) pixels); matches_12: (first, second) index pairs.  The engine is the solver's member: find_via_ransac continues its state
+    across calls, and use_fixed_seed gives each solver its own default-constructed engine, as util::create_random_engine does."""
+
+    _model = None
+
+    def __init__(self, undist_keypts_1, undist_keypts_2, matches_12, sigma, use_fixed_seed=False, device=0):
+        self.undist_keypts_1_ = _keypts(undist_keypts_1)
+        self.undist_keypts_2_ = _keypts(undist_keypts_2)
+        m = np.asarray(matches_12, np.int64).reshape(-1, 2)
+        if len(m) and (m.min() < 0 or m[:, 0].max() >= len(self.undist_keypts_1_) or m[:, 1].max() >= len(self.undist_keypts_2_)):
+            raise IndexError("match index outside the keypoints")  # std::vector::at throws in the reference
+        self.matches_12_ = np.ascontiguousarray(m.astype(np.int32))
+        self.sigma_ = np.float32(sigma)
+        self.device = device
+        self.random_engine_ = mt19937(None if use_fixed_seed else np.frombuffer(np.random.bytes(40), np.uint32))
+        self.solution_is_valid_ = False
+        self.best_cost_ = np.float32(0.0)
+        self.best_M_21_ = np.zeros((3, 3))
+        self.is_inlier_match_ = []
+        self.status_ = 0
+
+    def find_via_ransac(self, max_num_iter, recompute=True):
+        n = len(self.matches_12_)
+        if n < 8:
+            self.solution_is_valid_ = False
+            return
+        ms = draw_min_sets(n, max_num_iter, self.random_engine_, set_size=_SET_SIZE[self._model])
+        r = twoview_ransac_batch([dict(model=self._model, keypts_1=self.undist_keypts_1_, keypts_2=self.undist_keypts_2_,
+                                       matches_12=self.matches_12_, sigma=self.sigma_, min_sets=ms, recompute=recompute)], self.device)[0]
+        self.status_ = r["status"]
+        self.solution_is_valid_ = r["valid"]
+        self.best_cost_ = r["best_cost"]
+        if r["valid"]:
+            self.best_M_21_ = r["M_21"]
+        self.is_inlier_match_ = [bool(v) for v in r["inlier_flags"]]
+
+    def solution_is_valid(self):
+        return self.solution_is_valid_
+
+    def get_best_cost(self):
+        return self.best_cost_
+
+    def get_inlier_matches(self):
+        return list(self.is_inlier_match_)
+
+
+class homography_solver(_twoview_solver):
+    """solve::homography_solver: the four-point DLT inside RANSAC (min_sets of 4, early return below 8 matches)."""
+    _model = MODEL_H
+
+    def get_best_H_21(self):
+        return self.best_M_21_.copy()
+
+
+class fundamental_solver(_twoview_solver):
+    """solve::fundamental_solver: the normalised eight-point algorithm inside RANSAC."""
+    _model = MODEL_F
+
+    def get_best_F_21(self):
+        return self.best_M_21_.copy()

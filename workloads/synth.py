@@ -812,6 +812,97 @@ def make_essential_problem(seed=0, n=500, inlier_frac=0.6, model="perspective", 
     return dict(bearings_1=np.ascontiguousarray(b1), bearings_2=np.ascontiguousarray(b2), E_21=E, R_21=R, t_21=t, gt_inlier=inl)
 
 
+EUROC_MONO = dict(fx=458.654, fy=457.296, cx=367.215, cy=248.375, cols=752, rows=480)  # example/euroc/EuRoC_mono.yaml
+
+
+def make_twoview_problem(seed=0, n=500, inlier_frac=0.7, scene="general", case=None, noise=0.5, camera="euroc"):
+    """Two monocular frames for homography_solver / fundamental_solver: undistorted pixel keypoints of both frames, with extra unmatched
+    keypoints in each (normalisation runs over all of them), and matches in ascending order of the frame-1 index.  A true R_21 (a few
+    degrees), t_21 (0.3 m), inlier keypoints of frame 2 moved by Gaussian pixel noise `noise`, outliers at least 6 px from their true
+    epipolar line.  scene: "general" (depths 2-10 m) or "planar" (the plane n.X = 5 m in frame 1).  camera: "euroc" or "kitti".
+    case: None; "pure_rotation" (t_21 = 0); "collinear" (noise-free, R_21 = I, t_21 along x; four fifths of the points on one 3D
+    line parallel to the baseline, which images to one row of both frames, the same float y for every point, so normalisation keeps
+    them exactly collinear and most minimal sets make H's coefficient matrix lose rank); "n7" / "n8" (7 or 8 matches); "inliers5" / "inliers9" / "inliers10"
+    (exactly 5, 9 or 10 noise-free inliers among 10, 12 or 14 matches: RANSAC keeps exactly that many, so the recompute takes H's tall
+    path at 10 rows and F's square or tall path); "duplicated" (a fifth of the matches copy the coordinates of others in both frames).
+    Returns dict(keypts_1, keypts_2 ((n_k, 2) float32), matches_12 ((n, 2) int32), R_21, t_21, K, H_21 (planar or pure rotation, else
+    None), F_21 (None under pure rotation), gt_inlier (match order), cols, rows)."""
+    rng = np.random.default_rng(seed)
+    cam = EUROC_MONO if camera == "euroc" else KITTI
+    K = np.array([[cam["fx"], 0, cam["cx"]], [0, cam["fy"], cam["cy"]], [0, 0, 1.0]])
+    Ki = np.linalg.inv(K)
+    cols, rows = cam["cols"], cam["rows"]
+    fixed = {"n7": (7, 7), "n8": (8, 8), "inliers5": (10, 5), "inliers9": (12, 9), "inliers10": (14, 10)}
+    if case in fixed:
+        n, n_in = fixed[case]
+        if case.startswith("inliers"):
+            noise = 0.0
+    else:
+        n_in = int(round(inlier_frac * n))
+    if case == "collinear":
+        noise = 0.0
+    R = _rodrigues(0.05 * rng.standard_normal(3))
+    t = rng.standard_normal(3)
+    t *= 0.3 / np.linalg.norm(t)
+    if case == "pure_rotation":
+        t = np.zeros(3)
+    nrm = np.array([0.1 * rng.standard_normal(), 0.1 * rng.standard_normal(), 1.0])
+    if case == "collinear":
+        R, t, nrm[0] = np.eye(3), np.array([0.3, 0.0, 0.0]), 0.0
+    nrm /= np.linalg.norm(nrm)
+    line_y = 0.3
+    line_z = (5.0 - nrm[1] * line_y) / nrm[2] if scene == "planar" else 6.0
+    P, p1, p2 = [], [], []
+    while len(P) < n:
+        if case == "collinear" and rng.uniform() < 0.8:
+            X = np.array([rng.uniform(-2.0, 2.0), line_y, line_z])
+        else:
+            ray = Ki @ np.array([rng.uniform(10, cols - 10), rng.uniform(10, rows - 10), 1.0])
+            X = ray * (5.0 / (nrm @ ray) if scene == "planar" else rng.uniform(2, 10))
+        Y = R @ X + t
+        if X[2] <= 0 or Y[2] <= 0:
+            continue
+        a, b = K @ (X / X[2]), K @ (Y / Y[2])
+        if not (0 <= a[0] < cols and 0 <= a[1] < rows and 0 <= b[0] < cols and 0 <= b[1] < rows):
+            continue
+        P.append(X)
+        p1.append(a[:2])
+        p2.append(b[:2])
+    p1, p2 = np.array(p1), np.array(p2)
+    tx = np.array([[0, -t[2], t[1]], [t[2], 0, -t[0]], [-t[1], t[0], 0]])
+    F = None if case == "pure_rotation" else Ki.T @ tx @ R @ Ki
+    H = K @ (R + np.outer(t, nrm) / 5.0) @ Ki if (scene == "planar" or case == "pure_rotation") else None
+    if noise > 0:
+        p2 = p2 + noise * rng.standard_normal(p2.shape)
+    inl = np.zeros(n, bool)
+    inl[rng.permutation(n)[:n_in]] = True
+    for j in np.flatnonzero(~inl):
+        while True:
+            o = np.array([rng.uniform(0, cols), rng.uniform(0, rows)])
+            if F is None:
+                if np.linalg.norm(o - p2[j]) > 20.0:
+                    break
+                continue
+            line = F @ np.array([p1[j, 0], p1[j, 1], 1.0])
+            if abs(line @ np.array([o[0], o[1], 1.0])) / np.hypot(line[0], line[1]) > 6.0:
+                break
+        p2[j] = o
+    if case == "duplicated":
+        k = n // 5
+        src, dst = rng.choice(n, k, replace=False), rng.choice(n, k, replace=False)
+        p1[dst], p2[dst], inl[dst] = p1[src], p2[src], inl[src]
+    n_extra = max(5, n // 3)
+    kp1 = np.concatenate([p1, np.stack([rng.uniform(0, cols, n_extra), rng.uniform(0, rows, n_extra)], 1)])
+    kp2 = np.concatenate([p2, np.stack([rng.uniform(0, cols, n_extra), rng.uniform(0, rows, n_extra)], 1)])
+    perm1, perm2 = rng.permutation(len(kp1)), rng.permutation(len(kp2))
+    kp1, kp2 = kp1[perm1], kp2[perm2]
+    pos1, pos2 = np.argsort(perm1)[:n], np.argsort(perm2)[:n]  # where match j's keypoints landed
+    order = np.argsort(pos1)
+    matches = np.stack([pos1[order], pos2[order]], 1).astype(np.int32)
+    return dict(keypts_1=np.ascontiguousarray(kp1, np.float32), keypts_2=np.ascontiguousarray(kp2, np.float32), matches_12=matches, R_21=R,
+                t_21=t, K=K, H_21=H, F_21=F, gt_inlier=inl[order], cols=cols, rows=rows)
+
+
 def make_pose_graph(n_keyframes=500, seed=0, fix_scale=False, laps=1.5, window=8, rot_noise=2e-3, trans_noise=0.01, scale_noise=2e-3,
                     lm_per_keyframe=4, min_num_shared_lms=100, return_description=False):
     """A loop-closure pose graph for optimize.graph_optimizer, built by optimize.build_essential_graph.
