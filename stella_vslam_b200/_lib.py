@@ -35,7 +35,21 @@ class CameraIntrinsics(C.Structure):
     """b200_camera_intrinsics_t (include/b200vslam.h)."""
     _fields_ = [("model", C.c_int32), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
                 ("k1", C.c_double), ("k2", C.c_double), ("p1", C.c_double), ("p2", C.c_double), ("k3", C.c_double),
-                ("cols", C.c_double), ("rows", C.c_double)]
+                ("cols", C.c_double), ("rows", C.c_double), ("k4", C.c_double), ("distortion", C.c_double)]
+
+
+# camera::base::model_type_t names -> the model codes of b200_camera_intrinsics_t
+CAMERA_MODELS = {"perspective": 0, "equirectangular": 1, "fisheye": 2, "radial_division": 3}
+
+
+def camera_intrinsics(camera):
+    """b200_camera_intrinsics_t of a camera dict: model ("perspective" when absent, "equirectangular", "fisheye",
+    "radial_division"), fx, fy, cx, cy, k1, k2, p1, p2, k3, k4, distortion, cols, rows; missing values are 0."""
+    name = camera.get("model", "perspective")
+    if name not in CAMERA_MODELS:
+        raise ValueError(f"unknown camera model {name!r}; expected one of {sorted(CAMERA_MODELS)}")
+    return CameraIntrinsics(CAMERA_MODELS[name], *[float(camera.get(k, 0.0)) for k in
+                            ("fx", "fy", "cx", "cy", "k1", "k2", "p1", "p2", "k3", "cols", "rows", "k4", "distortion")])
 
 
 class RectifierParams(C.Structure):

@@ -2869,7 +2869,8 @@ int track_stage_c(b200_lba_t opt, cudaStream_t st, const TrackShared& sh, const 
         PoseProb pb{};
         pb.n = 0;
         pb.edge_off = (int)off;
-        pb.cam = Cam{sh.model, sh.fx, sh.fy, sh.cx, sh.cy, sh.fxb, sh.cols, sh.rows};
+        // fisheye and radial division use the perspective edges (reproj_edge_wrapper.h), i.e. edge model 0
+        pb.cam = Cam{sh.model == 1 ? 1 : 0, sh.fx, sh.fy, sh.cx, sh.cy, sh.fxb, sh.cols, sh.rows};
         const double* M = pose_cw[f];  // util::converter::to_g2o_SE3 (util/converter.cc:17-21)
         const double R[9] = {M[0], M[1], M[2], M[4], M[5], M[6], M[8], M[9], M[10]};
         rot_to_quat(R, pb.q);

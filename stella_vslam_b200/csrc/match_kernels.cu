@@ -1759,7 +1759,7 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const
     if (n_frames == 0) return B200_OK;
     if (!frames || !prm->scale_factors || !prm->inv_level_sigma_sq || prm->num_levels == 0 || prm->num_levels > 32 || prm->grid_cols <= 0
         || prm->grid_rows <= 0 || (long long)prm->grid_cols * prm->grid_rows > (1 << 20) || !(prm->img_bounds[1] > prm->img_bounds[0])
-        || !(prm->img_bounds[3] > prm->img_bounds[2]) || (prm->cam.model != 0 && prm->cam.model != 1) || prm->max_candidates < 0
+        || !(prm->img_bounds[3] > prm->img_bounds[2]) || !b200::chain::camera_valid(prm->cam) || prm->max_candidates < 0
         || prm->num_trials_robust < 0 || prm->num_trials < 0 || prm->num_each_iter < 0) {
         b200::set_error("b200_track_local_map: invalid parameters");
         return B200_ERR_INVALID;
@@ -1869,6 +1869,7 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const
     sh.model = prm->cam.model;
     sh.fx = prm->cam.fx; sh.fy = prm->cam.fy; sh.cx = prm->cam.cx; sh.cy = prm->cam.cy;
     sh.k1 = prm->cam.k1; sh.k2 = prm->cam.k2; sh.p1 = prm->cam.p1; sh.p2 = prm->cam.p2; sh.k3 = prm->cam.k3;
+    sh.k4 = prm->cam.k4; sh.distortion = prm->cam.distortion;
     sh.cols = prm->cam.cols; sh.rows = prm->cam.rows;
     sh.fxb = prm->focal_x_baseline;
     sh.min_x = prm->img_bounds[0]; sh.max_x = prm->img_bounds[1]; sh.min_y = prm->img_bounds[2]; sh.max_y = prm->img_bounds[3];

@@ -3,14 +3,26 @@
 // ABI), stage C (edge build + pose optimisation) in lba_kernels.cu.  Plain device pointers, no handles' internals cross a TU.
 #pragma once
 
+#include <cmath>
+
 #include "common.cuh"
 
 namespace b200 {
 namespace chain {
 
+// The camera models of b200_camera_intrinsics_t: 0 perspective, 1 equirectangular, 2 fisheye, 3 radial division.  Models 2 and 3 need
+// finite intrinsics and coefficients (models 0 and 1 are accepted as before, whatever their values).
+inline bool camera_valid(const b200_camera_intrinsics_t& c) {
+    if (c.model < 0 || c.model > 3) return false;
+    if (c.model < 2) return true;
+    const bool coeffs = c.model == 2 ? (std::isfinite(c.k1) && std::isfinite(c.k2) && std::isfinite(c.k3) && std::isfinite(c.k4))
+                                     : std::isfinite(c.distortion);
+    return coeffs && std::isfinite(c.fx) && std::isfinite(c.fy) && std::isfinite(c.cx) && std::isfinite(c.cy);
+}
+
 struct TrackShared {  // by-value kernel parameter
     int model;
-    double fx, fy, cx, cy, k1, k2, p1, p2, k3, cols, rows, fxb;
+    double fx, fy, cx, cy, k1, k2, p1, p2, k3, cols, rows, fxb, k4, distortion;
     float min_x, max_x, min_y, max_y;
     float ray_cos_thr, log_scale_factor, margin, delta;
     unsigned num_levels;

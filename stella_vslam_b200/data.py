@@ -7,7 +7,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import KP_DTYPE, CameraIntrinsics, check, lib, ptr
+from ._lib import KP_DTYPE, CameraIntrinsics, camera_intrinsics, check, lib, ptr
 
 # cv::KeyPoint as stored in the `undist_keypts` blob: 28 bytes
 CV_KEYPOINT_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"), ("response", "<f4"), ("octave", "<i4"), ("class_id", "<i4")])
@@ -26,8 +26,7 @@ def export_keyframe_blobs(extractor, frame=0, camera=None):
     n = C.c_int32()
     cam = None
     if camera is not None:
-        cam = CameraIntrinsics(1 if camera.get("model", "perspective") == "equirectangular" else 0,
-                               *[float(camera.get(k, 0.0)) for k in ("fx", "fy", "cx", "cy", "k1", "k2", "p1", "p2", "k3", "cols", "rows")])
+        cam = camera_intrinsics(camera)
     check(L.b200_orb_export_keyframe_blobs(extractor._h, int(frame), C.byref(cam) if cam is not None else None, ptr(kp), ptr(desc), cap, C.byref(n)))
     return kp[:n.value].copy(), desc[:n.value].copy()
 

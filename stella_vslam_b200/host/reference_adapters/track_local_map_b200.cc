@@ -10,7 +10,9 @@
 // Precondition: `extractor` is the (left) feature::orb_extractor whose LAST extract() produced curr_frm (true in system.cc:380-395:
 // one extract per frame, frame constructed from its outputs), so frame 0 of its last batch is this frame.
 #include "stella_vslam/camera/base.h"
+#include "stella_vslam/camera/fisheye.h"
 #include "stella_vslam/camera/perspective.h"
+#include "stella_vslam/camera/radial_division.h"
 #include "stella_vslam/data/frame.h"
 #include "stella_vslam/data/keyframe.h"
 #include "stella_vslam/data/landmark.h"
@@ -88,13 +90,33 @@ bool track_local_map_b200(data::frame& curr_frm, const std::vector<std::shared_p
     // ---- one chain call
     b200_track_params_t prm{};
     const auto* cam = curr_frm.camera_;
-    prm.cam.model = cam->model_type_ == camera::model_type_t::Equirectangular ? 1 : 0;
-    if (cam->model_type_ == camera::model_type_t::Perspective) {
-        const auto* p = static_cast<const camera::perspective*>(cam);
-        prm.cam.fx = p->fx_; prm.cam.fy = p->fy_; prm.cam.cx = p->cx_; prm.cam.cy = p->cy_;
-        prm.cam.k1 = p->k1_; prm.cam.k2 = p->k2_; prm.cam.p1 = p->p1_; prm.cam.p2 = p->p2_; prm.cam.k3 = p->k3_;
-    } else if (prm.cam.model == 0) {
-        throw std::runtime_error("track_local_map_b200: perspective and equirectangular cameras only (fisheye / radial division: stage-by-stage ABI)");
+    // model codes of b200_camera_intrinsics_t: 0 perspective, 1 equirectangular, 2 fisheye, 3 radial division (the double members;
+    // the fisheye undistortion rounds them to float on the device as cv_cam_matrix_ / cv_dist_params_ do)
+    switch (cam->model_type_) {
+        case camera::model_type_t::Perspective: {
+            const auto* p = static_cast<const camera::perspective*>(cam);
+            prm.cam.model = 0;
+            prm.cam.fx = p->fx_; prm.cam.fy = p->fy_; prm.cam.cx = p->cx_; prm.cam.cy = p->cy_;
+            prm.cam.k1 = p->k1_; prm.cam.k2 = p->k2_; prm.cam.p1 = p->p1_; prm.cam.p2 = p->p2_; prm.cam.k3 = p->k3_;
+            break;
+        }
+        case camera::model_type_t::Fisheye: {
+            const auto* p = static_cast<const camera::fisheye*>(cam);
+            prm.cam.model = 2;
+            prm.cam.fx = p->fx_; prm.cam.fy = p->fy_; prm.cam.cx = p->cx_; prm.cam.cy = p->cy_;
+            prm.cam.k1 = p->k1_; prm.cam.k2 = p->k2_; prm.cam.k3 = p->k3_; prm.cam.k4 = p->k4_;
+            break;
+        }
+        case camera::model_type_t::RadialDivision: {
+            const auto* p = static_cast<const camera::radial_division*>(cam);
+            prm.cam.model = 3;
+            prm.cam.fx = p->fx_; prm.cam.fy = p->fy_; prm.cam.cx = p->cx_; prm.cam.cy = p->cy_;
+            prm.cam.distortion = p->distortion_;
+            break;
+        }
+        default:
+            prm.cam.model = 1;  // equirectangular
+            break;
     }
     prm.cam.cols = cam->cols_;
     prm.cam.rows = cam->rows_;

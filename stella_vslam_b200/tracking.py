@@ -5,7 +5,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import match, optimize
+from . import _lib, feature, match, optimize
 from ._lib import CameraIntrinsics, check, lib, ptr
 
 
@@ -38,8 +38,8 @@ def _bind():
 
 
 def camera_intrinsics(camera):
-    return CameraIntrinsics(1 if camera.get("model", "perspective") == "equirectangular" else 0,
-                            *[float(camera.get(k, 0.0)) for k in ("fx", "fy", "cx", "cy", "k1", "k2", "p1", "p2", "k3", "cols", "rows")])
+    """b200_camera_intrinsics_t of a camera dict (perspective, equirectangular, fisheye or radial_division; see _lib.camera_intrinsics)."""
+    return _lib.camera_intrinsics(camera)
 
 
 class local_map_tracker:
@@ -60,7 +60,12 @@ class local_map_tracker:
         p.cam = camera_intrinsics(camera)
         p.focal_x_baseline = float(camera.get("fxb", 0.0))
         p.monocular = 1 if camera.get("setup", "monocular") == "monocular" else 0
-        b = img_bounds if img_bounds is not None else (0.0, camera.get("cols", 0.0), 0.0, camera.get("rows", 0.0))
+        if img_bounds is not None:
+            b = img_bounds
+        elif p.cam.model in (2, 3):  # fisheye / radial division: camera::*::compute_image_bounds
+            b = feature.camera_image_bounds(camera, extractor)
+        else:
+            b = (0.0, camera.get("cols", 0.0), 0.0, camera.get("rows", 0.0))
         p.img_bounds = (C.c_float * 4)(*[float(v) for v in b])
         p.grid_cols, p.grid_rows = int(grid[0]), int(grid[1])
         p.num_levels = int(op.num_levels_)
