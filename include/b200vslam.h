@@ -214,6 +214,27 @@ typedef struct {
 } b200_cv_keypoint_t;
 int b200_orb_export_keyframe_blobs(b200_orb_t h, int frame, const b200_camera_intrinsics_t* cam, b200_cv_keypoint_t* keypts_blob,
                                    uint8_t* desc_blob, int cap, int32_t* n);
+/* RGB-D frames: system::create_RGBD_frame after the extraction (src/stella_vslam/system.cc:467-530) for the first n_frames frames of the
+ * last extract on `h`, whose keypoints are read where they lie in HBM.  The depth maps are HOST buffers (frame f at depth_maps +
+ * f * frame_stride, rows `pitch` bytes apart) of type B200_DEPTH_16UC1 (TUM RGB-D) or B200_DEPTH_32FC1, the cv::Mat::type() codes, and
+ * exactly the extracted frames' size.  One upload, one launch and one download on the extractor's stream.  Per keypoint:
+ *   undist_keypts / bearings : camera::*::undistort_keypoints + convert_keypoints_to_bearings, the device functions of
+ *                              b200_keypoints_undistort (bit-identical to it)
+ *   depth                    : img_depth.at<float>(y, x) at the DISTORTED keypoint with x, y truncated to int (system.cc:499-503), after
+ *                              util::convert_to_true_depth (util/image_converter.cc:41-43) = convertTo(CV_32F, 1.0 / depthmap_factor),
+ *                              which OpenCV evaluates as (float)v * (float)(1.0 / depthmap_factor) (a plain copy for 32FC1 with factor 1);
+ *                              only the sampled pixels are converted
+ *   depths / x_right         : -1 / -1 unless 0 < depth (system.cc:505-507; a NaN is invalid here, the reference's `depth <= 0` lets it
+ *                              through), else depth / (float)(undist_x - focal_x_baseline / depth) in double (system.cc:509-510)
+ * Frame f writes entries f * cap ..; n_keypoints[f] = its keypoint count.  B200_ERR_CAPACITY when a frame has more than cap keypoints (its
+ * first cap are written).  B200_ERR_INVALID: another depth type, a depth map whose size differs from the extracted frames (the reference
+ * only warns, system.cc:469-474, and then reads out of bounds), model 1 (equirectangular: data/common.cc:236-238 throws for RGB-D), a
+ * depthmap_factor that is not positive and finite, n_frames beyond the last extract. */
+#define B200_DEPTH_16UC1 2
+#define B200_DEPTH_32FC1 5
+int b200_rgbd_depths(b200_orb_t h, int n_frames, const b200_camera_intrinsics_t* cam, double focal_x_baseline, double depthmap_factor, int depth_type,
+                     const void* depth_maps, int width, int height, size_t pitch, size_t frame_stride, int cap, b200_keypoint_t* undist_keypts,
+                     double* bearings, float* depths, float* x_right, int32_t* n_keypoints);
 /* The inverse for a keyframe loaded from a map file (host-only byte shuffling, no GPU work): cv::KeyPoint records -> b200_keypoint_t. */
 int b200_keyframe_blob_to_keypoints(const b200_cv_keypoint_t* keypts_blob, int n, b200_keypoint_t* keypts);
 
@@ -645,6 +666,54 @@ typedef struct b200_new_landmarks_problem {
 } b200_new_landmarks_problem_t;
 int b200_create_new_landmarks(b200_matcher_t h, int n_keyframes, b200_new_landmarks_problem_t* problems, float lowe_ratio, float residual_rad_thr,
                               float rays_parallax_deg_thr, int max_candidates);
+
+/* Depth-seeded landmarks of a stereo or RGB-D keyframe, for many keyframes in one upload, one launch (one CTA per problem) and one download
+ * on the matcher's stream:
+ *   mode 0 (B200_DEPTH_LM_KEYFRAME) : module::keyframe_inserter::create_new_keyframe (module/keyframe_inserter.cc:160-212): the keypoints
+ *       with 0 < depth sorted ascending by (depth, idx) as std::sort orders pair<float, unsigned>, walked with `count` = position in that
+ *       order; the walk stops at the first count with 100 < count && depth_thr < depth; a keypoint that already has a landmark
+ *       (has_landmark[idx] != 0) is skipped but still advances count.  At most B200_DEPTH_LM_MAX_SORT keypoints with 0 < depth per problem
+ *       (the sort runs in shared memory): more is B200_ERR_CAPACITY for that problem.
+ *   mode 1 (B200_DEPTH_LM_INITIAL)  : module::initializer::create_map_for_stereo (module/initializer.cc:363-387): every keypoint with
+ *       0 < depth, in index order; has_landmark is not read.
+ * Each created landmark: pos_w = data::triangulate_stereo (data/common.cc:192-260): unproj = (float)((x - cx) * depth * fx_inv) (likewise
+ * y) in double, pos_c = (unproj_x, unproj_y, depth), pos_w = R_wc pos_c + t_wc in double with each row summed left to right; then
+ * landmark::update_mean_normal_and_obs_scale_variance (data/landmark.cc:256-311) with its one observation, which is also its reference
+ * keyframe, at the frame's camera centre (t_wc) and scale_factors[octave]: the device function of b200_landmark_geometry.  Its descriptor
+ * (compute_descriptor of one observation) is the keypoint's own row: created_idx gives it.  Outputs are in creation order, i.e. the
+ * order of map_database::next_landmark_id_.  try_initialize_for_stereo's count (initializer.cc) is left to the caller.
+ * status per problem: B200_OK; B200_ERR_INVALID for model 1 (equirectangular) with a keypoint of 0 < depth (data/common.cc:236-238
+ * throws), an octave of a 0 < depth keypoint outside [0, num_levels), a null required pointer or a mode other than 0 / 1;
+ * B200_ERR_CAPACITY as above.  Problems whose status is not B200_OK write n_created = 0 and no landmarks; the call returns the first
+ * such status (B200_OK when every problem ran). */
+#define B200_DEPTH_LM_KEYFRAME 0
+#define B200_DEPTH_LM_INITIAL 1
+#define B200_DEPTH_LM_MAX_SORT 8192
+typedef struct b200_depth_landmarks_problem {
+    int32_t mode;                   /* B200_DEPTH_LM_KEYFRAME or B200_DEPTH_LM_INITIAL */
+    int32_t model;                  /* model code as in b200_camera_intrinsics_t: 0, 2 or 3; 1 is rejected once a depth is valid */
+    double pose_wc[16];             /* frame::get_pose_wc(), row-major: rot_wc, trans_wc (the camera centre) */
+    double fx_inv, fy_inv, cx, cy;  /* camera::perspective (fisheye, radial_division) members */
+    double depth_thr;               /* camera::base::depth_thr_ (mode 0) */
+    int32_t n_keypoints;
+    const float* x;                 /* frm_obs_.undist_keypts_[i].pt.x */
+    const float* y;
+    const int32_t* octave;          /* undist_keypts_[i].octave */
+    const float* depth;             /* frm_obs_.depths_ (b200_rgbd_depths or b200_stereo_compute) */
+    const uint8_t* has_landmark;    /* mode 0: curr_frm.get_landmark(idx) is set; NULL = none */
+    int32_t num_levels;             /* entries of scale_factors */
+    const float* scale_factors;     /* orb_params_->scale_factors_ */
+    float inv_scale_factor_last;    /* orb_params_->inv_scale_factors_[num_levels - 1] */
+    /* out, capacity n_keypoints each */
+    int32_t* created_idx;           /* keypoint index of each created landmark */
+    double* pos_w;                  /* 3 per landmark */
+    double* mean_normal;            /* 3 per landmark */
+    float* min_valid_dist;
+    float* max_valid_dist;
+    int32_t n_created;              /* out */
+    int32_t status;                 /* out */
+} b200_depth_landmarks_problem_t;
+int b200_depth_landmarks(b200_matcher_t h, int n_problems, b200_depth_landmarks_problem_t* problems);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Relocalisation's PnP: solve::pnp_solver (src/stella_vslam/solve/pnp_solver.{h,cc}) -- EPnP (Lepetit et al., IJCV 2009) inside

@@ -13,6 +13,7 @@
 //   b200::util::stereo_rectifier          <-> stella_vslam::util::stereo_rectifier          (util/stereo_rectifier.h:14-46)
 //   b200::solve::pnp_solver               <-> stella_vslam::solve::pnp_solver               (solve/pnp_solver.h:13-142)
 //   b200::solve::essential_solver         <-> stella_vslam::solve::essential_solver         (solve/essential_solver.h)
+//   b200::module::depth_landmarks         <-> the depth branches of module::keyframe_inserter and module::initializer
 #pragma once
 
 #include <cmath>
@@ -118,6 +119,32 @@ public:
         if (w) *w = lw;
         if (hgt) *hgt = lh;
         return out;
+    }
+    // system::create_RGBD_frame after the extraction (system.cc:467-530), b200_rgbd_depths: the first n_frames frames of the last
+    // extract; frame f's results start at f * cap (cap = max_keypoints(width, height)), counts[f] = its keypoints.  depth_type:
+    // B200_DEPTH_16UC1 or B200_DEPTH_32FC1 (cv::Mat::type()); the maps are host buffers of the extracted frames' size.
+    struct rgbd_frames {
+        int cap = 0;
+        std::vector<b200_keypoint_t> undist_keypts;
+        std::vector<double> bearings;
+        std::vector<float> depths, x_right;
+        std::vector<int32_t> counts;
+    };
+    rgbd_frames rgbd_depths(const b200_camera_intrinsics_t& cam, double focal_x_baseline, double depthmap_factor, int depth_type,
+                            const void* depth_maps, int width, int height, size_t pitch, size_t frame_stride, int n_frames) const {
+        rgbd_frames r;
+        r.cap = max_keypoints(width, height);
+        check(r.cap < 0 ? r.cap : B200_OK, "b200_orb_max_keypoints");
+        const size_t m = (size_t)r.cap * (n_frames > 0 ? n_frames : 0);
+        r.undist_keypts.resize(m);
+        r.bearings.resize(3 * m);
+        r.depths.resize(m);
+        r.x_right.resize(m);
+        r.counts.assign(n_frames > 0 ? n_frames : 0, 0);
+        check(b200_rgbd_depths(h_, n_frames, &cam, focal_x_baseline, depthmap_factor, depth_type, depth_maps, width, height, pitch, frame_stride, r.cap,
+                               r.undist_keypts.data(), r.bearings.data(), r.depths.data(), r.x_right.data(), r.counts.data()),
+              "b200_rgbd_depths");
+        return r;
     }
     b200_orb_t handle() const { return h_; }
 
@@ -307,6 +334,60 @@ private:
 };
 
 }  // namespace match
+
+namespace module {
+
+// The depth-seeded landmarks of stereo / RGB-D keyframes (b200_depth_landmarks): keyframe_inserter::create_new_keyframe's depth branch
+// (mode B200_DEPTH_LM_KEYFRAME, module/keyframe_inserter.cc:160-212) and initializer::create_map_for_stereo's landmark loop
+// (B200_DEPTH_LM_INITIAL, module/initializer.cc:363-387) for many frames in one call.
+class depth_landmarks {
+public:
+    struct result {
+        std::vector<int32_t> idx;  // keypoint of each created landmark, in creation order
+        std::vector<double> pos_w, mean_normal;
+        std::vector<float> min_valid_dist, max_valid_dist;
+        int32_t status = B200_OK;
+    };
+    explicit depth_landmarks(int device = 0) : m_(device) {}
+    // Problems with their inputs filled (the output pointers are set here).  Throws on the first rejected problem unless
+    // throw_on_error is false; then result::status tells which ones ran.
+    std::vector<result> create(std::vector<b200_depth_landmarks_problem_t> problems, bool throw_on_error = true) {
+        std::vector<result> out(problems.size());
+        for (size_t k = 0; k < problems.size(); ++k) {
+            auto& p = problems[k];
+            const size_t n = p.n_keypoints > 0 ? (size_t)p.n_keypoints : 0;
+            auto& r = out[k];
+            r.idx.resize(n);
+            r.pos_w.resize(3 * n);
+            r.mean_normal.resize(3 * n);
+            r.min_valid_dist.resize(n);
+            r.max_valid_dist.resize(n);
+            p.created_idx = r.idx.data();
+            p.pos_w = r.pos_w.data();
+            p.mean_normal = r.mean_normal.data();
+            p.min_valid_dist = r.min_valid_dist.data();
+            p.max_valid_dist = r.max_valid_dist.data();
+        }
+        const int rc = b200_depth_landmarks(m_.get(), (int)problems.size(), problems.data());
+        if (throw_on_error) check(rc, "b200_depth_landmarks");
+        for (size_t k = 0; k < problems.size(); ++k) {
+            const size_t c = (size_t)problems[k].n_created;
+            auto& r = out[k];
+            r.status = problems[k].status;
+            r.idx.resize(c);
+            r.pos_w.resize(3 * c);
+            r.mean_normal.resize(3 * c);
+            r.min_valid_dist.resize(c);
+            r.max_valid_dist.resize(c);
+        }
+        return out;
+    }
+
+private:
+    match::device_matcher m_;
+};
+
+}  // namespace module
 
 namespace optimize {
 

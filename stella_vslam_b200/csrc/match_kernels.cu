@@ -1201,16 +1201,12 @@ __global__ void __launch_bounds__(128) landmark_descriptor_kernel(const uint4* _
 __device__ __forceinline__ double norm3(double x, double y, double z) {
     return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)));
 }
-__global__ void __launch_bounds__(128) landmark_geometry_kernel(int n, const double* __restrict__ pos_w, const int* __restrict__ offsets,
-                                                                const double* __restrict__ cam_centers, const double* __restrict__ ref_center,
-                                                                const float* __restrict__ ref_scale, float inv_scale_last,
-                                                                double* __restrict__ mean_normal, float* __restrict__ max_valid,
-                                                                float* __restrict__ min_valid) {
-    const int l = blockIdx.x * blockDim.x + threadIdx.x;
-    if (l >= n) return;
-    const double px = pos_w[3 * (size_t)l], py = pos_w[3 * (size_t)l + 1], pz = pos_w[3 * (size_t)l + 2];
+// One landmark: observed from cam_centers[3 * o_begin .. 3 * o_end), reference keyframe centre ref_center.
+__device__ __forceinline__ void landmark_geometry_one(double px, double py, double pz, const double* __restrict__ cam_centers, int o_begin, int o_end,
+                                                      const double* __restrict__ ref_center, float ref_scale, float inv_scale_last,
+                                                      double* __restrict__ mean_normal, float& max_valid, float& min_valid) {
     double mx = 0.0, my = 0.0, mz = 0.0;
-    for (int o = offsets[l]; o < offsets[l + 1]; ++o) {
+    for (int o = o_begin; o < o_end; ++o) {
         const double vx = __dsub_rn(px, cam_centers[3 * (size_t)o]), vy = __dsub_rn(py, cam_centers[3 * (size_t)o + 1]),
                      vz = __dsub_rn(pz, cam_centers[3 * (size_t)o + 2]);
         const double nrm = norm3(vx, vy, vz);
@@ -1220,13 +1216,141 @@ __global__ void __launch_bounds__(128) landmark_geometry_kernel(int n, const dou
         mz = __dadd_rn(mz, pos ? __ddiv_rn(vz, nrm) : vz);
     }
     const double mn = norm3(mx, my, mz);
-    mean_normal[3 * (size_t)l] = mn > 0.0 ? __ddiv_rn(mx, mn) : mx;
-    mean_normal[3 * (size_t)l + 1] = mn > 0.0 ? __ddiv_rn(my, mn) : my;
-    mean_normal[3 * (size_t)l + 2] = mn > 0.0 ? __ddiv_rn(mz, mn) : mz;
-    const double dist = norm3(__dsub_rn(px, ref_center[3 * (size_t)l]), __dsub_rn(py, ref_center[3 * (size_t)l + 1]), __dsub_rn(pz, ref_center[3 * (size_t)l + 2]));
-    const float mxv = __double2float_rn(__dmul_rn(dist, (double)ref_scale[l]));
-    max_valid[l] = mxv;
-    min_valid[l] = __fmul_rn(mxv, inv_scale_last);
+    mean_normal[0] = mn > 0.0 ? __ddiv_rn(mx, mn) : mx;
+    mean_normal[1] = mn > 0.0 ? __ddiv_rn(my, mn) : my;
+    mean_normal[2] = mn > 0.0 ? __ddiv_rn(mz, mn) : mz;
+    const double dist = norm3(__dsub_rn(px, ref_center[0]), __dsub_rn(py, ref_center[1]), __dsub_rn(pz, ref_center[2]));
+    const float mxv = __double2float_rn(__dmul_rn(dist, (double)ref_scale));
+    max_valid = mxv;
+    min_valid = __fmul_rn(mxv, inv_scale_last);
+}
+
+__global__ void __launch_bounds__(128) landmark_geometry_kernel(int n, const double* __restrict__ pos_w, const int* __restrict__ offsets,
+                                                                const double* __restrict__ cam_centers, const double* __restrict__ ref_center,
+                                                                const float* __restrict__ ref_scale, float inv_scale_last,
+                                                                double* __restrict__ mean_normal, float* __restrict__ max_valid,
+                                                                float* __restrict__ min_valid) {
+    const int l = blockIdx.x * blockDim.x + threadIdx.x;
+    if (l >= n) return;
+    landmark_geometry_one(pos_w[3 * (size_t)l], pos_w[3 * (size_t)l + 1], pos_w[3 * (size_t)l + 2], cam_centers, offsets[l], offsets[l + 1],
+                          ref_center + 3 * (size_t)l, ref_scale[l], inv_scale_last, mean_normal + 3 * (size_t)l, max_valid[l], min_valid[l]);
+}
+
+// b200_depth_landmarks: one CTA per problem.  Mode 0 sorts the (depth bits << 32 | idx) keys of the keypoints with 0 < depth in
+// shared memory (positive floats order like their bit patterns, and idx breaks ties, so the order is std::sort's on pair<float,
+// unsigned>); both modes then compact the walked positions with a block-wide scan so that every created landmark knows its slot.
+struct DepthLmDev {
+    int mode, n, n_valid, npow;  // n_valid / npow: mode 0's key count and its power-of-two padding
+    double rwc[9], twc[3];
+    double fx_inv, fy_inv, cx, cy, depth_thr;
+    const float *x, *y, *depth;
+    const int* octave;
+    const unsigned char* has_lm;  // may be null
+    const float* sf;
+    float inv_last;
+    int* out_idx;
+    double *pos_w, *mean_normal;
+    float *min_valid, *max_valid;
+    int* n_created;
+};
+constexpr int kDepthLmThreads = 512;
+
+// exclusive prefix of `flag` over the CTA (kDepthLmThreads threads, all of them calling); *total = the sum
+__device__ __forceinline__ int cta_exclusive_scan(int flag, int* s_warp, int* total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned ballot = __ballot_sync(0xffffffffu, flag);
+    const int in_warp = __popc(ballot & ((1u << lane) - 1u));
+    if (lane == 0) s_warp[warp] = __popc(ballot);
+    __syncthreads();
+    if (warp == 0) {
+        const int v = lane < kDepthLmThreads / 32 ? s_warp[lane] : 0;
+        int inc = v;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const int t = __shfl_up_sync(0xffffffffu, inc, d);
+            if (lane >= d) inc += t;
+        }
+        if (lane < kDepthLmThreads / 32) s_warp[lane] = inc - v;
+        if (lane == kDepthLmThreads / 32 - 1) *total = inc;
+    }
+    __syncthreads();
+    const int r = s_warp[warp] + in_warp;
+    __syncthreads();  // s_warp is reused by the next call
+    return r;
+}
+
+__global__ void __launch_bounds__(kDepthLmThreads) depth_landmarks_kernel(const DepthLmDev* __restrict__ probs) {
+    extern __shared__ unsigned long long s_keys[];
+    __shared__ int s_warp[32];
+    __shared__ int s_total, s_fill, s_le;
+    const DepthLmDev& P = probs[blockIdx.x];
+    if (P.n_created == nullptr) return;  // the host rejected this problem
+    const int tid = threadIdx.x;
+    int walk;  // positions walked: sorted keys (mode 0) or keypoint indices (mode 1)
+    if (P.mode == 0) {
+        if (tid == 0) s_fill = s_le = 0;
+        __syncthreads();
+        for (int i = tid; i < P.n; i += kDepthLmThreads) {
+            const float d = P.depth[i];
+            if (0.f < d) {
+                s_keys[atomicAdd(&s_fill, 1)] = ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)i;
+                if (!(P.depth_thr < (double)d)) atomicAdd(&s_le, 1);
+            }
+        }
+        __syncthreads();
+        for (int i = P.n_valid + tid; i < P.npow; i += kDepthLmThreads) s_keys[i] = ~0ull;
+        __syncthreads();
+        for (int k = 2; k <= P.npow; k <<= 1)  // bitonic sort, ascending
+            for (int j = k >> 1; j > 0; j >>= 1) {
+                for (int i = tid; i < P.npow; i += kDepthLmThreads) {
+                    const int ixj = i ^ j;
+                    if (ixj > i) {
+                        const unsigned long long a = s_keys[i], b = s_keys[ixj];
+                        if ((a > b) == ((i & k) == 0)) {
+                            s_keys[i] = b;
+                            s_keys[ixj] = a;
+                        }
+                    }
+                }
+                __syncthreads();
+            }
+        // keyframe_inserter.cc:187-191: stop at the first count with 100 < count && depth_thr < depth.  The depths ascend, so the keys
+        // with depth <= depth_thr are a prefix of s_le entries and the walk covers max(101, s_le) of them.
+        walk = min(P.n_valid, max(101, s_le));
+    } else {
+        walk = P.n;
+    }
+    int base_out = 0;
+    for (int p0 = 0; p0 < walk; p0 += kDepthLmThreads) {
+        const int p = p0 + tid;
+        int idx = -1;
+        if (p < walk) {
+            if (P.mode == 0) {
+                idx = (int)(unsigned)(s_keys[p] & 0xffffffffull);
+                if (P.has_lm && P.has_lm[idx]) idx = -1;  // keyframe_inserter.cc:194-200: skipped, count still advances
+            } else if (0.f < P.depth[p]) {
+                idx = p;
+            }
+        }
+        const int slot = base_out + cta_exclusive_scan(idx >= 0, s_warp, &s_total);
+        base_out += s_total;
+        if (idx < 0) continue;
+        // data::triangulate_stereo (data/common.cc:203-214): float x, y, depth; double cx_, fx_inv_
+        const double z = (double)P.depth[idx];
+        const double pc0 = (double)__double2float_rn(__dmul_rn(__dmul_rn(__dsub_rn((double)P.x[idx], P.cx), z), P.fx_inv));
+        const double pc1 = (double)__double2float_rn(__dmul_rn(__dmul_rn(__dsub_rn((double)P.y[idx], P.cy), z), P.fy_inv));
+        double pw[3];
+#pragma unroll
+        for (int r = 0; r < 3; ++r)
+            pw[r] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(P.rwc[3 * r], pc0), __dmul_rn(P.rwc[3 * r + 1], pc1)), __dmul_rn(P.rwc[3 * r + 2], z)), P.twc[r]);
+        P.out_idx[slot] = idx;
+        P.pos_w[3 * (size_t)slot] = pw[0];
+        P.pos_w[3 * (size_t)slot + 1] = pw[1];
+        P.pos_w[3 * (size_t)slot + 2] = pw[2];
+        landmark_geometry_one(pw[0], pw[1], pw[2], P.twc, 0, 1, P.twc, P.sf[P.octave[idx]], P.inv_last, P.mean_normal + 3 * (size_t)slot,
+                              P.max_valid[slot], P.min_valid[slot]);
+    }
+    if (tid == 0) *P.n_created = base_out;
 }
 
 struct Matcher {
@@ -2375,6 +2499,138 @@ int b200_landmark_geometry(b200_matcher_t h, int n_landmarks, const double* pos_
     std::memcpy(max_valid_dist, hb + o_mx, 4 * N);
     std::memcpy(min_valid_dist, hb + o_mi, 4 * N);
     return B200_OK;
+}
+
+int b200_depth_landmarks(b200_matcher_t h, int n_problems, b200_depth_landmarks_problem_t* problems) {
+    B200_RANGE("b200:match:depth_landmarks");
+    if (!h || n_problems < 0 || (n_problems > 0 && !problems)) return B200_ERR_INVALID;
+    using b200::match::DepthLmDev;
+    // validation on the host: the problems that fail it are not launched
+    std::vector<int> nv(n_problems, 0);
+    int first_bad = B200_OK;
+    for (int p = 0; p < n_problems; ++p) {
+        b200_depth_landmarks_problem_t& P = problems[p];
+        P.n_created = 0;
+        int st = B200_OK;
+        if ((P.mode != B200_DEPTH_LM_KEYFRAME && P.mode != B200_DEPTH_LM_INITIAL) || P.n_keypoints < 0 || P.num_levels < 1 || !P.scale_factors
+            || (P.n_keypoints > 0 && (!P.x || !P.y || !P.octave || !P.depth || !P.created_idx || !P.pos_w || !P.mean_normal || !P.min_valid_dist
+                                      || !P.max_valid_dist))) {
+            b200::set_error("b200_depth_landmarks: problem %d: bad mode, count or pointer", p);
+            st = B200_ERR_INVALID;
+        }
+        for (int i = 0; st == B200_OK && i < P.n_keypoints; ++i) {
+            if (!(0.f < P.depth[i])) continue;
+            ++nv[p];
+            if (P.model == 1) {
+                b200::set_error("b200_depth_landmarks: problem %d: equirectangular camera with a valid depth (data/common.cc:236-238 throws)", p);
+                st = B200_ERR_INVALID;
+            } else if (P.octave[i] < 0 || P.octave[i] >= P.num_levels) {
+                b200::set_error("b200_depth_landmarks: problem %d: keypoint %d has octave %d, the table has %d levels", p, i, P.octave[i], P.num_levels);
+                st = B200_ERR_INVALID;
+            }
+        }
+        if (st == B200_OK && P.mode == B200_DEPTH_LM_KEYFRAME && nv[p] > B200_DEPTH_LM_MAX_SORT) {
+            b200::set_error("b200_depth_landmarks: problem %d has %d keypoints with a valid depth, at most %d can be sorted", p, nv[p],
+                            B200_DEPTH_LM_MAX_SORT);
+            st = B200_ERR_CAPACITY;
+        }
+        P.status = st;
+        if (st != B200_OK && first_bad == B200_OK) first_bad = st;
+    }
+    // one pinned staging block: the problem table, then per problem its inputs (x, y, depth, octave, has_landmark, scale factors) and
+    // its outputs (n_created, idx, pos_w, mean_normal, min / max valid distance)
+    auto al = [](size_t v) { return b200::round_up(v, (size_t)256); };
+    struct Lay { size_t in, out, n, lv; };
+    std::vector<Lay> lay(n_problems);
+    size_t o = al(sizeof(DepthLmDev) * (size_t)std::max(n_problems, 1));
+    for (int p = 0; p < n_problems; ++p) {
+        const bool run = problems[p].status == B200_OK;
+        lay[p].n = run ? (size_t)problems[p].n_keypoints : 0;
+        lay[p].lv = run ? (size_t)problems[p].num_levels : 0;
+        lay[p].in = o;
+        o += 4 * al(4 * lay[p].n) + al(lay[p].n) + al(4 * lay[p].lv);
+    }
+    const size_t in_bytes = o;
+    for (int p = 0; p < n_problems; ++p) {
+        lay[p].out = o;
+        o += al(4) + al(4 * lay[p].n) + 2 * al(24 * lay[p].n) + 2 * al(4 * lay[p].n);
+    }
+    const size_t out_end = o;
+    auto& m = h->m;
+    B200_CUDA(cudaSetDevice(m.device));
+    int rc;
+    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, out_end))) return rc;
+    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, out_end))) return rc;
+    unsigned char *hb = m.h_guided, *db = m.d_guided;
+    DepthLmDev* dev = reinterpret_cast<DepthLmDev*>(hb);
+    int npow_max = 1;
+    for (int p = 0; p < n_problems; ++p) {
+        const b200_depth_landmarks_problem_t& P = problems[p];
+        DepthLmDev& D = dev[p];
+        std::memset(&D, 0, sizeof(D));
+        if (P.status != B200_OK) continue;  // n_created == nullptr: the kernel skips it
+        const size_t n = lay[p].n, a4 = al(4 * n);
+        size_t b = lay[p].in;
+        D.mode = P.mode;
+        D.n = P.n_keypoints;
+        D.n_valid = nv[p];
+        D.npow = 1;
+        if (P.mode == B200_DEPTH_LM_KEYFRAME)
+            while (D.npow < nv[p]) D.npow <<= 1;
+        npow_max = std::max(npow_max, D.npow);
+        for (int r = 0; r < 3; ++r) {
+            for (int c = 0; c < 3; ++c) D.rwc[3 * r + c] = P.pose_wc[4 * r + c];
+            D.twc[r] = P.pose_wc[4 * r + 3];
+        }
+        D.fx_inv = P.fx_inv; D.fy_inv = P.fy_inv; D.cx = P.cx; D.cy = P.cy; D.depth_thr = P.depth_thr;
+        D.inv_last = P.inv_scale_factor_last;
+        if (n) {
+            std::memcpy(hb + b, P.x, 4 * n);              D.x = (const float*)(db + b);      b += a4;
+            std::memcpy(hb + b, P.y, 4 * n);              D.y = (const float*)(db + b);      b += a4;
+            std::memcpy(hb + b, P.depth, 4 * n);          D.depth = (const float*)(db + b);  b += a4;
+            std::memcpy(hb + b, P.octave, 4 * n);         D.octave = (const int*)(db + b);   b += a4;
+            if (P.has_landmark && P.mode == B200_DEPTH_LM_KEYFRAME) {
+                std::memcpy(hb + b, P.has_landmark, n);
+                D.has_lm = db + b;
+            }
+            b += al(n);
+        }
+        std::memcpy(hb + b, P.scale_factors, 4 * lay[p].lv);
+        D.sf = (const float*)(db + b);
+        size_t q = lay[p].out;
+        D.n_created = (int*)(db + q);          q += al(4);
+        D.out_idx = (int*)(db + q);            q += a4;
+        D.pos_w = (double*)(db + q);           q += al(24 * n);
+        D.mean_normal = (double*)(db + q);     q += al(24 * n);
+        D.min_valid = (float*)(db + q);        q += a4;
+        D.max_valid = (float*)(db + q);
+    }
+    if (n_problems == 0) return B200_OK;
+    cudaStream_t st = m.stream;
+    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaMemsetAsync(db + in_bytes, 0, out_end - in_bytes, st));
+    const size_t smem = sizeof(unsigned long long) * (size_t)npow_max;
+    B200_CUDA(cudaFuncSetAttribute(b200::match::depth_landmarks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    b200::match::depth_landmarks_kernel<<<n_problems, b200::match::kDepthLmThreads, smem, st>>>((const DepthLmDev*)db);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaMemcpyAsync(hb + in_bytes, db + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    for (int p = 0; p < n_problems; ++p) {
+        b200_depth_landmarks_problem_t& P = problems[p];
+        if (P.status != B200_OK) continue;
+        const size_t n = lay[p].n, a4 = al(4 * n);
+        size_t q = lay[p].out;
+        int k = 0;
+        std::memcpy(&k, hb + q, 4);            q += al(4);
+        P.n_created = k;
+        const size_t K = (size_t)k;
+        std::memcpy(P.created_idx, hb + q, 4 * K);      q += a4;
+        std::memcpy(P.pos_w, hb + q, 24 * K);           q += al(24 * n);
+        std::memcpy(P.mean_normal, hb + q, 24 * K);     q += al(24 * n);
+        std::memcpy(P.min_valid_dist, hb + q, 4 * K);   q += a4;
+        std::memcpy(P.max_valid_dist, hb + q, 4 * K);
+    }
+    return first_bad;
 }
 
 int b200_match_cross_check(const int32_t* idx2_in_1, int n1, const int32_t* idx1_in_2, int n2, int32_t* mutual_out, int32_t* n_mutual) {

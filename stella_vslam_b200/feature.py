@@ -155,6 +155,35 @@ class orb_extractor:
             check(lib().b200_keypoints_undistort(self._h, C.byref(cam), ptr(kps), n, ptr(out), ptr(bearings)))
         return out, bearings
 
+    def rgbd_depths(self, camera, depth_maps, depthmap_factor, focal_x_baseline, n_frames=None, cap=None):
+        """system::create_RGBD_frame after the extraction (system.cc:467-530) for the first n_frames frames of the last extract (all of
+        them by default): undistorted keypoints and bearings as undistort_keypoints gives them, the depth sampled at each distorted
+        keypoint after util::convert_to_true_depth(depthmap_factor), and x_right = undist_x - focal_x_baseline / depth (-1 / -1 where
+        the depth is not positive).  depth_maps: (h, w) or (n, h, w) uint16 (CV_16UC1) or float32 (CV_32FC1) numpy array of the
+        extracted frames' size.  Returns one dict(undist_keypts, bearings, depths, x_right) per frame."""
+        maps = np.asarray(depth_maps)
+        if maps.ndim == 2:
+            maps = maps[None]
+        types = {np.dtype(np.uint16): 2, np.dtype(np.float32): 5}  # B200_DEPTH_16UC1 / B200_DEPTH_32FC1
+        if maps.ndim != 3 or maps.dtype not in types:
+            raise ValueError(f"depth maps must be (h, w) or (n, h, w) uint16 or float32 arrays, got {maps.dtype} {maps.shape}")
+        maps = np.ascontiguousarray(maps)
+        n = maps.shape[0] if n_frames is None else int(n_frames)
+        if n > maps.shape[0]:
+            raise ValueError(f"{n} frames requested, {maps.shape[0]} depth maps given")
+        if cap is None:
+            cap = check_pos(lib().b200_orb_max_keypoints(self._h, maps.shape[2], maps.shape[1]))
+        und = np.zeros((max(n, 1), max(cap, 1)), KP_DTYPE)
+        bearings = np.zeros((max(n, 1), max(cap, 1), 3))
+        depths, x_right = np.zeros((max(n, 1), max(cap, 1)), np.float32), np.zeros((max(n, 1), max(cap, 1)), np.float32)
+        counts = np.zeros(max(n, 1), np.int32)
+        cam = _lib.camera_intrinsics(camera)
+        check(lib().b200_rgbd_depths(self._h, n, C.byref(cam), float(focal_x_baseline), float(depthmap_factor), types[maps.dtype], ptr(maps),
+                                     maps.shape[2], maps.shape[1], maps.strides[1], maps.strides[0], cap, ptr(und), ptr(bearings), ptr(depths),
+                                     ptr(x_right), ptr(counts)))
+        return [dict(undist_keypts=und[f, :counts[f]].copy(), bearings=bearings[f, :counts[f]].copy(), depths=depths[f, :counts[f]].copy(),
+                     x_right=x_right[f, :counts[f]].copy()) for f in range(n)]
+
     def can_observe(self, camera, pose_cw, landmarks, ray_cos_thr=0.5, img_bounds=None):
         """data::frame::can_observe (data/frame.cc:59-84) for the local landmarks (tracking_module.cc:559-594).
         landmarks: dict(pos_w (n,3), mean_normal (n,3), min_valid_dist (n,), max_valid_dist (n,)).

@@ -199,6 +199,59 @@ def create_new_landmarks(cur_keyfrm, neighbours, lowe_ratio=0.95, residual_deg_t
     return create_new_landmarks_batch([(cur_keyfrm, neighbours)], lowe_ratio, residual_deg_thr * np.pi / 180.0, bow=bow, **kw)[0]
 
 
+class DepthLandmarksProblem(C.Structure):
+    """b200_depth_landmarks_problem_t."""
+    _fields_ = [("mode", C.c_int32), ("model", C.c_int32), ("pose_wc", C.c_double * 16), ("fx_inv", C.c_double), ("fy_inv", C.c_double),
+                ("cx", C.c_double), ("cy", C.c_double), ("depth_thr", C.c_double), ("n_keypoints", C.c_int32), ("x", C.c_void_p),
+                ("y", C.c_void_p), ("octave", C.c_void_p), ("depth", C.c_void_p), ("has_landmark", C.c_void_p), ("num_levels", C.c_int32),
+                ("scale_factors", C.c_void_p), ("inv_scale_factor_last", C.c_float), ("created_idx", C.c_void_p), ("pos_w", C.c_void_p),
+                ("mean_normal", C.c_void_p), ("min_valid_dist", C.c_void_p), ("max_valid_dist", C.c_void_p), ("n_created", C.c_int32),
+                ("status", C.c_int32)]
+
+
+DEPTH_LANDMARKS_KEYFRAME, DEPTH_LANDMARKS_INITIAL = 0, 1
+DEPTH_LANDMARKS_MAX_SORT = 8192  # B200_DEPTH_LM_MAX_SORT: keypoints with a valid depth one mode-0 problem may have
+
+
+def depth_landmarks(problems, device=0, raise_on_error=True):
+    """b200_depth_landmarks: the landmarks a stereo / RGB-D keyframe makes straight from its depths, for many frames in one call.
+    Each problem is a dict: mode (0 = keyframe_inserter::create_new_keyframe, 1 = initializer::create_map_for_stereo), model (camera
+    model code, default 0), pose_wc (4x4), fx_inv, fy_inv, cx, cy, depth_thr (mode 0), x, y, octave, depth (per undistorted keypoint),
+    has_landmark (mode 0, optional), scale_factors, inv_scale_factor_last.  Returns per problem dict(idx, pos_w, mean_normal,
+    min_valid_dist, max_valid_dist, status) with the landmarks in creation order.  raise_on_error=False returns the per-problem status
+    (0, or the B200 error code of a rejected problem) instead of raising."""
+    keep, arr = [], (DepthLandmarksProblem * max(len(problems), 1))()
+    outs = []
+    for k, pr in enumerate(problems):
+        P = arr[k]
+        n = len(pr["x"])
+        P.mode, P.model = int(pr["mode"]), int(pr.get("model", 0))
+        pose = np.asarray(pr["pose_wc"], np.float64).reshape(16)
+        for e in range(16):
+            P.pose_wc[e] = float(pose[e])
+        P.fx_inv, P.fy_inv, P.cx, P.cy = (float(pr[f]) for f in ("fx_inv", "fy_inv", "cx", "cy"))
+        P.depth_thr = float(pr.get("depth_thr", 0.0))
+        P.n_keypoints = n
+        P.x, P.y = _arr(keep, pr["x"], np.float32), _arr(keep, pr["y"], np.float32)
+        P.octave, P.depth = _arr(keep, pr["octave"], np.int32), _arr(keep, pr["depth"], np.float32)
+        P.has_landmark = _arr(keep, pr.get("has_landmark"), np.uint8)
+        sf = np.asarray(pr["scale_factors"], np.float32)
+        P.num_levels, P.scale_factors = len(sf), _arr(keep, sf, np.float32)
+        P.inv_scale_factor_last = float(pr["inv_scale_factor_last"])
+        m = max(n, 1)
+        o = dict(idx=np.zeros(m, np.int32), pos_w=np.zeros((m, 3)), mean_normal=np.zeros((m, 3)), min_valid_dist=np.zeros(m, np.float32),
+                 max_valid_dist=np.zeros(m, np.float32))
+        keep.append(o)
+        P.created_idx, P.pos_w, P.mean_normal = o["idx"].ctypes.data, o["pos_w"].ctypes.data, o["mean_normal"].ctypes.data
+        P.min_valid_dist, P.max_valid_dist = o["min_valid_dist"].ctypes.data, o["max_valid_dist"].ctypes.data
+        outs.append(o)
+    _setup()
+    rc = lib().b200_depth_landmarks(_matcher(device), len(problems), arr)
+    if raise_on_error:
+        check(rc)
+    return [dict({f: v[:arr[k].n_created].copy() for f, v in o.items()}, status=int(arr[k].status)) for k, o in enumerate(outs)]
+
+
 _argtypes_set = False
 
 
@@ -209,4 +262,5 @@ def _setup():
     L = lib()
     L.b200_triangulate_pairs.argtypes = [C.c_void_p, C.c_int, C.POINTER(TriangulateProblem)]
     L.b200_create_new_landmarks.argtypes = [C.c_void_p, C.c_int, C.POINTER(NewLandmarksProblem), C.c_float, C.c_float, C.c_float, C.c_int]
+    L.b200_depth_landmarks.argtypes = [C.c_void_p, C.c_int, C.POINTER(DepthLandmarksProblem)]
     _argtypes_set = True

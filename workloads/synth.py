@@ -1075,3 +1075,35 @@ def make_sim3_pair(seed=0, n_matches=300, models=("perspective", "perspective"),
     return dict(n_matches=n, fix_scale=bool(fix_scale), sim3_12=init, rot_1w=R1, trans_1w=t1, rot_2w=rot_2w, trans_2w=trans_2w, cam_1=cam1,
                 cam_2=cam2, obs_1=obs_1.astype(np.float32), inv_sigma_sq_1=inv_sigma[lv1], pos_w_2=pos_w_2, obs_2=obs_2.astype(np.float32),
                 inv_sigma_sq_2=inv_sigma[lv2], pos_w_1=pos_w_1, gt_sim3_12=gt, gt_outlier=bad)
+
+
+def make_rgbd_frames(w=640, h=480, seed=0, depthmap_factor=5000.0, n_planes=4, hole_frac=0.05, saturated_frac=0.01, float_specials_frac=0.03):
+    """An RGB-D frame as a TUM RGB-D sensor gives it: the gray frame of make_frame and a depth map built from a few planes between 0.3 and
+    10 m.  Returns (gray u8 (h, w), depth u16 (h, w) at `depthmap_factor` counts per metre, depth f32 (h, w) in metres).
+    The u16 map has zero-depth holes and saturated (65535) pixels; the f32 variant is the u16 map over the factor, with NaN, negative
+    values and +inf sprinkled in."""
+    rng = np.random.default_rng(seed)
+    gray = make_frame(w, h, seed=seed)
+    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
+    depth = np.full((h, w), np.inf)
+    for _ in range(n_planes):  # z = z0 + gx * (x - cx) + gy * (y - cy) over a random rectangle; the nearest plane wins
+        z0 = rng.uniform(0.3, 10.0)
+        gx, gy = rng.uniform(-4e-3, 4e-3, 2)
+        x0, y0 = rng.integers(0, w // 2), rng.integers(0, h // 2)
+        x1, y1 = rng.integers(x0 + w // 4, w + 1), rng.integers(y0 + h // 4, h + 1)
+        z = np.clip(z0 + gx * (xx - w / 2) + gy * (yy - h / 2), 0.3, 10.0)
+        inside = (xx >= x0) & (xx < x1) & (yy >= y0) & (yy < y1)
+        depth = np.where(inside & (z < depth), z, depth)
+    depth = np.where(np.isinf(depth), rng.uniform(0.3, 10.0), depth)  # background wall
+    d16 = np.clip(np.rint(depth * depthmap_factor), 0, 65535).astype(np.uint16)
+    holes = rng.random((h, w)) < hole_frac
+    holes |= (xx >= rng.integers(0, w - 40)) & (xx < rng.integers(40, w)) & (yy < 12)  # a dropped band, as structured-light sensors lose
+    d16[holes] = 0
+    d16[rng.random((h, w)) < saturated_frac] = 65535
+    d32 = (d16.astype(np.float32) * np.float32(1.0 / depthmap_factor)).astype(np.float32)
+    special = rng.random((h, w)) < float_specials_frac
+    kinds = rng.integers(0, 3, (h, w))
+    d32[special & (kinds == 0)] = np.nan
+    d32[special & (kinds == 1)] = -rng.uniform(0.1, 5.0, int((special & (kinds == 1)).sum())).astype(np.float32)
+    d32[special & (kinds == 2)] = np.inf
+    return gray, d16, d32
