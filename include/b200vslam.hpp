@@ -672,11 +672,28 @@ private:
 namespace b200 {
 namespace solve {
 
-// util::create_random_array(4, 0, n - 1, engine), max_num_iter times from one engine (b200_pnp_draw_min_sets), max_num_iter x 4
-inline std::vector<int32_t> draw_min_sets(b200_mt19937_t& engine, uint32_t n_matches, uint32_t max_num_iter) {
-    std::vector<int32_t> out(4 * (size_t)max_num_iter);
-    check(b200_pnp_draw_min_sets(&engine, n_matches, max_num_iter, out.data()), "b200_pnp_draw_min_sets");
+// util::create_random_engine: a default-constructed engine, or one seeded by std::seed_seq over ten std::random_device words
+inline void create_random_engine(b200_mt19937_t& engine, bool use_fixed_seed) {
+    if (use_fixed_seed) {
+        check(b200_mt19937_seed(&engine, nullptr, 0), "b200_mt19937_seed");
+        return;
+    }
+    std::random_device rd;
+    uint32_t words[10];
+    for (auto& w : words) w = rd();
+    check(b200_mt19937_seed(&engine, words, 10), "b200_mt19937_seed");
+}
+
+// util::create_random_array(set_size, 0, n - 1, engine), max_num_iter times from one engine (b200_draw_min_sets), max_num_iter x set_size
+inline std::vector<int32_t> draw_min_sets(b200_mt19937_t& engine, uint32_t set_size, uint32_t n_matches, uint32_t max_num_iter) {
+    std::vector<int32_t> out((size_t)set_size * max_num_iter);
+    check(b200_draw_min_sets(&engine, set_size, n_matches, max_num_iter, out.data()), "b200_draw_min_sets");
     return out;
+}
+
+// PnP's minimal sets of 4
+inline std::vector<int32_t> draw_min_sets(b200_mt19937_t& engine, uint32_t n_matches, uint32_t max_num_iter) {
+    return draw_min_sets(engine, 4, n_matches, max_num_iter);
 }
 
 // find_via_ransac for many problems in one call (b200_pnp_ransac); the problems' out fields are filled
@@ -697,14 +714,7 @@ public:
             throw std::invalid_argument("pnp_solver: bearings, octaves and points must have one entry per match");
         for (int32_t o : octaves_)
             if (o < 0 || (size_t)o >= scale_factors_.size()) throw std::out_of_range("pnp_solver: octave outside the scale factors");
-        if (use_fixed_seed) {  // util::create_random_engine
-            check(b200_mt19937_seed(&engine_, nullptr, 0), "b200_mt19937_seed");
-        } else {
-            std::random_device rd;
-            uint32_t words[10];
-            for (auto& w : words) w = rd();
-            check(b200_mt19937_seed(&engine_, words, 10), "b200_mt19937_seed");
-        }
+        create_random_engine(engine_, use_fixed_seed);
         if (!h_) {
             check(b200_lba_create(0, &h_), "b200_lba_create");
             own_ = true;
@@ -787,14 +797,6 @@ private:
     std::vector<bool> is_inlier_match_;
 };
 
-
-// util::create_random_array(set_size, 0, n - 1, engine), max_num_iter times from one engine (b200_draw_min_sets), max_num_iter x set_size
-inline std::vector<int32_t> draw_min_sets(b200_mt19937_t& engine, uint32_t set_size, uint32_t n_matches, uint32_t max_num_iter) {
-    std::vector<int32_t> out((size_t)set_size * max_num_iter);
-    check(b200_draw_min_sets(&engine, set_size, n_matches, max_num_iter, out.data()), "b200_draw_min_sets");
-    return out;
-}
-
 // essential_solver::find_via_ransac for many problems in one call (b200_essential_ransac); the problems' out fields are filled
 inline void essential_ransac_batch(b200_lba_t h, std::vector<b200_essential_problem_t>& problems) {
     check(b200_essential_ransac(h, (int)problems.size(), problems.data()), "b200_essential_ransac");
@@ -816,14 +818,7 @@ public:
             b1_.insert(b1_.end(), bearings_1.begin() + 3 * m.first, bearings_1.begin() + 3 * m.first + 3);
             b2_.insert(b2_.end(), bearings_2.begin() + 3 * m.second, bearings_2.begin() + 3 * m.second + 3);
         }
-        if (use_fixed_seed) {  // util::create_random_engine
-            check(b200_mt19937_seed(&engine_, nullptr, 0), "b200_mt19937_seed");
-        } else {
-            std::random_device rd;
-            uint32_t words[10];
-            for (auto& w : words) w = rd();
-            check(b200_mt19937_seed(&engine_, words, 10), "b200_mt19937_seed");
-        }
+        create_random_engine(engine_, use_fixed_seed);
     }
     ~essential_solver() {
         if (own_) b200_lba_destroy(h_);

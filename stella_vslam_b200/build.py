@@ -21,6 +21,7 @@ SOURCES = {
     "lba_kernels.cu": [],
     # the rectification maps are built on the host in double; keep the host compiler from contracting them to FMA
     "rectify_kernels.cu": ["-Xcompiler", "-ffp-contract=off"],
+    "random_array.cu": [],
     "pnp_kernels.cu": [],
     "essential_kernels.cu": [],
     "twoview_kernels.cu": [],

@@ -1,6 +1,6 @@
 // essential_kernels.cu -- solve::essential_solver (src/stella_vslam/solve/essential_solver.cc) on the device: find_via_ransac with the
-// five-point minimal set for many problems in one launch sequence on the b200_lba_t handle's stream, and the host-side restatement of
-// util::create_random_array for any set size.
+// five-point minimal set for many problems in one launch sequence on the b200_lba_t handle's stream.  The minimal sets are drawn on the
+// host (random_array.cu).
 //
 // find_via_ransac is split in three launches:
 //   essential_hypothesis_kernel  one thread per (problem, iteration): compute_E_21_minimal on the minimal set (essential_core.h),
@@ -19,16 +19,10 @@
 
 #include "common.cuh"
 #include "epnp.cuh"
+#include "ransac_host.cuh"
 #include "util_trig.cuh"
 
 namespace b200 {
-namespace lba {
-int borrow_buffers(b200_lba_t h, size_t dev_bytes, size_t host_bytes, cudaStream_t* stream, unsigned char** d, unsigned char** hst);
-}
-namespace pnp {
-uint32_t uniform_below(b200_mt19937_t* e, uint32_t range);
-}
-
 namespace ess {
 
 using pnp::apply_householder_left;
@@ -38,15 +32,7 @@ using tri::dd;
 using tri::dm;
 using tri::ds;
 
-#define ES_FN __device__
-#define ES_BIG __device__ __noinline__
-#define ES_SQRT(x) __dsqrt_rn(x)
-#define ES_MAKE_HOUSEHOLDER(v, len, stride, tau, beta) pnp::make_householder((v), (len), (stride), (tau), (beta))
-#include "essential_core.h"
-#undef ES_FN
-#undef ES_BIG
-#undef ES_SQRT
-#undef ES_MAKE_HOUSEHOLDER
+#include "essential_core.cuh"
 
 constexpr int kMinSet = 5;
 constexpr int kMaxCand = 10;
@@ -155,64 +141,17 @@ __global__ void __launch_bounds__(64) essential_select_kernel(int n_problems, co
     es_check_inliers(pb1, pb2, P.n, r.E, thr, fl, &cost);
     if (P.recompute && r.num_inliers >= 8) {
         int32_t* idx = idx_scratch + P.match_off;
-        int m = 0;
-        for (int j = 0; j < P.n; ++j)
-            if (fl[j]) idx[m++] = j;
+        const int m = compact_inliers(fl, P.n, idx);
         r.status |= es_nonminimal(pb1, pb2, idx, m, mat_scratch + 9 * (size_t)P.match_off, r.E);
         es_check_inliers(pb1, pb2, P.n, r.E, thr, fl, &r.best_cost);
     }
     results[q] = r;
 }
 
-// util::create_random_array(set_size, 0, n - 1, engine) as libstdc++ evaluates it: make_size = size_t(set_size * 1.2) draws of
-// uniform_int_distribution<unsigned>, sort + unique (truncated to set_size), repeated until set_size remain, then std::shuffle.
-void create_random_array(b200_mt19937_t* e, uint32_t set_size, uint32_t n, uint32_t* v, int32_t* out) {
-    const size_t make_size = (size_t)(set_size * 1.2);
-    size_t size = 0;
-    while (size != set_size) {
-        while (size < make_size) v[size++] = pnp::uniform_below(e, n);
-        for (size_t i = 1; i < size; ++i)
-            for (size_t j = i; j > 0 && v[j - 1] > v[j]; --j) {
-                const uint32_t t = v[j];
-                v[j] = v[j - 1];
-                v[j - 1] = t;
-            }
-        size_t u = 0;
-        for (size_t i = 0; i < size; ++i)
-            if (u == 0 || v[u - 1] != v[i]) v[u++] = v[i];
-        size = u < set_size ? u : set_size;
-    }
-    // std::shuffle: with a 32-bit engine and set_size^2 <= 2^32 - 1, swap positions come in pairs from one draw
-    uint32_t t;
-    size_t i = 1;
-    if (set_size % 2 == 0) {
-        const uint32_t d = pnp::uniform_below(e, 2);
-        t = v[i], v[i] = v[d], v[d] = t;
-        ++i;
-    }
-    while (i < set_size) {
-        const uint32_t r = (uint32_t)i + 1;
-        const uint32_t x = pnp::uniform_below(e, r * (r + 1));
-        t = v[i], v[i] = v[x / (r + 1)], v[x / (r + 1)] = t;
-        ++i;
-        t = v[i], v[i] = v[x % (r + 1)], v[x % (r + 1)] = t;
-        ++i;
-    }
-    for (uint32_t k = 0; k < set_size; ++k) out[k] = (int32_t)v[k];
-}
-
 }  // namespace ess
 }  // namespace b200
 
 extern "C" {
-
-int b200_draw_min_sets(b200_mt19937_t* e, uint32_t set_size, uint32_t n_matches, uint32_t max_num_iter, int32_t* out) {
-    // set_size <= 65535 keeps set_size^2 within the engine's range (the paired shuffle) and the products below in 32 bits
-    if (!e || set_size < 1 || set_size > 65535u || n_matches < set_size || (max_num_iter > 0 && !out)) return B200_ERR_INVALID;
-    std::vector<uint32_t> v((size_t)(set_size * 1.2) + set_size);
-    for (uint32_t it = 0; it < max_num_iter; ++it) b200::ess::create_random_array(e, set_size, n_matches, v.data(), out + (size_t)set_size * it);
-    return B200_OK;
-}
 
 int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t* problems) {
     B200_RANGE("b200:essential:ransac");
@@ -234,16 +173,8 @@ int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t
             return B200_ERR_INVALID;
         }
         const bool runs = n >= kMinSet;
+        if (!b200::min_sets_ok("b200_essential_ransac", q, runs, P.max_num_iter, P.min_sets, kMinSet, n)) return B200_ERR_INVALID;
         const int n_hyp = runs ? (int)P.max_num_iter : 0;
-        if (runs && (P.max_num_iter > (uint32_t)INT_MAX || (n_hyp > 0 && !P.min_sets))) {
-            b200::set_error("b200_essential_ransac: problem %d: bad max_num_iter or null min_sets", q);
-            return B200_ERR_INVALID;
-        }
-        for (long long k = 0; k < (long long)kMinSet * n_hyp; ++k)
-            if (P.min_sets[k] < 0 || P.min_sets[k] >= n) {
-                b200::set_error("b200_essential_ransac: problem %d: min_sets entry %lld = %d outside [0, %d)", q, k, P.min_sets[k], n);
-                return B200_ERR_INVALID;
-            }
         pd[q] = ProblemDev{n, (int)total, (int)total_hyp, n_hyp, runs, P.recompute != 0};
         total += n;
         total_hyp += n_hyp;
@@ -253,25 +184,19 @@ int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t
         }
     }
     const size_t T = (size_t)std::max(total, 1LL), NH = (size_t)std::max(total_hyp, 1LL);
-    auto al = [](size_t& o, size_t bytes) {
-        const size_t r = o;
-        o = b200::round_up(o + bytes, (size_t)256);
-        return r;
-    };
-    size_t o = 0;
-    const size_t o_probs = al(o, sizeof(ProblemDev) * n_problems), o_b1 = al(o, 24 * T), o_b2 = al(o, 24 * T);
-    const size_t o_ms = al(o, 4 * kMinSet * NH), o_hp = al(o, 4 * NH);
-    const size_t in_bytes = o;
-    const size_t o_res = al(o, sizeof(ResultDev) * n_problems), o_fl = al(o, T);
-    const size_t out_end = o;
-    const size_t o_cand = al(o, 8 * 9 * kMaxCand * NH), o_hyp = al(o, sizeof(HypDev) * NH), o_sc = al(o, sizeof(ScoreDev) * kMaxCand * NH);
-    const size_t o_idx = al(o, 4 * T), o_mat = al(o, 72 * T);
+    b200::Staging a;
+    const size_t o_probs = a.take(sizeof(ProblemDev) * n_problems), o_b1 = a.take(24 * T), o_b2 = a.take(24 * T);
+    const size_t o_ms = a.take(4 * kMinSet * NH), o_hp = a.take(4 * NH);
+    const size_t in_bytes = a.end;
+    const size_t o_res = a.take(sizeof(ResultDev) * n_problems), o_fl = a.take(T);
+    const size_t out_end = a.end;
+    const size_t o_cand = a.take(8 * 9 * kMaxCand * NH), o_hyp = a.take(sizeof(HypDev) * NH), o_sc = a.take(sizeof(ScoreDev) * kMaxCand * NH);
+    const size_t o_idx = a.take(4 * T), o_mat = a.take(72 * T);
     cudaStream_t st;
     unsigned char *db, *hb;
-    int rc = b200::lba::borrow_buffers(h, o, out_end, &st, &db, &hb);
+    int rc = b200::lba::borrow_buffers(h, a.end, out_end, &st, &db, &hb);
     if (rc) return rc;
     std::memcpy(hb + o_probs, pd.data(), sizeof(ProblemDev) * n_problems);
-    int* hyp_problem = reinterpret_cast<int*>(hb + o_hp);
     for (int q = 0; q < n_problems; ++q) {
         const b200_essential_problem_t& P = problems[q];
         const size_t off = (size_t)pd[q].match_off, n = (size_t)P.n_matches;
@@ -279,8 +204,8 @@ int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t
             std::memcpy(hb + o_b1 + 24 * off, P.bearings_1, 24 * n);
             std::memcpy(hb + o_b2 + 24 * off, P.bearings_2, 24 * n);
         }
-        if (pd[q].n_hyp) std::memcpy(hb + o_ms + 4 * kMinSet * (size_t)pd[q].hyp_off, P.min_sets, 4 * kMinSet * (size_t)pd[q].n_hyp);
-        for (int k = 0; k < pd[q].n_hyp; ++k) hyp_problem[pd[q].hyp_off + k] = q;
+        b200::stage_min_sets(q, P.min_sets, kMinSet, pd[q].n_hyp, kMinSet * (size_t)pd[q].hyp_off, pd[q].hyp_off, (int32_t*)(hb + o_ms),
+                             (int*)(hb + o_hp));
     }
     B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
     const double* d_b1 = (const double*)(db + o_b1);

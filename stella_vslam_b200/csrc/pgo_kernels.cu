@@ -26,9 +26,6 @@
 #include "sim3.cuh"
 
 namespace b200 {
-namespace lba {
-int borrow_buffers(b200_lba_t h, size_t dev_bytes, size_t host_bytes, cudaStream_t* stream, unsigned char** d, unsigned char** hst);
-}
 
 namespace pgo {
 

@@ -1,6 +1,5 @@
 // pnp_kernels.cu -- solve::pnp_solver (src/stella_vslam/solve/pnp_solver.cc) on the device: find_via_ransac for many problems in one
-// launch sequence, the static compute_pose, and the host-side restatement of the minimal-set sampler (util::create_random_array on
-// std::mt19937, src/stella_vslam/util/random_array.cc).
+// launch sequence, and the static compute_pose.  The minimal sets are drawn on the host (random_array.cu).
 //
 // find_via_ransac is split in two launches:
 //   pnp_hypothesis_kernel  one thread per (problem, hypothesis): EPnP on the minimal set (epnp.cuh), then check_inliers' cost summed
@@ -16,13 +15,10 @@
 
 #include "common.cuh"
 #include "epnp.cuh"
+#include "ransac_host.cuh"
 #include "util_trig.cuh"
 
 namespace b200 {
-namespace lba {
-int borrow_buffers(b200_lba_t h, size_t dev_bytes, size_t host_bytes, cudaStream_t* stream, unsigned char** d, unsigned char** hst);
-}
-
 namespace pnp {
 
 struct ProblemDev {
@@ -142,9 +138,7 @@ __global__ void __launch_bounds__(64) pnp_select_kernel(int n_problems, const Pr
     check_inliers(b, p, max_cos + P.match_off, P.n, r.R, r.t, fl, cost);
     if (P.recompute) {
         int32_t* idx = idx_scratch + P.match_off;
-        int m = 0;
-        for (int j = 0; j < P.n; ++j)
-            if (fl[j]) idx[m++] = j;
+        const int m = compact_inliers(fl, P.n, idx);
         bool wrote;
         int status;
         compute_pose(Pts{b, p, idx, m}, P.gn_iter, r.R, r.t, wrote, status);
@@ -173,113 +167,10 @@ __global__ void __launch_bounds__(64) epnp_kernel(int n_problems, const double* 
     probs[q] = E;
 }
 
-// ---------------------------------------------------------------------------------------------------------------------------------
-// std::mt19937 and util::create_random_array(4, 0, n - 1, engine) as libstdc++ evaluates them
-
-void mt_twist(b200_mt19937_t* e) {
-    uint32_t* x = e->state;
-    for (int k = 0; k < 624; ++k) {
-        const uint32_t y = (x[k] & 0x80000000u) | (x[(k + 1) % 624] & 0x7fffffffu);
-        x[k] = x[(k + 397) % 624] ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
-    }
-    e->index = 0;
-}
-
-uint32_t mt_next(b200_mt19937_t* e) {
-    if (e->index >= 624) mt_twist(e);
-    uint32_t y = e->state[e->index++];
-    y ^= y >> 11;
-    y ^= (y << 7) & 0x9d2c5680u;
-    y ^= (y << 15) & 0xefc60000u;
-    y ^= y >> 18;
-    return y;
-}
-
-// uniform_int_distribution{0, range - 1} on a 32-bit engine: Lemire's nearly divisionless method (libstdc++ _S_nd)
-uint32_t uniform_below(b200_mt19937_t* e, uint32_t range) {
-    uint64_t product = (uint64_t)mt_next(e) * range;
-    uint32_t low = (uint32_t)product;
-    if (low < range) {
-        const uint32_t threshold = (uint32_t)(0u - range) % range;
-        while (low < threshold) {
-            product = (uint64_t)mt_next(e) * range;
-            low = (uint32_t)product;
-        }
-    }
-    return (uint32_t)(product >> 32);
-}
-
-void create_random_array4(b200_mt19937_t* e, uint32_t n, int32_t* out) {
-    uint32_t v[8];
-    int size = 0;
-    while (size != 4) {
-        while (size < 4) v[size++] = uniform_below(e, n);  // make_size = size_t(4 * 1.2) = 4
-        // sort + unique
-        for (int i = 1; i < size; ++i)
-            for (int j = i; j > 0 && v[j - 1] > v[j]; --j) {
-                const uint32_t t = v[j];
-                v[j] = v[j - 1];
-                v[j - 1] = t;
-            }
-        int u = 0;
-        for (int i = 0; i < size; ++i)
-            if (u == 0 || v[u - 1] != v[i]) v[u++] = v[i];
-        size = u;
-    }
-    // std::shuffle of 4 elements: (urngrange / 4 >= 4) -> one swap with {0, 1}, then a pair from one draw in {0, 3 * 4 - 1}
-    uint32_t t;
-    const uint32_t d = uniform_below(e, 2);
-    t = v[1], v[1] = v[d], v[d] = t;
-    const uint32_t x = uniform_below(e, 12);
-    t = v[2], v[2] = v[x / 4], v[x / 4] = t;
-    t = v[3], v[3] = v[x % 4], v[x % 4] = t;
-    for (int i = 0; i < 4; ++i) out[i] = (int32_t)v[i];
-}
-
 }  // namespace pnp
 }  // namespace b200
 
 extern "C" {
-
-int b200_mt19937_seed(b200_mt19937_t* e, const uint32_t* seed_seq, int n_seed) {
-    if (!e || n_seed < 0 || (n_seed > 0 && !seed_seq)) return B200_ERR_INVALID;
-    uint32_t* x = e->state;
-    if (n_seed == 0) {
-        x[0] = 5489u;
-        for (uint32_t i = 1; i < 624; ++i) x[i] = 1812433253u * (x[i - 1] ^ (x[i - 1] >> 30)) + i;
-    } else {  // std::seed_seq::generate over 624 words, then mersenne_twister_engine::seed(seed_seq&)
-        const uint32_t n = 624, s = (uint32_t)n_seed, t = 11, p = (n - t) / 2, q = p + t, m = (s + 1 > n) ? s + 1 : n;
-        for (uint32_t k = 0; k < n; ++k) x[k] = 0x8b8b8b8bu;
-        auto T = [](uint32_t v) { return v ^ (v >> 27); };
-        for (uint32_t k = 0; k < m; ++k) {
-            const uint32_t r1 = 1664525u * T(x[k % n] ^ x[(k + p) % n] ^ x[(k + n - 1) % n]);
-            const uint32_t r2 = r1 + (k == 0 ? s : (k <= s ? k % n + seed_seq[k - 1] : k % n));
-            x[(k + p) % n] += r1;
-            x[(k + q) % n] += r2;
-            x[k % n] = r2;
-        }
-        for (uint32_t k = m; k < m + n; ++k) {
-            const uint32_t r3 = 1566083941u * T(x[k % n] + x[(k + p) % n] + x[(k + n - 1) % n]);
-            const uint32_t r4 = r3 - k % n;
-            x[(k + p) % n] ^= r3;
-            x[(k + q) % n] ^= r4;
-            x[k % n] = r4;
-        }
-        bool zero = (x[0] & 0x80000000u) == 0;
-        for (uint32_t i = 1; i < n && zero; ++i) zero = x[i] == 0;
-        if (zero) x[0] = 0x80000000u;
-    }
-    e->index = 624;
-    return B200_OK;
-}
-
-uint32_t b200_mt19937_next(b200_mt19937_t* e) { return e ? b200::pnp::mt_next(e) : 0u; }
-
-int b200_pnp_draw_min_sets(b200_mt19937_t* e, uint32_t n_matches, uint32_t max_num_iter, int32_t* out) {
-    if (!e || n_matches < 4 || (max_num_iter > 0 && !out)) return B200_ERR_INVALID;
-    for (uint32_t it = 0; it < max_num_iter; ++it) b200::pnp::create_random_array4(e, n_matches, out + 4 * (size_t)it);
-    return B200_OK;
-}
 
 int b200_pnp_ransac(b200_lba_t h, int n_problems, b200_pnp_problem_t* problems) {
     B200_RANGE("b200:pnp:ransac");
@@ -302,16 +193,8 @@ int b200_pnp_ransac(b200_lba_t h, int n_problems, b200_pnp_problem_t* problems) 
                 return B200_ERR_INVALID;
             }
         const bool runs = !((unsigned)n < 4u || (unsigned)n < P.min_num_inliers);
+        if (!b200::min_sets_ok("b200_pnp_ransac", q, runs, P.max_num_iter, P.min_sets, 4, n)) return B200_ERR_INVALID;
         const int n_hyp = runs ? (int)P.max_num_iter : 0;
-        if (runs && (P.max_num_iter > (uint32_t)INT_MAX || (n_hyp > 0 && !P.min_sets))) {
-            b200::set_error("b200_pnp_ransac: problem %d: bad max_num_iter or null min_sets", q);
-            return B200_ERR_INVALID;
-        }
-        for (long long k = 0; k < 4LL * n_hyp; ++k)
-            if (P.min_sets[k] < 0 || P.min_sets[k] >= n) {
-                b200::set_error("b200_pnp_ransac: problem %d: min_sets entry %lld = %d outside [0, %d)", q, k, P.min_sets[k], n);
-                return B200_ERR_INVALID;
-            }
         pd[q] = ProblemDev{n, (int)total, (int)total_hyp, n_hyp, runs, P.min_num_inliers, P.gauss_newton_num_iter, P.recompute != 0};
         total += n;
         total_hyp += n_hyp;
@@ -321,24 +204,18 @@ int b200_pnp_ransac(b200_lba_t h, int n_problems, b200_pnp_problem_t* problems) 
         }
     }
     const size_t T = (size_t)std::max(total, 1LL), NH = (size_t)std::max(total_hyp, 1LL);
-    auto al = [](size_t& o, size_t bytes) {
-        const size_t r = o;
-        o = b200::round_up(o + bytes, (size_t)256);
-        return r;
-    };
-    size_t o = 0;
-    const size_t o_probs = al(o, sizeof(ProblemDev) * n_problems), o_b = al(o, 24 * T), o_p = al(o, 24 * T), o_sf = al(o, 4 * T);
-    const size_t o_ms = al(o, 16 * NH), o_hp = al(o, 4 * NH);
-    const size_t in_bytes = o;
-    const size_t o_res = al(o, sizeof(ResultDev) * n_problems), o_fl = al(o, T);
-    const size_t out_end = o;
-    const size_t o_mc = al(o, 4 * T), o_hyp = al(o, sizeof(HypDev) * NH), o_idx = al(o, 4 * T);
+    b200::Staging a;
+    const size_t o_probs = a.take(sizeof(ProblemDev) * n_problems), o_b = a.take(24 * T), o_p = a.take(24 * T), o_sf = a.take(4 * T);
+    const size_t o_ms = a.take(16 * NH), o_hp = a.take(4 * NH);
+    const size_t in_bytes = a.end;
+    const size_t o_res = a.take(sizeof(ResultDev) * n_problems), o_fl = a.take(T);
+    const size_t out_end = a.end;
+    const size_t o_mc = a.take(4 * T), o_hyp = a.take(sizeof(HypDev) * NH), o_idx = a.take(4 * T);
     cudaStream_t st;
     unsigned char *db, *hb;
-    int rc = b200::lba::borrow_buffers(h, o, out_end, &st, &db, &hb);
+    int rc = b200::lba::borrow_buffers(h, a.end, out_end, &st, &db, &hb);
     if (rc) return rc;
     std::memcpy(hb + o_probs, pd.data(), sizeof(ProblemDev) * n_problems);
-    int* hyp_problem = reinterpret_cast<int*>(hb + o_hp);
     for (int q = 0; q < n_problems; ++q) {
         const b200_pnp_problem_t& P = problems[q];
         const size_t off = (size_t)pd[q].match_off, n = (size_t)P.n_matches;
@@ -348,8 +225,7 @@ int b200_pnp_ransac(b200_lba_t h, int n_problems, b200_pnp_problem_t* problems) 
             float* sf = reinterpret_cast<float*>(hb + o_sf) + off;
             for (size_t j = 0; j < n; ++j) sf[j] = P.scale_factors[P.octaves[j]];
         }
-        if (pd[q].n_hyp) std::memcpy(hb + o_ms + 16 * (size_t)pd[q].hyp_off, P.min_sets, 16 * (size_t)pd[q].n_hyp);
-        for (int k = 0; k < pd[q].n_hyp; ++k) hyp_problem[pd[q].hyp_off + k] = q;
+        b200::stage_min_sets(q, P.min_sets, 4, pd[q].n_hyp, 4 * (size_t)pd[q].hyp_off, pd[q].hyp_off, (int32_t*)(hb + o_ms), (int*)(hb + o_hp));
     }
     B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
     const double* d_b = (const double*)(db + o_b);
@@ -405,8 +281,9 @@ int b200_epnp_compute_pose(b200_lba_t h, int n_problems, b200_epnp_problem_t* pr
         total += P.n;
         if (total > INT_MAX / 4) return B200_ERR_INVALID;
     }
-    const size_t o_probs = 0, o_b = b200::round_up(sizeof(EpnpDev) * n_problems, (size_t)256), o_p = o_b + b200::round_up(24 * (size_t)total, (size_t)256);
-    const size_t bytes = o_p + 24 * (size_t)total;
+    b200::Staging a;
+    const size_t o_probs = a.take(sizeof(EpnpDev) * n_problems), o_b = a.take(24 * (size_t)total), o_p = a.take(24 * (size_t)total);
+    const size_t bytes = a.end;
     cudaStream_t st;
     unsigned char *db, *hb;
     int rc = b200::lba::borrow_buffers(h, bytes, bytes, &st, &db, &hb);

@@ -23,13 +23,10 @@
 
 #include "common.cuh"
 #include "epnp.cuh"
+#include "ransac_host.cuh"
 #include "util_trig.cuh"  // util_cos, which essential_core.h (included below for its SVD pieces) calls in es_cos_angle_thr
 
 namespace b200 {
-namespace lba {
-int borrow_buffers(b200_lba_t h, size_t dev_bytes, size_t host_bytes, cudaStream_t* stream, unsigned char** d, unsigned char** hst);
-}
-
 namespace twoview {
 
 using pnp::apply_householder_left;
@@ -44,16 +41,8 @@ __device__ __forceinline__ float tv_fs(float a, float b) { return __fsub_rn(a, b
 __device__ __forceinline__ float tv_fm(float a, float b) { return __fmul_rn(a, b); }
 __device__ __forceinline__ float tv_fd(float a, float b) { return __fdiv_rn(a, b); }
 
-#define ES_FN __device__
-#define ES_BIG __device__ __noinline__
-#define ES_SQRT(x) __dsqrt_rn(x)
-#define ES_MAKE_HOUSEHOLDER(v, len, stride, tau, beta) pnp::make_householder((v), (len), (stride), (tau), (beta))
-#include "essential_core.h"
+#include "essential_core.cuh"
 #include "twoview_core.h"
-#undef ES_FN
-#undef ES_BIG
-#undef ES_SQRT
-#undef ES_MAKE_HOUSEHOLDER
 
 constexpr int kMinRows = 8;  // both models return early below 8 matches (H: min_set_size * 2)
 
@@ -214,9 +203,7 @@ __global__ void __launch_bounds__(64) twoview_select_kernel(int n_problems, cons
     tv_check_inliers(P.model, k1, k2, mt, P.n, r.M, P.sigma, fl, &cost);
     if (P.recompute) {
         int32_t* idx = idx_scratch + P.match_off;
-        int m = 0;
-        for (int j = 0; j < P.n; ++j)
-            if (fl[j]) idx[m++] = j;
+        const int m = compact_inliers(fl, P.n, idx);
         double Mn[9];
         if (tv_estimate(P.model, kn1 + 2 * (size_t)P.kp1_off, kn2 + 2 * (size_t)P.kp2_off, mt, idx, m, mat_scratch + 18 * (size_t)P.match_off,
                         Mn, &r.status)) {
@@ -260,16 +247,8 @@ int b200_twoview_ransac(b200_lba_t h, int n_problems, b200_twoview_problem_t* pr
             }
         const int set_size = P.model == B200_TWOVIEW_H ? 4 : 8;
         const bool runs = n >= kMinRows;
+        if (!b200::min_sets_ok("b200_twoview_ransac", q, runs, P.max_num_iter, P.min_sets, set_size, n)) return B200_ERR_INVALID;
         const int n_hyp = runs ? (int)P.max_num_iter : 0;
-        if (runs && (P.max_num_iter > (uint32_t)INT_MAX || (n_hyp > 0 && !P.min_sets))) {
-            b200::set_error("b200_twoview_ransac: problem %d: bad max_num_iter or null min_sets", q);
-            return B200_ERR_INVALID;
-        }
-        for (long long k = 0; k < (long long)set_size * n_hyp; ++k)
-            if (P.min_sets[k] < 0 || P.min_sets[k] >= n) {
-                b200::set_error("b200_twoview_ransac: problem %d: min_sets entry %lld = %d outside [0, %d)", q, k, P.min_sets[k], n);
-                return B200_ERR_INVALID;
-            }
         pd[q] = ProblemDev{P.model, n, (int)total, n1, (int)total_k1, n2, (int)total_k2, set_size, (int)total_hyp, (int)total_ms, n_hyp,
                            runs, P.recompute != 0, P.sigma};
         total += n;
@@ -284,34 +263,27 @@ int b200_twoview_ransac(b200_lba_t h, int n_problems, b200_twoview_problem_t* pr
     }
     const size_t T = (size_t)std::max(total, 1LL), K1 = (size_t)std::max(total_k1, 1LL), K2 = (size_t)std::max(total_k2, 1LL);
     const size_t NH = (size_t)std::max(total_hyp, 1LL), NMS = (size_t)std::max(total_ms, 1LL);
-    auto al = [](size_t& o, size_t bytes) {
-        const size_t r = o;
-        o = b200::round_up(o + bytes, (size_t)256);
-        return r;
-    };
-    size_t o = 0;
-    const size_t o_probs = al(o, sizeof(ProblemDev) * n_problems), o_k1 = al(o, 8 * K1), o_k2 = al(o, 8 * K2), o_mt = al(o, 8 * T);
-    const size_t o_ms = al(o, 4 * NMS), o_hp = al(o, 4 * NH);
-    const size_t in_bytes = o;
-    const size_t o_res = al(o, sizeof(ResultDev) * n_problems), o_fl = al(o, T);
-    const size_t out_end = o;
-    const size_t o_n1 = al(o, 8 * K1), o_n2 = al(o, 8 * K2), o_norm = al(o, sizeof(NormDev) * n_problems);
-    const size_t o_hyp = al(o, sizeof(HypDev) * NH), o_sc = al(o, sizeof(ScoreDev) * NH);
-    const size_t o_idx = al(o, 4 * T), o_mat = al(o, 8 * 18 * T);
+    b200::Staging a;
+    const size_t o_probs = a.take(sizeof(ProblemDev) * n_problems), o_k1 = a.take(8 * K1), o_k2 = a.take(8 * K2), o_mt = a.take(8 * T);
+    const size_t o_ms = a.take(4 * NMS), o_hp = a.take(4 * NH);
+    const size_t in_bytes = a.end;
+    const size_t o_res = a.take(sizeof(ResultDev) * n_problems), o_fl = a.take(T);
+    const size_t out_end = a.end;
+    const size_t o_n1 = a.take(8 * K1), o_n2 = a.take(8 * K2), o_norm = a.take(sizeof(NormDev) * n_problems);
+    const size_t o_hyp = a.take(sizeof(HypDev) * NH), o_sc = a.take(sizeof(ScoreDev) * NH);
+    const size_t o_idx = a.take(4 * T), o_mat = a.take(8 * 18 * T);
     cudaStream_t st;
     unsigned char *db, *hb;
-    int rc = b200::lba::borrow_buffers(h, o, out_end, &st, &db, &hb);
+    int rc = b200::lba::borrow_buffers(h, a.end, out_end, &st, &db, &hb);
     if (rc) return rc;
     std::memcpy(hb + o_probs, pd.data(), sizeof(ProblemDev) * n_problems);
-    int* hyp_problem = reinterpret_cast<int*>(hb + o_hp);
     for (int q = 0; q < n_problems; ++q) {
         const b200_twoview_problem_t& P = problems[q];
         const ProblemDev& D = pd[q];
         if (D.n1) std::memcpy(hb + o_k1 + 8 * (size_t)D.kp1_off, P.keypts_1, 8 * (size_t)D.n1);
         if (D.n2) std::memcpy(hb + o_k2 + 8 * (size_t)D.kp2_off, P.keypts_2, 8 * (size_t)D.n2);
         if (D.n) std::memcpy(hb + o_mt + 8 * (size_t)D.match_off, P.matches_12, 8 * (size_t)D.n);
-        if (D.n_hyp) std::memcpy(hb + o_ms + 4 * (size_t)D.ms_off, P.min_sets, 4 * (size_t)D.set_size * D.n_hyp);
-        for (int k = 0; k < D.n_hyp; ++k) hyp_problem[D.hyp_off + k] = q;
+        b200::stage_min_sets(q, P.min_sets, D.set_size, D.n_hyp, (size_t)D.ms_off, D.hyp_off, (int32_t*)(hb + o_ms), (int*)(hb + o_hp));
     }
     B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
     const ProblemDev* d_probs = (const ProblemDev*)(db + o_probs);

@@ -1,6 +1,6 @@
 """Host-side mirrors of solve::pnp_solver (src/stella_vslam/solve/pnp_solver.{h,cc}): EPnP inside RANSAC on the device
 (b200_pnp_ransac / b200_epnp_compute_pose on a b200_lba_t handle), with the minimal sets drawn on the host exactly as
-util::create_random_array draws them from the solver's std::mt19937 (b200_pnp_draw_min_sets).
+util::create_random_array draws them from the solver's std::mt19937 (b200_draw_min_sets).
 
 Arrays: bearings and points are (n, 3) float64, octaves (n,) int, scale_factors the ORB pyramid's float32 scale factors.
 
@@ -57,7 +57,6 @@ def _L():
         L.b200_mt19937_seed.argtypes = [C.POINTER(Mt19937), C.POINTER(C.c_uint32), C.c_int]
         L.b200_mt19937_next.argtypes = [C.POINTER(Mt19937)]
         L.b200_mt19937_next.restype = C.c_uint32
-        L.b200_pnp_draw_min_sets.argtypes = [C.POINTER(Mt19937), C.c_uint32, C.c_uint32, C.POINTER(C.c_int32)]
         L.b200_draw_min_sets.argtypes = [C.POINTER(Mt19937), C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_int32)]
         L.b200_essential_ransac.argtypes = [vp, C.c_int, C.POINTER(EssentialProblem)]
         L.b200_twoview_ransac.argtypes = [vp, C.c_int, C.POINTER(TwoviewProblem)]
@@ -85,18 +84,59 @@ def mt19937(seed_seq=None):
     return e
 
 
+def _random_engine(use_fixed_seed):
+    """util::create_random_engine: a default-constructed engine, or one seeded by std::seed_seq over ten std::random_device words."""
+    return mt19937(None if use_fixed_seed else np.frombuffer(np.random.bytes(40), np.uint32))
+
+
 def draw_min_sets(n_matches, max_num_iter, engine=None, set_size=4):
     """max_num_iter calls of util::create_random_array(set_size, 0, n_matches - 1, engine), (max_num_iter, set_size) int32.  engine: an
     Mt19937 (advanced in place) or None for a default-constructed one.  set_size 4 is PnP's minimal set, 5 the essential solver's."""
     e = mt19937() if engine is None else engine
     k = int(set_size)
     out = np.zeros((max(int(max_num_iter), 1), max(k, 1)), np.int32)
-    ptr = out.ctypes.data_as(C.POINTER(C.c_int32))
-    if k == 4:
-        check(_L().b200_pnp_draw_min_sets(C.byref(e), int(n_matches), int(max_num_iter), ptr))
-    else:
-        check(_L().b200_draw_min_sets(C.byref(e), k, int(n_matches), int(max_num_iter), ptr))
+    check(_L().b200_draw_min_sets(C.byref(e), k, int(n_matches), int(max_num_iter), out.ctypes.data_as(C.POINTER(C.c_int32))))
     return out[:int(max_num_iter)]
+
+
+def _run_batch(entry, StructT, pack, problems, device):
+    """Packs each problem dict into a StructT with pack(problem, keep) -> (struct, inlier flag buffer), then calls the entry point named
+    entry on the batch.  Returns the filled structs and the flag buffers, one per problem."""
+    keep, flags = [], []
+    arr = (StructT * max(len(problems), 1))()
+    for i, pr in enumerate(problems):
+        arr[i], fl = pack(pr, keep)
+        flags.append(fl)
+    check(getattr(_L(), entry)(_handle(device), len(problems), arr))
+    return arr[:len(problems)], flags
+
+
+class _ransac_solver:
+    """What the RANSAC solvers share: the engine is the solver's member, so find_via_ransac continues its state across calls; the
+    validity, status and inlier flags of the last call."""
+
+    def __init__(self, use_fixed_seed, device):
+        self.device = device
+        self.random_engine_ = _random_engine(use_fixed_seed)
+        self.solution_is_valid_ = False
+        self.is_inlier_match_ = []
+        self.status_ = 0
+
+    def _find_via_ransac(self, early_return, max_num_iter, set_size, batch, problem):
+        """Returns before any draw when early_return (None), else draws the minimal sets from the engine, solves the one problem with
+        batch and returns its result dict."""
+        if early_return:
+            self.solution_is_valid_ = False
+            return None
+        ms = draw_min_sets(self.num_matches_, max_num_iter, self.random_engine_, set_size=set_size)
+        r = batch([dict(problem, min_sets=ms)], self.device)[0]
+        self.status_ = r["status"]
+        self.solution_is_valid_ = r["valid"]
+        self.is_inlier_match_ = [bool(v) for v in r["inlier_flags"]]
+        return r
+
+    def solution_is_valid(self):
+        return self.solution_is_valid_
 
 
 def _pack(prob, keep):
@@ -124,19 +164,14 @@ def pnp_ransac_batch(problems, device=0):
     """b200_pnp_ransac over dicts(bearings, points, octaves, scale_factors, min_sets (max_num_iter x 4), min_num_inliers=10,
     gauss_newton_num_iter=10, recompute=True).  Returns per problem dict(status, valid, best_iter, num_inliers, min_cost, rot_cw, trans_cw,
     inlier_flags (None on the early return)); rot_cw / trans_cw are None unless valid."""
-    keep, flags = [], []
-    arr = (PnpProblem * max(len(problems), 1))()
-    for i, pr in enumerate(problems):
-        arr[i], fl = _pack(pr, keep)
-        flags.append(fl)
-    check(_L().b200_pnp_ransac(_handle(device), len(problems), arr))
+    arr, flags = _run_batch("b200_pnp_ransac", PnpProblem, _pack, problems, device)
     out = []
-    for i, pr in enumerate(problems):
-        S, n = arr[i], arr[i].n_matches
+    for S, fl in zip(arr, flags):
+        n = S.n_matches
         early = n < 4 or n < S.min_num_inliers
         out.append(dict(status=S.status, valid=bool(S.valid), best_iter=S.best_iter, num_inliers=S.num_inliers, min_cost=S.min_cost,
                         rot_cw=np.array(S.rot_cw).reshape(3, 3) if S.valid else None, trans_cw=np.array(S.trans_cw) if S.valid else None,
-                        inlier_flags=None if early else flags[i][:n].astype(bool)))
+                        inlier_flags=None if early else fl[:n].astype(bool)))
     return out
 
 
@@ -158,7 +193,7 @@ def compute_pose_batch(problems, device=0):
                  wrote=bool(arr[i].wrote), status=arr[i].status) for i in range(len(problems))]
 
 
-class pnp_solver:
+class pnp_solver(_ransac_solver):
     """solve::pnp_solver.  The engine is the solver's member: find_via_ransac continues its state across calls."""
 
     def __init__(self, valid_bearings, octaves, valid_points, scale_factors, min_num_inliers=10, use_fixed_seed=False,
@@ -172,35 +207,21 @@ class pnp_solver:
             raise ValueError("bearings, octaves and points must have one entry per match")
         if n and (self.octaves_.min() < 0 or self.octaves_.max() >= len(self.scale_factors_)):
             raise IndexError("octave outside the scale factors")  # std::vector::at throws in the reference
+        super().__init__(use_fixed_seed, device)
         self.num_matches_ = n
         self.min_num_inliers_ = int(min_num_inliers)
         self.gauss_newton_num_iter_ = int(gauss_newton_num_iter)
-        self.device = device
-        # create_random_engine: a default-constructed engine, or one seeded by std::seed_seq over ten std::random_device words
-        self.random_engine_ = mt19937(None if use_fixed_seed else np.frombuffer(np.random.bytes(40), np.uint32))
-        self.solution_is_valid_ = False
         self.best_rot_cw_ = np.zeros((3, 3))
         self.best_trans_cw_ = np.zeros(3)
-        self.is_inlier_match = []
-        self.status_ = 0
 
     def find_via_ransac(self, max_num_iter, recompute=True):
         n = self.num_matches_
-        if n < 4 or n < self.min_num_inliers_:
-            self.solution_is_valid_ = False
-            return
-        ms = draw_min_sets(n, max_num_iter, self.random_engine_)
-        r = pnp_ransac_batch([dict(bearings=self.bearings_, points=self.points_, octaves=self.octaves_, scale_factors=self.scale_factors_,
-                                   min_num_inliers=self.min_num_inliers_, gauss_newton_num_iter=self.gauss_newton_num_iter_,
-                                   recompute=recompute, min_sets=ms)], self.device)[0]
-        self.status_ = r["status"]
-        self.solution_is_valid_ = r["valid"]
-        if r["valid"]:
+        r = self._find_via_ransac(n < 4 or n < self.min_num_inliers_, max_num_iter, 4, pnp_ransac_batch,
+                                  dict(bearings=self.bearings_, points=self.points_, octaves=self.octaves_, scale_factors=self.scale_factors_,
+                                       min_num_inliers=self.min_num_inliers_, gauss_newton_num_iter=self.gauss_newton_num_iter_,
+                                       recompute=recompute))
+        if r is not None and r["valid"]:
             self.best_rot_cw_, self.best_trans_cw_ = r["rot_cw"], r["trans_cw"]
-        self.is_inlier_match = [bool(v) for v in r["inlier_flags"]]
-
-    def solution_is_valid(self):
-        return self.solution_is_valid_
 
     def get_best_rotation(self):
         return self.best_rot_cw_.copy()
@@ -214,7 +235,7 @@ class pnp_solver:
         return T
 
     def get_inlier_flags(self):
-        return list(self.is_inlier_match)
+        return list(self.is_inlier_match_)
 
     @staticmethod
     def compute_pose(bearing_vectors, pos_ws, rot_cw=None, trans_cw=None, num_iter=5, device=0):
@@ -248,23 +269,13 @@ def essential_ransac_batch(problems, device=0):
     """b200_essential_ransac over dicts(bearings_1, bearings_2 (n x 3, gathered through matches_12), min_sets (max_num_iter x 5),
     recompute=True, min_set_size=5).  Returns per problem dict(status, valid, best_iter, best_candidate, num_inliers, best_cost (float32),
     E_21 (None unless valid), inlier_flags (None on the early return))."""
-    keep, flags = [], []
-    arr = (EssentialProblem * max(len(problems), 1))()
-    for i, pr in enumerate(problems):
-        arr[i], fl = _pack_essential(pr, keep)
-        flags.append(fl)
-    check(_L().b200_essential_ransac(_handle(device), len(problems), arr))
-    out = []
-    for i in range(len(problems)):
-        S, n = arr[i], arr[i].n_matches
-        out.append(dict(status=S.status, valid=bool(S.valid), best_iter=S.best_iter, best_candidate=S.best_candidate,
-                        num_inliers=S.num_inliers, best_cost=np.float32(S.best_cost),
-                        E_21=np.array(S.E_21).reshape(3, 3) if S.valid else None,
-                        inlier_flags=None if n < S.min_set_size else flags[i][:n].astype(bool)))
-    return out
+    arr, flags = _run_batch("b200_essential_ransac", EssentialProblem, _pack_essential, problems, device)
+    return [dict(status=S.status, valid=bool(S.valid), best_iter=S.best_iter, best_candidate=S.best_candidate, num_inliers=S.num_inliers,
+                 best_cost=np.float32(S.best_cost), E_21=np.array(S.E_21).reshape(3, 3) if S.valid else None,
+                 inlier_flags=None if S.n_matches < S.min_set_size else fl[:S.n_matches].astype(bool)) for S, fl in zip(arr, flags)]
 
 
-class essential_solver:
+class essential_solver(_ransac_solver):
     """solve::essential_solver.  matches_12: (first, second) index pairs into bearings_1 / bearings_2.  The engine is the solver's
     member: find_via_ransac continues its state across calls."""
 
@@ -274,36 +285,22 @@ class essential_solver:
         m = np.asarray(matches_12, np.int64).reshape(-1, 2)
         if len(m) and (m.min() < 0 or m[:, 0].max() >= len(b1) or m[:, 1].max() >= len(b2)):
             raise IndexError("match index outside the bearings")  # std::vector::at throws in the reference
+        super().__init__(use_fixed_seed, device)
         self.bearings_1_ = np.ascontiguousarray(b1[m[:, 0]])
         self.bearings_2_ = np.ascontiguousarray(b2[m[:, 1]])
         self.num_matches_ = len(m)
-        self.device = device
-        self.random_engine_ = mt19937(None if use_fixed_seed else np.frombuffer(np.random.bytes(40), np.uint32))
-        self.solution_is_valid_ = False
         self.best_cost_ = np.float32(0.0)
         self.best_E_21_ = np.zeros((3, 3))
-        self.is_inlier_match_ = []
-        self.status_ = 0
 
     def find_via_ransac(self, max_num_iter, recompute=True, min_set_size=5):
         if int(min_set_size) != 5:
             raise ValueError("essential_solver: only the five-point minimal set (min_set_size = 5) is supported")
-        n = self.num_matches_
-        if n < min_set_size:
-            self.solution_is_valid_ = False
-            return
-        ms = draw_min_sets(n, max_num_iter, self.random_engine_, set_size=5)
-        r = essential_ransac_batch([dict(bearings_1=self.bearings_1_, bearings_2=self.bearings_2_, min_sets=ms, recompute=recompute)],
-                                   self.device)[0]
-        self.status_ = r["status"]
-        self.solution_is_valid_ = r["valid"]
-        self.best_cost_ = r["best_cost"]
-        if r["valid"]:
-            self.best_E_21_ = r["E_21"]
-        self.is_inlier_match_ = [bool(v) for v in r["inlier_flags"]]
-
-    def solution_is_valid(self):
-        return self.solution_is_valid_
+        r = self._find_via_ransac(self.num_matches_ < min_set_size, max_num_iter, 5, essential_ransac_batch,
+                                  dict(bearings_1=self.bearings_1_, bearings_2=self.bearings_2_, recompute=recompute))
+        if r is not None:
+            self.best_cost_ = r["best_cost"]
+            if r["valid"]:
+                self.best_E_21_ = r["E_21"]
 
     def get_best_cost(self):
         return self.best_cost_
@@ -368,22 +365,13 @@ def twoview_ransac_batch(problems, device=0):
     matches_12 ((n, 2) keypoint index pairs), min_sets (max_num_iter x 4 for H, x 8 for F), sigma=1.0, recompute=True).  H and F
     problems mix freely in one call.  Returns per problem dict(status, valid, best_iter, num_inliers, best_cost (float32), M_21 (None
     unless valid), inlier_flags (None on the early return, n < 8))."""
-    keep, flags = [], []
-    arr = (TwoviewProblem * max(len(problems), 1))()
-    for i, pr in enumerate(problems):
-        arr[i], fl = _pack_twoview(pr, keep)
-        flags.append(fl)
-    check(_L().b200_twoview_ransac(_handle(device), len(problems), arr))
-    out = []
-    for i in range(len(problems)):
-        S, n = arr[i], arr[i].n_matches
-        out.append(dict(status=S.status, valid=bool(S.valid), best_iter=S.best_iter, num_inliers=S.num_inliers,
-                        best_cost=np.float32(S.best_cost), M_21=np.array(S.M_21).reshape(3, 3) if S.valid else None,
-                        inlier_flags=None if n < 8 else flags[i][:n].astype(bool)))
-    return out
+    arr, flags = _run_batch("b200_twoview_ransac", TwoviewProblem, _pack_twoview, problems, device)
+    return [dict(status=S.status, valid=bool(S.valid), best_iter=S.best_iter, num_inliers=S.num_inliers, best_cost=np.float32(S.best_cost),
+                 M_21=np.array(S.M_21).reshape(3, 3) if S.valid else None, inlier_flags=None if S.n_matches < 8 else fl[:S.n_matches].astype(bool))
+            for S, fl in zip(arr, flags)]
 
 
-class _twoview_solver:
+class _twoview_solver(_ransac_solver):
     """The shared surface of homography_solver and fundamental_solver.  undist_keypts_*: every undistorted keypoint of each frame
     ((n, 2) pixels); matches_12: (first, second) index pairs.  The engine is the solver's member: find_via_ransac continues its state
     across calls, and use_fixed_seed gives each solver its own default-constructed engine, as util::create_random_engine does."""
@@ -391,38 +379,26 @@ class _twoview_solver:
     _model = None
 
     def __init__(self, undist_keypts_1, undist_keypts_2, matches_12, sigma, use_fixed_seed=False, device=0):
+        super().__init__(use_fixed_seed, device)
         self.undist_keypts_1_ = _keypts(undist_keypts_1)
         self.undist_keypts_2_ = _keypts(undist_keypts_2)
         m = np.asarray(matches_12, np.int64).reshape(-1, 2)
         if len(m) and (m.min() < 0 or m[:, 0].max() >= len(self.undist_keypts_1_) or m[:, 1].max() >= len(self.undist_keypts_2_)):
             raise IndexError("match index outside the keypoints")  # std::vector::at throws in the reference
         self.matches_12_ = np.ascontiguousarray(m.astype(np.int32))
+        self.num_matches_ = len(m)
         self.sigma_ = np.float32(sigma)
-        self.device = device
-        self.random_engine_ = mt19937(None if use_fixed_seed else np.frombuffer(np.random.bytes(40), np.uint32))
-        self.solution_is_valid_ = False
         self.best_cost_ = np.float32(0.0)
         self.best_M_21_ = np.zeros((3, 3))
-        self.is_inlier_match_ = []
-        self.status_ = 0
 
     def find_via_ransac(self, max_num_iter, recompute=True):
-        n = len(self.matches_12_)
-        if n < 8:
-            self.solution_is_valid_ = False
-            return
-        ms = draw_min_sets(n, max_num_iter, self.random_engine_, set_size=_SET_SIZE[self._model])
-        r = twoview_ransac_batch([dict(model=self._model, keypts_1=self.undist_keypts_1_, keypts_2=self.undist_keypts_2_,
-                                       matches_12=self.matches_12_, sigma=self.sigma_, min_sets=ms, recompute=recompute)], self.device)[0]
-        self.status_ = r["status"]
-        self.solution_is_valid_ = r["valid"]
-        self.best_cost_ = r["best_cost"]
-        if r["valid"]:
-            self.best_M_21_ = r["M_21"]
-        self.is_inlier_match_ = [bool(v) for v in r["inlier_flags"]]
-
-    def solution_is_valid(self):
-        return self.solution_is_valid_
+        r = self._find_via_ransac(self.num_matches_ < 8, max_num_iter, _SET_SIZE[self._model], twoview_ransac_batch,
+                                  dict(model=self._model, keypts_1=self.undist_keypts_1_, keypts_2=self.undist_keypts_2_,
+                                       matches_12=self.matches_12_, sigma=self.sigma_, recompute=recompute))
+        if r is not None:
+            self.best_cost_ = r["best_cost"]
+            if r["valid"]:
+                self.best_M_21_ = r["M_21"]
 
     def get_best_cost(self):
         return self.best_cost_

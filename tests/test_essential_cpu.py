@@ -1,5 +1,4 @@
-"""solve::essential_solver on the CPU: the oracle's stages against numpy / scipy, the RANSAC rules, check_inliers' NaN handling and the
-minimal-set sampler against libstdc++."""
+"""solve::essential_solver on the CPU: the oracle's stages against numpy / scipy, the RANSAC rules and check_inliers' NaN handling."""
 import os
 import subprocess
 import tempfile
@@ -238,76 +237,6 @@ def test_check_inliers_matches_numpy(seed):
     ref_flags, ref_cost = _check_inliers_numpy(p["bearings_1"], p["bearings_2"], E)
     assert (flags == ref_flags).all() and num == ref_flags.sum()
     assert cost.tobytes() == ref_cost.tobytes()
-
-
-_SAMPLER = r"""
-#include <algorithm>
-#include <cstdio>
-#include <cstdlib>
-#include <random>
-#include <vector>
-// util::create_random_array (src/stella_vslam/util/random_array.cc) restated with the standard library it relies on
-static std::vector<unsigned> create_random_array(size_t size, unsigned lo, unsigned hi, std::mt19937& e) {
-    std::uniform_int_distribution<unsigned> d(lo, hi);
-    const auto make_size = static_cast<size_t>(size * 1.2);
-    std::vector<unsigned> v;
-    v.reserve(size);
-    while (v.size() != size) {
-        while (v.size() < make_size) v.push_back(d(e));
-        std::sort(v.begin(), v.end());
-        auto u = std::unique(v.begin(), v.end());
-        if (size < static_cast<size_t>(std::distance(v.begin(), u))) u = std::next(v.begin(), size);
-        v.erase(u, v.end());
-    }
-    std::shuffle(v.begin(), v.end(), e);
-    return v;
-}
-int main(int argc, char** argv) {
-    const unsigned size = atoi(argv[1]), n = atoi(argv[2]), iters = atoi(argv[3]), nseed = atoi(argv[4]);
-    std::mt19937 e;
-    if (nseed) {
-        std::vector<std::uint_least32_t> w;
-        for (unsigned k = 0; k < nseed; ++k) w.push_back((unsigned)strtoul(argv[5 + k], nullptr, 10));
-        std::seed_seq s(w.begin(), w.end());
-        e = std::mt19937(s);
-    }
-    for (unsigned it = 0; it < iters; ++it)
-        for (unsigned x : create_random_array(size, 0u, n - 1, e)) printf("%u\n", x);
-    printf("%u\n", (unsigned)e());
-}
-"""
-
-
-@pytest.fixture(scope="module")
-def sampler_exe():
-    d = tempfile.mkdtemp(prefix="b200_sampler_")
-    src, exe = os.path.join(d, "s.cc"), os.path.join(d, "s")
-    with open(src, "w") as f:
-        f.write(_SAMPLER)
-    subprocess.check_call([os.environ.get("CXX", "g++"), "-O1", "-std=c++17", "-o", exe, src])
-    return exe
-
-
-@pytest.mark.parametrize("set_size", [4, 5, 8])
-@pytest.mark.parametrize("seed", [None, (1, 2, 3), (7, 0xFFFFFFFF, 12345, 99, 5, 6, 7, 8, 9, 10)])
-def test_draw_min_sets_matches_libstdcxx(sampler_exe, set_size, seed):
-    from stella_vslam_b200 import solve
-    words = [] if seed is None else list(seed)
-    for n, iters in [(set_size, 40), (set_size + 1, 40), (37, 300), (1500, 300)]:
-        out = subprocess.check_output([sampler_exe, str(set_size), str(n), str(iters), str(len(words))] + [str(w) for w in words])
-        ref = np.array(out.split(), np.uint64)
-        e = solve.mt19937(words or None)
-        got = solve.draw_min_sets(n, iters, e, set_size=set_size)
-        assert got.shape == (iters, set_size)
-        np.testing.assert_array_equal(got.reshape(-1).astype(np.uint64), ref[:-1])
-        assert solve._L().b200_mt19937_next(e) == int(ref[-1])  # the engine continues where the reference's does
-
-
-def test_draw_min_sets_rejects_too_few_matches():
-    from stella_vslam_b200 import solve
-    from stella_vslam_b200._lib import B200Error
-    with pytest.raises(B200Error):
-        solve.draw_min_sets(4, 3, solve.mt19937(), set_size=5)
 
 
 def test_solver_early_return_draws_nothing():

@@ -1,8 +1,6 @@
 """solve::pnp_solver on the CPU: the restated Eigen pieces against numpy, EPnP against the true pose and cv2, the RANSAC rules on
-hand-built inputs, max_cos_errors_ against util::cos, and the minimal-set sampler against std::mt19937 / libstdc++."""
-import ctypes as C
+hand-built inputs and max_cos_errors_ against util::cos."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -222,79 +220,3 @@ def test_no_inlier_decision_near_its_threshold(model):
         mc = O.max_cos_errors(pr["scale_factors"], pr["octaves"]).astype(np.float64)
         assert np.min(np.abs(cosang - mc)) > 1e-12
         np.testing.assert_array_equal(r["inlier_flags"], cosang > mc)
-
-
-# --- the sampler ---------------------------------------------------------------------------------------------------------------
-
-def test_engine_raw_stream_is_mt19937():
-    from stella_vslam_b200 import solve
-    e = solve.mt19937()
-    mine = np.array([solve._L().b200_mt19937_next(C.byref(e)) for _ in range(2000)], np.uint64)
-    bg = np.random.MT19937()
-    bg._legacy_seeding(5489)
-    np.testing.assert_array_equal(mine, bg.random_raw(2000))
-
-
-CPP = r"""
-#include <algorithm>
-#include <cstdio>
-#include <cstdlib>
-#include <random>
-#include <vector>
-// the draws of util::create_random_array(4, 0, n - 1, engine): uniform_int_distribution<unsigned>, sort, unique, shuffle
-static std::vector<unsigned> draw(std::mt19937& e, unsigned n) {
-    std::uniform_int_distribution<unsigned> d(0, n - 1);
-    const size_t make_size = static_cast<size_t>(4 * 1.2);
-    std::vector<unsigned> v;
-    while (v.size() != 4) {
-        while (v.size() < make_size) v.push_back(d(e));
-        std::sort(v.begin(), v.end());
-        auto u = std::unique(v.begin(), v.end());
-        if (4 < static_cast<size_t>(std::distance(v.begin(), u))) u = std::next(v.begin(), 4);
-        v.erase(u, v.end());
-    }
-    std::shuffle(v.begin(), v.end(), e);
-    return v;
-}
-int main(int argc, char** argv) {
-    const unsigned n = atoi(argv[1]), iters = atoi(argv[2]);
-    std::vector<std::uint_least32_t> words;
-    for (int i = 3; i < argc; ++i) words.push_back(strtoul(argv[i], 0, 10));
-    std::mt19937 e;
-    if (!words.empty()) {
-        std::seed_seq s(words.begin(), words.end());
-        e = std::mt19937(s);
-    }
-    for (unsigned i = 0; i < iters; ++i)
-        for (unsigned x : draw(e, n)) printf("%u\n", x);
-}
-"""
-
-
-@pytest.fixture(scope="module")
-def cpp_sampler(tmp_path_factory):
-    d = tmp_path_factory.mktemp("sampler")
-    (d / "s.cc").write_text(CPP)
-    subprocess.check_call([os.environ.get("CXX", "g++"), "-O1", "-std=c++17", "-o", str(d / "s"), str(d / "s.cc")])
-    return str(d / "s")
-
-
-@pytest.mark.parametrize("n,seed", [(4, ()), (5, ()), (10, ()), (300, ()), (123457, ()), (50, (1, 2, 3)),
-                                    (1000, tuple(range(10, 20))), (7, (4294967295, 0, 17))])
-def test_min_sets_match_libstdcxx(cpp_sampler, n, seed):
-    from stella_vslam_b200 import solve
-    out = subprocess.check_output([cpp_sampler, str(n), "40"] + [str(s) for s in seed], text=True)
-    ref = np.array(out.split(), np.int64).reshape(40, 4)
-    mine = solve.draw_min_sets(n, 40, solve.mt19937(seed or None))
-    np.testing.assert_array_equal(mine, ref)
-
-
-def test_min_sets_distinct_and_continuing():
-    from stella_vslam_b200 import solve
-    e = solve.mt19937((7, 8))
-    a, b = solve.draw_min_sets(9, 10, e), solve.draw_min_sets(9, 20, e)
-    whole = solve.draw_min_sets(9, 30, solve.mt19937((7, 8)))
-    np.testing.assert_array_equal(np.concatenate([a, b]), whole)
-    assert all(len(set(r)) == 4 and r.min() >= 0 and r.max() < 9 for r in whole)
-    with pytest.raises(Exception):
-        solve.draw_min_sets(3, 1)
