@@ -47,9 +47,11 @@ struct NvtxRange {
 // Require a Hopper-class (compute capability 9.x) device; there is no fallback path.
 int require_device(int device);
 
+struct StagingArena;  // staging.cuh
+
 namespace lba {
-// The handle's stream and its device / pinned host staging buffers, grown to at least the given sizes (lba_kernels.cu).
-int borrow_buffers(b200_lba_t h, size_t dev_bytes, size_t host_bytes, cudaStream_t* stream, unsigned char** d, unsigned char** hst);
+// With the handle's device set: its stream and its staging arena, grown to at least the given sizes (lba_kernels.cu).
+int staging(b200_lba_t h, size_t dev_bytes, size_t host_bytes, cudaStream_t* stream, StagingArena** arena);
 }
 
 }  // namespace b200

@@ -20,6 +20,7 @@
 #include "common.cuh"
 #include "epnp.cuh"
 #include "ransac_host.cuh"
+#include "staging.cuh"
 #include "util_trig.cuh"
 
 namespace b200 {
@@ -184,7 +185,7 @@ int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t
         }
     }
     const size_t T = (size_t)std::max(total, 1LL), NH = (size_t)std::max(total_hyp, 1LL);
-    b200::Staging a;
+    b200::Layout a;
     const size_t o_probs = a.take(sizeof(ProblemDev) * n_problems), o_b1 = a.take(24 * T), o_b2 = a.take(24 * T);
     const size_t o_ms = a.take(4 * kMinSet * NH), o_hp = a.take(4 * NH);
     const size_t in_bytes = a.end;
@@ -193,9 +194,10 @@ int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t
     const size_t o_cand = a.take(8 * 9 * kMaxCand * NH), o_hyp = a.take(sizeof(HypDev) * NH), o_sc = a.take(sizeof(ScoreDev) * kMaxCand * NH);
     const size_t o_idx = a.take(4 * T), o_mat = a.take(72 * T);
     cudaStream_t st;
-    unsigned char *db, *hb;
-    int rc = b200::lba::borrow_buffers(h, a.end, out_end, &st, &db, &hb);
+    b200::StagingArena* A;
+    int rc = b200::lba::staging(h, a.end, out_end, &st, &A);
     if (rc) return rc;
+    unsigned char *db = A->d, *hb = A->h;
     std::memcpy(hb + o_probs, pd.data(), sizeof(ProblemDev) * n_problems);
     for (int q = 0; q < n_problems; ++q) {
         const b200_essential_problem_t& P = problems[q];
@@ -207,7 +209,7 @@ int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t
         b200::stage_min_sets(q, P.min_sets, kMinSet, pd[q].n_hyp, kMinSet * (size_t)pd[q].hyp_off, pd[q].hyp_off, (int32_t*)(hb + o_ms),
                              (int*)(hb + o_hp));
     }
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(A->upload(in_bytes, st));
     const double* d_b1 = (const double*)(db + o_b1);
     const double* d_b2 = (const double*)(db + o_b2);
     if (total_hyp > 0) {
@@ -226,7 +228,7 @@ int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t
         n_problems, (const ProblemDev*)(db + o_probs), d_b1, d_b2, (const double*)(db + o_cand), (const HypDev*)(db + o_hyp),
         (const ScoreDev*)(db + o_sc), (int32_t*)(db + o_idx), (double*)(db + o_mat), db + o_fl, (ResultDev*)(db + o_res));
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpyAsync(hb + o_res, db + o_res, out_end - o_res, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A->download(o_res, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
     const ResultDev* res = reinterpret_cast<const ResultDev*>(hb + o_res);
     for (int q = 0; q < n_problems; ++q) {

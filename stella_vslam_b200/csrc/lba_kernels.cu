@@ -31,6 +31,7 @@
 #include "common.cuh"
 #include "lm_common.cuh"
 #include "quat.cuh"
+#include "staging.cuh"
 #include "track_chain.cuh"
 
 namespace b200 {
@@ -1955,10 +1956,7 @@ struct Solver {
     int device = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    unsigned char* d_arena = nullptr;
-    size_t arena_cap = 0;
-    unsigned char* h_stage = nullptr;  // pinned upload staging
-    size_t h_cap = 0;
+    StagingArena arena;
     double* h_res = nullptr;           // pinned readback
     size_t h_res_cap = 0;
     float last_ms = 0.f;
@@ -2003,21 +2001,7 @@ struct Solver {
         return e;
     }
 
-    int ensure(size_t dev_bytes, size_t host_bytes, size_t res_doubles) {
-        if (dev_bytes > arena_cap) {
-            if (d_arena) B200_CUDA(cudaFree(d_arena));
-            d_arena = nullptr;
-            arena_cap = 0;
-            B200_CUDA(cudaMalloc(&d_arena, dev_bytes + dev_bytes / 4));
-            arena_cap = dev_bytes + dev_bytes / 4;
-        }
-        if (host_bytes > h_cap) {
-            if (h_stage) B200_CUDA(cudaFreeHost(h_stage));
-            h_stage = nullptr;
-            h_cap = 0;
-            B200_CUDA(cudaHostAlloc(&h_stage, host_bytes + host_bytes / 4, cudaHostAllocDefault));
-            h_cap = host_bytes + host_bytes / 4;
-        }
+    int ensure_res(size_t res_doubles) {
         if (res_doubles > h_res_cap) {
             if (h_res) B200_CUDA(cudaFreeHost(h_res));
             h_res = nullptr;
@@ -2036,17 +2020,6 @@ struct Solver {
         B200_CUDA(cudaHostGetDevicePointer((void**)&d_abort, h_abort, 0));
         abort_cap = n * 2;
         return B200_OK;
-    }
-};
-
-struct Carver {
-    size_t off = 0;
-    template <typename T>
-    size_t take(size_t n) {
-        off = round_up(off, (size_t)256);
-        const size_t o = off;
-        off += sizeof(T) * std::max<size_t>(n, 1);
-        return o;
     }
 };
 
@@ -2138,7 +2111,7 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
     }
     // ---- arena layout -------------------------------------------------------------------------------------------------------
     std::vector<WinOff> wo(nw);
-    Carver cv;
+    Layout cv;
     const size_t o_wins = cv.take<WinDev>(nw), o_ctl = cv.take<LmCtl>(nw);
     for (int x = 0; x < nw; ++x) {
         const HostWin& h = hw[x];
@@ -2150,16 +2123,14 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
         o.e_delta = cv.take<float>(E); o.pose_col = cv.take<int>(K); o.pt_col = cv.take<int>(L); o.q0 = cv.take<double>(4 * K);
         o.t0 = cv.take<double>(3 * K); o.Rt0 = cv.take<double>(12 * K); o.pts0 = cv.take<double>(3 * L);
     }
-    const size_t upload_bytes = round_up(cv.off, (size_t)256);
-    cv.off = upload_bytes;
+    const size_t upload_bytes = cv.end;
     for (int x = 0; x < nw; ++x) {
         const HostWin& h = hw[x];
         WinOff& o = wo[x];
         o.pt_cnt = cv.take<int>(h.L); o.pose_cnt = cv.take<int>(h.Kf); o.level = cv.take<unsigned char>(h.E); o.chi0 = cv.take<double>(h.E);
         o.fail = cv.take<int>(1); o.tickets = cv.take<int>(2); o.bad = cv.take<int>(1); o.blk_done = cv.take<int>(h.n_blocks);
     }
-    const size_t zero_end = round_up(cv.off, (size_t)256);
-    cv.off = zero_end;
+    const size_t zero_end = cv.end;
     for (int x = 0; x < nw; ++x) {
         const HostWin& h = hw[x];
         WinOff& o = wo[x];
@@ -2182,21 +2153,21 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
         }
         o.r_chi = cv.take<double>(h.lbc); o.r_diag = cv.take<double>(h.lbc); o.r_scale = cv.take<double>(h.lbc); o.r_result = cv.take<double>(8);
     }
-    const size_t export_begin = round_up(cv.off, (size_t)256);
-    cv.off = export_begin;
+    const size_t export_begin = cv.end;
     for (int x = 0; x < nw; ++x) {
         const HostWin& h = hw[x];
         WinOff& o = wo[x];
         o.qf = cv.take<double>(4 * (size_t)h.K); o.tf = cv.take<double>(3 * (size_t)h.K); o.pf = cv.take<double>(3 * (size_t)h.L);
         o.out = cv.take<unsigned char>(h.E);
     }
-    const size_t export_bytes = round_up(cv.off, (size_t)256) - export_begin;
+    const size_t export_bytes = cv.end - export_begin;
     const size_t ctl_doubles = ceil_div(sizeof(LmCtl) * (size_t)nw, sizeof(double)) + 8;
-    int rc = S.ensure(cv.off + 512, upload_bytes, ceil_div(export_bytes, sizeof(double)) + 2 * ctl_doubles + 64);
+    int rc = S.arena.reserve(cv.end + 512, upload_bytes, S.stream);
     if (rc) return rc;
+    if ((rc = S.ensure_res(ceil_div(export_bytes, sizeof(double)) + 2 * ctl_doubles + 64))) return rc;
     if ((rc = S.ensure_abort(nw))) return rc;
-    unsigned char* d = S.d_arena;
-    unsigned char* hs = S.h_stage;
+    unsigned char* d = S.arena.d;
+    unsigned char* hs = S.arena.h;
     LmCtl* h_ctl2[2] = {reinterpret_cast<LmCtl*>(S.h_res), reinterpret_cast<LmCtl*>(S.h_res + ctl_doubles)};  // read-back mirrors of the control blocks
     LmCtl* h_ctl = h_ctl2[0];
     unsigned char* h_export = reinterpret_cast<unsigned char*>(S.h_res + 2 * ctl_doubles + 8);
@@ -2273,7 +2244,7 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
         S.h_abort[x] = 0;
         c.abort_word = (stops && stops[act[x]]) ? S.d_abort + x : nullptr;
     }
-    if (debug) fprintf(stderr, "[lba] %d windows staged in %.3f ms (upload %.2f MB, arena %.1f MB)\n", nw, ms_since(t_begin), upload_bytes / 1e6, cv.off / 1e6);
+    if (debug) fprintf(stderr, "[lba] %d windows staged in %.3f ms (upload %.2f MB, arena %.1f MB)\n", nw, ms_since(t_begin), upload_bytes / 1e6, cv.end / 1e6);
     cudaStream_t st = S.stream;
     int launches = 0;
     S.prof_kind.clear();
@@ -2290,7 +2261,7 @@ static int solve_batch(Solver& S, int n_all, const b200_lba_problem_t* Ps, int i
         return B200_OK;
     };
     B200_CUDA(cudaEventRecord(S.ev0, st));
-    B200_CUDA(cudaMemcpyAsync(d, hs, upload_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(S.arena.upload(upload_bytes, st));
     B200_CUDA(cudaMemsetAsync(d + upload_bytes, 0, zero_end - upload_bytes, st));
     if ((rc = mark(-1))) return rc;
     const WinDev* wins = (const WinDev*)(d + o_wins);
@@ -2592,16 +2563,15 @@ struct b200_lba_s {
 
 namespace b200 {
 namespace lba {
-// The device, stream and buffers of a handle, for entry points of other translation units that run on its stream (the PnP solver,
-// pnp_kernels.cu): at least dev_bytes of device arena and host_bytes of pinned staging, valid until the handle's next call.
-int borrow_buffers(b200_lba_t h, size_t dev_bytes, size_t host_bytes, cudaStream_t* stream, unsigned char** d, unsigned char** hst) {
+// For the entry points of other translation units that run on a handle's stream (PnP, essential and two-view RANSAC, pose graph,
+// Sim3 refinement): its arena holds at least dev_bytes on the device and host_bytes in the mirror until the handle's next call.
+int staging(b200_lba_t h, size_t dev_bytes, size_t host_bytes, cudaStream_t* stream, StagingArena** arena) {
     Solver& S = h->s;
     B200_CUDA(cudaSetDevice(S.device));
-    const int rc = S.ensure(dev_bytes, host_bytes, 0);
+    const int rc = S.arena.reserve(dev_bytes, host_bytes, S.stream);
     if (rc) return rc;
     *stream = S.stream;
-    *d = S.d_arena;
-    *hst = S.h_stage;
+    *arena = &S.arena;
     return B200_OK;
 }
 }  // namespace lba
@@ -2660,8 +2630,7 @@ int b200_lba_destroy(b200_lba_t h) {
     if (!h) return B200_OK;
     cudaSetDevice(h->s.device);
     if (h->s.stream) cudaStreamSynchronize(h->s.stream);
-    cudaFree(h->s.d_arena);
-    if (h->s.h_stage) cudaFreeHost(h->s.h_stage);
+    h->s.arena.release();
     if (h->s.h_res) cudaFreeHost(h->s.h_res);
     if (h->s.h_abort) cudaFreeHost(h->s.h_abort);
     if (h->s.ev0) cudaEventDestroy(h->s.ev0);
@@ -2766,16 +2735,15 @@ int b200_pose_optimize(b200_lba_t h, int n_problems, const b200_lba_problem_t* p
         total_edges += (size_t)P.n_edges;
     }
     if (total_edges > 0 && !outlier_flags) return B200_ERR_INVALID;
-    Carver up;
-    const size_t o_probs = up.take<PoseProb>(n_problems), o_edges = up.take<PoseEdge>(total_edges);
-    const size_t upload_bytes = b200::round_up(up.off, (size_t)256);
-    Carver dv;
-    dv.off = upload_bytes;
-    const size_t o_level = dv.take<unsigned char>(total_edges), o_flags = dv.take<unsigned char>(total_edges);
-    const size_t o_pose = dv.take<double>(16 * (size_t)n_problems), o_valid = dv.take<unsigned>(n_problems);
-    int rc = S.ensure(dv.off + 256, upload_bytes, 16);
+    b200::Layout L;
+    const size_t o_probs = L.take<PoseProb>(n_problems), o_edges = L.take<PoseEdge>(total_edges);
+    const size_t upload_bytes = L.end;
+    const size_t o_level = L.take<unsigned char>(total_edges), o_flags = L.take<unsigned char>(total_edges);
+    const size_t o_pose = L.take<double>(16 * (size_t)n_problems), o_valid = L.take<unsigned>(n_problems);
+    cudaStream_t st = S.stream;
+    int rc = S.arena.reserve(L.end + 256, upload_bytes, st);
     if (rc) return rc;
-    unsigned char* hs = S.h_stage;
+    unsigned char* hs = S.arena.h;
     PoseProb* hp = reinterpret_cast<PoseProb*>(hs + o_probs);
     PoseEdge* he = reinterpret_cast<PoseEdge*>(hs + o_edges);
     size_t off = 0;
@@ -2803,10 +2771,9 @@ int b200_pose_optimize(b200_lba_t h, int n_problems, const b200_lba_problem_t* p
         }
         off += (size_t)P.n_edges;
     }
-    unsigned char* d = S.d_arena;
-    cudaStream_t st = S.stream;
+    unsigned char* d = S.arena.d;
     B200_CUDA(cudaEventRecord(S.ev0, st));
-    B200_CUDA(cudaMemcpyAsync(d, hs, upload_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(S.arena.upload(upload_bytes, st));
     pose_optimize_kernel<<<n_problems, kPoseThreads, 0, st>>>((const PoseProb*)(d + o_probs), (const PoseEdge*)(d + o_edges), d + o_level, d + o_flags,
                                                              num_trials_robust, num_trials, num_each_iter, (double*)(d + o_pose),
                                                              (unsigned*)(d + o_valid));
@@ -2855,15 +2822,13 @@ int track_stage_c(b200_lba_t opt, cudaStream_t st, const TrackShared& sh, const 
     Solver& S = opt->s;
     size_t total = 0;
     for (int f = 0; f < n_frames; ++f) total += (size_t)h_frames[f].kp_cap;
-    Carver up;
-    const size_t o_probs = up.take<PoseProb>(n_frames);
-    const size_t upload_bytes = round_up(up.off, (size_t)256);
-    Carver dv;
-    dv.off = upload_bytes;
-    const size_t o_edges = dv.take<PoseEdge>(total), o_kp = dv.take<int>(total), o_level = dv.take<unsigned char>(total), o_flags = dv.take<unsigned char>(total);
-    int rc = S.ensure(dv.off + 256, upload_bytes, 16);
+    Layout L;
+    const size_t o_probs = L.take<PoseProb>(n_frames);
+    const size_t upload_bytes = L.end;
+    const size_t o_edges = L.take<PoseEdge>(total), o_kp = L.take<int>(total), o_level = L.take<unsigned char>(total), o_flags = L.take<unsigned char>(total);
+    int rc = S.arena.reserve(L.end + 256, upload_bytes, st);
     if (rc) return rc;
-    PoseProb* hp = reinterpret_cast<PoseProb*>(S.h_stage + o_probs);
+    PoseProb* hp = S.arena.host<PoseProb>(o_probs);
     size_t off = 0;
     for (int f = 0; f < n_frames; ++f) {
         PoseProb pb{};
@@ -2879,8 +2844,8 @@ int track_stage_c(b200_lba_t opt, cudaStream_t st, const TrackShared& sh, const 
         hp[f] = pb;
         off += (size_t)h_frames[f].kp_cap;
     }
-    unsigned char* d = S.d_arena;
-    B200_CUDA(cudaMemcpyAsync(d, S.h_stage, upload_bytes, cudaMemcpyHostToDevice, st));
+    unsigned char* d = S.arena.d;
+    B200_CUDA(S.arena.upload(upload_bytes, st));
     PoseProb* dp = reinterpret_cast<PoseProb*>(d + o_probs);
     track_edges_kernel<<<n_frames, kTrackEdgeThreads, 0, st>>>(sh, d_frames, dp, (PoseEdge*)(d + o_edges), (int*)(d + o_kp));
     if (ev_edges_done) B200_CUDA(cudaEventRecord(ev_edges_done, st));

@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "staging.cuh"
 #include "track_chain.cuh"
 #include "triangulate.cuh"
 
@@ -1379,27 +1380,8 @@ struct Matcher {
     size_t matched_cap = 0;
     unsigned* d_taken = nullptr;
     size_t taken_cap = 0;
-    // staging for the host-buffer entry points
-    unsigned char* d_stage = nullptr;
-    size_t stage_cap = 0;
-    size_t last_h2d = 0, last_d2h = 0;
-    // grid-guided matchers: pinned host staging + device arena
-    unsigned char* h_guided = nullptr;
-    size_t h_guided_cap = 0;
-    unsigned char* d_guided = nullptr;
-    size_t d_guided_cap = 0;
-
-    int grow_pinned(unsigned char** p, size_t* cap, size_t bytes) {
-        if (bytes <= *cap) return B200_OK;
-        B200_CUDA(cudaStreamSynchronize(stream));
-        if (*p) B200_CUDA(cudaFreeHost(*p));
-        *p = nullptr;
-        *cap = 0;
-        const size_t want = bytes + bytes / 4 + 256;
-        B200_CUDA(cudaMallocHost((void**)p, want));
-        *cap = want;
-        return B200_OK;
-    }
+    // staging of every host-buffer entry point (each one synchronises before it returns, so they can share it)
+    StagingArena arena;
 
     int grow(void** p, size_t* cap, size_t bytes) {
         if (bytes <= *cap) return B200_OK;
@@ -1504,9 +1486,7 @@ int b200_matcher_destroy(b200_matcher_t h) {
     cudaFree(h->m.d_lists);
     cudaFree(h->m.d_matched);
     cudaFree(h->m.d_taken);
-    cudaFree(h->m.d_stage);
-    cudaFree(h->m.d_guided);
-    if (h->m.h_guided) cudaFreeHost(h->m.h_guided);
+    h->m.arena.release();
     for (int i = 0; i < 3; ++i)
         if (h->m.ev_t[i]) cudaEventDestroy(h->m.ev_t[i]);
     for (int i = 0; i < 7; ++i)
@@ -1624,23 +1604,17 @@ int b200_match_bruteforce(b200_matcher_t h, int n_problems, const uint8_t* desc1
         meta[2 * n_problems + p] = cnt2[p] > 0 ? off2[p] - lo2 : 0;
         meta[3 * n_problems + p] = cnt2[p];
     }
-    // device staging (256-byte aligned): desc1 | desc2 | angle1 | angle2 | valid2 | meta | pairs | n_pairs
-    auto al = [](size_t v) { return b200::round_up(v, (size_t)256); };
+    // device staging, copied straight from the caller's buffers: desc1 | desc2 | angle1 | angle2 | valid2 | meta | pairs | n_pairs
     const size_t a1_bytes = ext1 > 0 ? (size_t)(ext1 - 1) * angle1_stride + sizeof(float) : 0;
     const size_t a2_bytes = ext2 > 0 ? (size_t)(ext2 - 1) * angle2_stride + sizeof(float) : 0;
-    size_t o = 0;
-    const size_t o_d1 = o; o += al((size_t)32 * std::max(ext1, 1));
-    const size_t o_d2 = o; o += al((size_t)32 * std::max(ext2, 1));
-    const size_t o_a1 = o; o += al(std::max(a1_bytes, (size_t)4));
-    const size_t o_a2 = o; o += al(std::max(a2_bytes, (size_t)4));
-    const size_t o_v2 = o; o += al((size_t)std::max(ext2, 1));
-    const size_t o_mt = o; o += al(sizeof(int) * meta.size());
-    const size_t o_pr = o; o += al(sizeof(int) * 2 * (size_t)pairs_stride * n_problems);
-    const size_t o_np = o; o += al(sizeof(int) * (size_t)n_problems);
-    int rc = m.grow((void**)&m.d_stage, &m.stage_cap, o);
-    if (rc) return rc;
-    unsigned char* s = m.d_stage;
+    b200::Layout L;
+    const size_t o_d1 = L.take((size_t)32 * ext1), o_d2 = L.take((size_t)32 * ext2), o_a1 = L.take(a1_bytes), o_a2 = L.take(a2_bytes);
+    const size_t o_v2 = L.take((size_t)ext2), o_mt = L.take<int>(meta.size()), o_pr = L.take<int>(2 * (size_t)pairs_stride * n_problems);
+    const size_t o_np = L.take<int>(n_problems);
     cudaStream_t st = m.stream;
+    int rc = m.arena.reserve(L.end, 0, st);
+    if (rc) return rc;
+    unsigned char* s = m.arena.d;
     if (ext1 > 0) {
         B200_CUDA(cudaMemcpyAsync(s + o_d1, desc1 + (size_t)32 * lo1, (size_t)32 * ext1, cudaMemcpyHostToDevice, st));
         B200_CUDA(cudaMemcpyAsync(s + o_a1, (const unsigned char*)angle1 + (size_t)lo1 * angle1_stride, a1_bytes, cudaMemcpyHostToDevice, st));
@@ -1657,8 +1631,6 @@ int b200_match_bruteforce(b200_matcher_t h, int n_problems, const uint8_t* desc1
     rc = m.run(n_problems, S1, S2, valid2 ? s + o_v2 : nullptr, max_n1, max_n2, lowe_ratio, check_orientation, s + o_pr, pairs_stride,
                s + o_np);
     if (rc) return rc;
-    m.last_h2d = (size_t)32 * (ext1 + ext2) + a1_bytes + a2_bytes + (valid2 ? ext2 : 0) + sizeof(int) * meta.size();
-    m.last_d2h = sizeof(int) * ((size_t)n_problems + 2 * (size_t)pairs_stride * n_problems);
     B200_CUDA(cudaMemcpyAsync(n_pairs, s + o_np, sizeof(int) * n_problems, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaMemcpyAsync(pairs, s + o_pr, sizeof(int) * 2 * (size_t)pairs_stride * n_problems, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
@@ -1675,7 +1647,6 @@ int b200_match_guided(b200_matcher_t h, int n_problems, b200_guided_problem_t* p
     auto& m = h->m;
     B200_CUDA(cudaSetDevice(m.device));
     const int cap = max_candidates ? max_candidates : 256;
-    auto al = [](size_t v) { return b200::round_up(v, (size_t)256); };
     // layout of the arena: [GuidedDev x n][inputs of every problem][outputs of every problem][scratch]; the first two parts are
     // mirrored in pinned host memory and go up in one copy, the output part comes back in one copy.
     struct Lay {
@@ -1684,7 +1655,8 @@ int b200_match_guided(b200_matcher_t h, int n_problems, b200_guided_problem_t* p
         size_t cstart, citems, ccur, lists, llen, own;                                       // scratch
     };
     std::vector<Lay> lay(n_problems);
-    size_t o = al(sizeof(GuidedDev) * (size_t)n_problems);
+    b200::Layout a;
+    a.take<GuidedDev>(n_problems);  // at offset 0
     int max_q = 0, max_train = 0;
     for (int p = 0; p < n_problems; ++p) {
         const b200_guided_problem_t& P = problems[p];
@@ -1705,90 +1677,87 @@ int b200_match_guided(b200_matcher_t h, int n_problems, b200_guided_problem_t* p
             return B200_ERR_INVALID;
         }
         Lay& L = lay[p];
-        const size_t nt = (size_t)std::max(P.n_train, 1), nq = (size_t)std::max(P.n_queries, 1);
-        L.tx = o; o += al(4 * nt);
-        L.ty = o; o += al(4 * nt);
-        L.toct = o; o += al(nt);
-        L.tang = o; o += al(4 * nt);
-        L.txr = o; o += al(4 * nt);
-        L.tdesc = o; o += al(32 * nt);
-        L.qdesc = o; o += al(32 * nq);
-        L.qx = o; o += al(4 * nq);
-        L.qy = o; o += al(4 * nq);
-        L.qm = o; o += al(4 * nq);
-        L.qlo = o; o += al(nq);
-        L.qhi = o; o += al(nq);
-        L.qxr = o; o += al(4 * nq);
-        L.qang = o; o += al(4 * nq);
-        L.qval = o; o += al(nq);
-        L.qrep = o; o += al(16 * nq);
-        L.sig = o; o += al(4 * 256);
-        L.occ = o; o += al(nt);  // in AND out: kept at the end of the problem's input block
+        const size_t nt = (size_t)P.n_train, nq = (size_t)P.n_queries;
+        L.tx = a.take(4 * nt);
+        L.ty = a.take(4 * nt);
+        L.toct = a.take(nt);
+        L.tang = a.take(4 * nt);
+        L.txr = a.take(4 * nt);
+        L.tdesc = a.take(32 * nt);
+        L.qdesc = a.take(32 * nq);
+        L.qx = a.take(4 * nq);
+        L.qy = a.take(4 * nq);
+        L.qm = a.take(4 * nq);
+        L.qlo = a.take(nq);
+        L.qhi = a.take(nq);
+        L.qxr = a.take(4 * nq);
+        L.qang = a.take(4 * nq);
+        L.qval = a.take(nq);
+        L.qrep = a.take(16 * nq);
+        L.sig = a.take(4 * 256);
+        L.occ = a.take(nt);  // in AND out: kept at the end of the problem's input block
         max_q = std::max(max_q, P.n_queries);
         max_train = std::max(max_train, P.n_train);
     }
-    const size_t in_bytes = o;
-    const size_t out_begin = o;
+    const size_t in_bytes = a.end;
+    const size_t out_begin = a.end;
     for (int p = 0; p < n_problems; ++p) {
         Lay& L = lay[p];
-        L.mout = o; o += al(4 * (size_t)std::max(problems[p].n_queries, 1));
-        L.nm = o; o += al(4);
+        L.mout = a.take(4 * (size_t)problems[p].n_queries);
+        L.nm = a.take(4);
     }
-    const size_t o_overflow = o;
-    o += al(4);
-    const size_t out_end = o;
+    const size_t o_overflow = a.take(4);
+    const size_t out_end = a.end;
     for (int p = 0; p < n_problems; ++p) {
         const b200_guided_problem_t& P = problems[p];
         Lay& L = lay[p];
         const size_t cells = (size_t)P.grid_cols * P.grid_rows;
-        L.cstart = o; o += al(4 * (cells + 1));
-        L.citems = o; o += al(4 * (size_t)std::max(P.n_train, 1));
-        L.ccur = o; o += al(4 * cells);
-        L.lists = o; o += al(8 * (size_t)cap * std::max(P.n_queries, 1));
-        L.llen = o; o += al(4 * (size_t)std::max(P.n_queries, 1));
-        L.own = o; o += al(4 * (size_t)std::max(P.n_train, 1));
+        L.cstart = a.take(4 * (cells + 1));
+        L.citems = a.take(4 * (size_t)P.n_train);
+        L.ccur = a.take(4 * cells);
+        L.lists = a.take(8 * (size_t)cap * P.n_queries);
+        L.llen = a.take(4 * (size_t)P.n_queries);
+        L.own = a.take(4 * (size_t)P.n_train);
     }
     const size_t rs_bytes = (size_t)std::max(max_train, 1) * 6 + 16;  // claim (int) + state (u16) per keypoint
     if (rs_bytes > 200 * 1024) {
         b200::set_error("b200_match_guided: %d keypoints per frame exceed the on-chip occupancy table", max_train);
         return B200_ERR_CAPACITY;
     }
+    cudaStream_t st = m.stream;
     int rc;
-    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, o))) return rc;
-    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, out_end))) return rc;
-    unsigned char *hb = m.h_guided, *db = m.d_guided;
-    GuidedDev* hg = reinterpret_cast<GuidedDev*>(hb);
-    auto put = [&](size_t off, const void* src, size_t bytes) {
-        if (src && bytes) std::memcpy(hb + off, src, bytes);
-    };
+    if ((rc = m.arena.reserve(a.end, out_end, st))) return rc;
+    b200::StagingArena& A = m.arena;
+    unsigned char *hb = A.h, *db = A.d;
+    GuidedDev* hg = A.host<GuidedDev>(0);
     for (int p = 0; p < n_problems; ++p) {
         const b200_guided_problem_t& P = problems[p];
         const Lay& L = lay[p];
         const size_t nt = (size_t)P.n_train, nq = (size_t)P.n_queries;
-        put(L.tx, P.t_x, 4 * nt);
-        put(L.ty, P.t_y, 4 * nt);
-        put(L.toct, P.t_octave, nt);
-        put(L.tang, P.t_angle, 4 * nt);
-        put(L.txr, P.t_x_right, 4 * nt);
-        put(L.tdesc, P.t_desc, 32 * nt);
-        put(L.qdesc, P.q_desc, 32 * nq);
-        put(L.qx, P.q_x, 4 * nq);
-        put(L.qy, P.q_y, 4 * nq);
-        put(L.qm, P.q_margin, 4 * nq);
-        put(L.qlo, P.q_min_level, nq);
-        put(L.qhi, P.q_max_level, nq);
-        put(L.qxr, P.q_x_right, 4 * nq);
-        put(L.qang, P.q_angle, 4 * nq);
+        A.put(L.tx, P.t_x, 4 * nt);
+        A.put(L.ty, P.t_y, 4 * nt);
+        A.put(L.toct, P.t_octave, nt);
+        A.put(L.tang, P.t_angle, 4 * nt);
+        A.put(L.txr, P.t_x_right, 4 * nt);
+        A.put(L.tdesc, P.t_desc, 32 * nt);
+        A.put(L.qdesc, P.q_desc, 32 * nq);
+        A.put(L.qx, P.q_x, 4 * nq);
+        A.put(L.qy, P.q_y, 4 * nq);
+        A.put(L.qm, P.q_margin, 4 * nq);
+        A.put(L.qlo, P.q_min_level, nq);
+        A.put(L.qhi, P.q_max_level, nq);
+        A.put(L.qxr, P.q_x_right, 4 * nq);
+        A.put(L.qang, P.q_angle, 4 * nq);
         if (P.q_valid || P.q_has_observation)  // bit 0: valid, bit 1: has_observation()
             for (int q = 0; q < nq; ++q)
                 hb[L.qval + q] = (unsigned char)(((!P.q_valid || P.q_valid[q]) ? 1 : 0) | ((!P.q_has_observation || P.q_has_observation[q]) ? 2 : 0));
         const bool reproj = mode == B200_GUIDED_FUSE && P.do_reprojection_matching;
         if (reproj) {
-            put(L.qrep, P.q_reproj, 16 * nq);
+            A.put(L.qrep, P.q_reproj, 16 * nq);
             std::memset(hb + L.sig, 0, 4 * 256);
-            put(L.sig, P.inv_level_sigma_sq, 4 * (size_t)P.n_levels);
+            A.put(L.sig, P.inv_level_sigma_sq, 4 * (size_t)P.n_levels);
         }
-        if (P.t_occupied && mode != B200_GUIDED_AREA) put(L.occ, P.t_occupied, nt);
+        if (P.t_occupied && mode != B200_GUIDED_AREA) A.put(L.occ, P.t_occupied, nt);
         else std::memset(hb + L.occ, 0, nt);
         GuidedDev g{};
         g.n_train = P.n_train;
@@ -1826,10 +1795,9 @@ int b200_match_guided(b200_matcher_t h, int n_problems, b200_guided_problem_t* p
         g.n_matches = (int*)(db + L.nm);
         hg[p] = g;
     }
-    cudaStream_t st = m.stream;
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(A.upload(in_bytes, st));
     B200_CUDA(cudaMemsetAsync(db + o_overflow, 0, 4, st));
-    const GuidedDev* dg = reinterpret_cast<const GuidedDev*>(db);
+    const GuidedDev* dg = A.dev<const GuidedDev>(0);
     b200::match::guided_grid_kernel<<<n_problems, 1024, 0, st>>>(dg);
     b200::match::guided_candidates_kernel<<<dim3(std::max(1, b200::ceil_div(max_q, 128)), n_problems), 128, 0, st>>>(dg, mode, check_orientation,
                                                                                                                      (int*)(db + o_overflow));
@@ -1838,17 +1806,12 @@ int b200_match_guided(b200_matcher_t h, int n_problems, b200_guided_problem_t* p
     b200::match::guided_resolve_kernel<GuidedDev><<<n_problems, 32, rs_bytes, st>>>(dg, mode, thr, lowe_ratio);
     B200_CUDA(cudaGetLastError());
     // outputs: occupancy lives in the input block (copied back per problem only when asked for), the rest is contiguous
-    B200_CUDA(cudaMemcpyAsync(hb + out_begin, db + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
-    size_t occ_bytes = 0;
+    B200_CUDA(A.download(out_begin, out_end, st));
     const bool writes_occupancy = mode == B200_GUIDED_LANDMARKS || mode == B200_GUIDED_LAST_FRAME || mode == B200_GUIDED_FUSE;
     for (int p = 0; p < n_problems; ++p)
-        if (writes_occupancy && problems[p].t_occupied && problems[p].n_train > 0) {
+        if (writes_occupancy && problems[p].t_occupied && problems[p].n_train > 0)
             B200_CUDA(cudaMemcpyAsync(hb + lay[p].occ, db + lay[p].occ, (size_t)problems[p].n_train, cudaMemcpyDeviceToHost, st));
-            occ_bytes += (size_t)problems[p].n_train;
-        }
     B200_CUDA(cudaStreamSynchronize(st));
-    m.last_h2d = in_bytes;
-    m.last_d2h = out_end - out_begin + occ_bytes;
     const int overflow = *reinterpret_cast<const int*>(hb + o_overflow);
     if (overflow > 0) {
         b200::set_error("b200_match_guided: a search window returned %d keypoints, max_candidates is %d", overflow, cap);
@@ -1902,7 +1865,6 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const
     }
     B200_CUDA(cudaSetDevice(m.device));
     const int cap = prm->max_candidates ? prm->max_candidates : 256;
-    auto al = [](size_t v) { return b200::round_up(v, (size_t)256); };
     struct Lay {
         size_t xr, kl, pos, nrm, lo, hi, desc, skip, hobs;                       // inputs
         size_t obs, klo, kout, status, mout, nm;                                   // outputs
@@ -1911,9 +1873,9 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const
     };
     std::vector<Lay> lay(n_frames);
     int max_lm = 0;
-    size_t o = al(sizeof(TrackFrameDev) * (size_t)n_frames);
-    const size_t o_gd = o;
-    o += al(sizeof(GuidedDev) * (size_t)n_frames);
+    b200::Layout a;
+    a.take<TrackFrameDev>(n_frames);  // at offset 0
+    const size_t o_gd = a.take<GuidedDev>(n_frames);
     for (int f = 0; f < n_frames; ++f) {
         const b200_track_frame_t& F = frames[f];
         if (F.frame < 0 || F.frame >= batch || !F.pose_cw || F.n_landmarks < 0 || F.n_keypoints_in < 0 || F.kp_cap < 0
@@ -1923,72 +1885,69 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const
             return B200_ERR_INVALID;
         }
         Lay& L = lay[f];
-        const size_t nk = (size_t)std::max(F.n_keypoints_in, 1), nl = (size_t)std::max(F.n_landmarks, 1);
-        L.xr = o; o += al(4 * nk);
-        L.kl = o; o += al(4 * nk);
-        L.pos = o; o += al(24 * nl);
-        L.nrm = o; o += al(24 * nl);
-        L.lo = o; o += al(4 * nl);
-        L.hi = o; o += al(4 * nl);
-        L.desc = o; o += al(32 * nl);
-        L.skip = o; o += al(nl);
-        L.hobs = o; o += al(nl);
+        const size_t nk = (size_t)F.n_keypoints_in, nl = (size_t)F.n_landmarks;
+        L.xr = a.take(4 * nk);
+        L.kl = a.take(4 * nk);
+        L.pos = a.take(24 * nl);
+        L.nrm = a.take(24 * nl);
+        L.lo = a.take(4 * nl);
+        L.hi = a.take(4 * nl);
+        L.desc = a.take(32 * nl);
+        L.skip = a.take(nl);
+        L.hobs = a.take(nl);
         max_lm = std::max(max_lm, F.n_landmarks);
     }
-    const size_t in_bytes = o, out_begin = o;
+    const size_t in_bytes = a.end, out_begin = a.end;
     const size_t kc = (size_t)std::max(stride, 1);
     for (int f = 0; f < n_frames; ++f) {
         Lay& L = lay[f];
-        const size_t nl = (size_t)std::max(frames[f].n_landmarks, 1);
-        L.obs = o; o += al(nl);
-        L.klo = o; o += al(4 * kc);
-        L.kout = o; o += al(kc);
-        L.status = o; o += al(16);
-        L.mout = o; o += al(4 * nl);
-        L.nm = o; o += al(4);
+        const size_t nl = (size_t)frames[f].n_landmarks;
+        L.obs = a.take(nl);
+        L.klo = a.take(4 * kc);
+        L.kout = a.take(kc);
+        L.status = a.take(16);
+        L.mout = a.take(4 * nl);
+        L.nm = a.take(4);
     }
-    const size_t o_pose = o; o += al(8 * 16 * (size_t)n_frames);
-    const size_t o_nvalid = o; o += al(4 * (size_t)n_frames);
-    const size_t o_overflow = o; o += al(4);
-    const size_t out_end = o;
+    const size_t o_pose = a.take(8 * 16 * (size_t)n_frames);
+    const size_t o_nvalid = a.take(4 * (size_t)n_frames);
+    const size_t o_overflow = a.take(4);
+    const size_t out_end = a.end;
     const size_t cells = (size_t)prm->grid_cols * prm->grid_rows;
     for (int f = 0; f < n_frames; ++f) {
         Lay& L = lay[f];
-        const size_t nl = (size_t)std::max(frames[f].n_landmarks, 1);
-        L.und = o; o += al(sizeof(b200_keypoint_t) * kc);
-        L.tx = o; o += al(4 * kc);
-        L.ty = o; o += al(4 * kc);
-        L.toct = o; o += al(kc);
-        L.occ = o; o += al(kc);
-        L.qx = o; o += al(4 * nl);
-        L.qy = o; o += al(4 * nl);
-        L.qm = o; o += al(4 * nl);
-        L.qxr = o; o += al(4 * nl);
-        L.qlo = o; o += al(nl);
-        L.qhi = o; o += al(nl);
-        L.qval = o; o += al(nl);
-        L.cstart = o; o += al(4 * (cells + 1));
-        L.citems = o; o += al(4 * kc);
-        L.ccur = o; o += al(4 * cells);
-        L.lists = o; o += al(8 * (size_t)cap * nl);
-        L.llen = o; o += al(4 * nl);
-        L.own = o; o += al(4 * kc);
+        const size_t nl = (size_t)frames[f].n_landmarks;
+        L.und = a.take(sizeof(b200_keypoint_t) * kc);
+        L.tx = a.take(4 * kc);
+        L.ty = a.take(4 * kc);
+        L.toct = a.take(kc);
+        L.occ = a.take(kc);
+        L.qx = a.take(4 * nl);
+        L.qy = a.take(4 * nl);
+        L.qm = a.take(4 * nl);
+        L.qxr = a.take(4 * nl);
+        L.qlo = a.take(nl);
+        L.qhi = a.take(nl);
+        L.qval = a.take(nl);
+        L.cstart = a.take(4 * (cells + 1));
+        L.citems = a.take(4 * kc);
+        L.ccur = a.take(4 * cells);
+        L.lists = a.take(8 * (size_t)cap * nl);
+        L.llen = a.take(4 * nl);
+        L.own = a.take(4 * kc);
     }
     const size_t rs_bytes = kc * 6 + 16;
     if (rs_bytes > 200 * 1024) {
         b200::set_error("b200_track_local_map: %d keypoints per frame exceed the on-chip occupancy table", stride);
         return B200_ERR_CAPACITY;
     }
-    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, o))) return rc;
-    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, out_end))) return rc;
+    if ((rc = m.arena.reserve(a.end, out_end, m.stream))) return rc;
     for (int i = 0; i < 7; ++i)
         if (!m.ev_track[i]) B200_CUDA(cudaEventCreate(&m.ev_track[i]));
-    unsigned char *hb = m.h_guided, *db = m.d_guided;
-    TrackFrameDev* hf = reinterpret_cast<TrackFrameDev*>(hb);
-    GuidedDev* hg = reinterpret_cast<GuidedDev*>(hb + o_gd);
-    auto put = [&](size_t off, const void* src, size_t bytes) {
-        if (src && bytes) std::memcpy(hb + off, src, bytes);
-    };
+    b200::StagingArena& A = m.arena;
+    unsigned char *hb = A.h, *db = A.d;
+    TrackFrameDev* hf = A.host<TrackFrameDev>(0);
+    GuidedDev* hg = A.host<GuidedDev>(o_gd);
     TrackShared sh{};
     sh.model = prm->cam.model;
     sh.fx = prm->cam.fx; sh.fy = prm->cam.fy; sh.cx = prm->cam.cx; sh.cy = prm->cam.cy;
@@ -2011,15 +1970,15 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const
         const b200_track_frame_t& F = frames[f];
         const Lay& L = lay[f];
         const size_t nk = (size_t)F.n_keypoints_in, nl = (size_t)F.n_landmarks;
-        put(L.xr, F.kp_x_right, 4 * nk);
-        put(L.kl, F.kp_landmark, 4 * nk);
-        put(L.pos, F.lm_pos_w, 24 * nl);
-        put(L.nrm, F.lm_mean_normal, 24 * nl);
-        put(L.lo, F.lm_min_valid_dist, 4 * nl);
-        put(L.hi, F.lm_max_valid_dist, 4 * nl);
-        put(L.desc, F.lm_desc, 32 * nl);
-        put(L.skip, F.lm_skip, nl);
-        put(L.hobs, F.lm_has_observation, nl);
+        A.put(L.xr, F.kp_x_right, 4 * nk);
+        A.put(L.kl, F.kp_landmark, 4 * nk);
+        A.put(L.pos, F.lm_pos_w, 24 * nl);
+        A.put(L.nrm, F.lm_mean_normal, 24 * nl);
+        A.put(L.lo, F.lm_min_valid_dist, 4 * nl);
+        A.put(L.hi, F.lm_max_valid_dist, 4 * nl);
+        A.put(L.desc, F.lm_desc, 32 * nl);
+        A.put(L.skip, F.lm_skip, nl);
+        A.put(L.hobs, F.lm_has_observation, nl);
         poses[f] = F.pose_cw;
         TrackFrameDev t{};
         t.kps = d_kps + (size_t)F.frame * stride;
@@ -2097,10 +2056,10 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const
     }
     if ((rc = m.join())) return rc;
     B200_CUDA(cudaEventRecord(m.ev_track[0], st));
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(A.upload(in_bytes, st));
     B200_CUDA(cudaMemsetAsync(db + out_begin, 0, out_end - out_begin, st));
-    const TrackFrameDev* df = reinterpret_cast<const TrackFrameDev*>(db);
-    GuidedDev* dg = reinterpret_cast<GuidedDev*>(db + o_gd);
+    const TrackFrameDev* df = A.dev<const TrackFrameDev>(0);
+    GuidedDev* dg = A.dev<GuidedDev>(o_gd);
     if ((rc = b200::chain::track_stage_a(st, sh, df, n_frames, stride, max_lm))) return rc;
     b200::match::track_set_counts_kernel<<<b200::ceil_div(n_frames, 128), 128, 0, st>>>(dg, df, n_frames);
     B200_CUDA(cudaEventRecord(m.ev_track[1], st));
@@ -2118,11 +2077,9 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const
                                          (double*)(db + o_pose), (unsigned*)(db + o_nvalid), m.ev_track[5])))
         return rc;
     B200_CUDA(cudaEventRecord(m.ev_track[6], st));
-    B200_CUDA(cudaMemcpyAsync(hb + out_begin, db + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A.download(out_begin, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
     m.track_timed = true;
-    m.last_h2d = in_bytes;
-    m.last_d2h = out_end - out_begin;
     const int overflow = *reinterpret_cast<const int*>(hb + o_overflow);
     if (overflow > 0) {
         b200::set_error("b200_track_local_map: a search window returned %d keypoints, max_candidates is %d", overflow, cap);
@@ -2169,20 +2126,8 @@ int b200_match_pairs(b200_matcher_t h, int n_problems, b200_pairs_problem_t* pro
     unsigned list_thr = b200::match::kThrLow;
     if (!tri)
         while (list_thr < 255u && lowe_ratio * (float)(list_thr + 1) < (float)b200::match::kThrLow) ++list_thr;
-    auto al = [](size_t v) { return b200::round_up(v, (size_t)256); };
-    struct Item {
-        size_t off;
-        const void* src;
-        size_t bytes;
-    };
-    std::vector<Item> items;
-    size_t o = al(sizeof(PairsDev) * (size_t)n_problems);
-    auto add = [&](const void* src, size_t bytes) {
-        const size_t at = o;
-        items.push_back({at, src, src ? bytes : 0});
-        o += al(std::max(bytes, (size_t)1));
-        return at;
-    };
+    b200::Layout a;
+    a.take<PairsDev>(n_problems);  // at offset 0
     struct Lay {
         size_t d1, a1, v1, nd1, b1, s1, st1, d2, a2, v2, nd2, b2, st2, mout, nm, lists, llen;
     };
@@ -2198,49 +2143,61 @@ int b200_match_pairs(b200_matcher_t h, int n_problems, b200_pairs_problem_t* pro
         }
         Lay& L = lay[p];
         const size_t n1 = (size_t)P.n1, n2 = (size_t)P.n2;
-        L.d1 = add(P.desc1, 32 * n1);
-        L.a1 = add(check_orientation ? P.angle1 : nullptr, 4 * n1);
-        L.v1 = add(P.valid1, n1);
-        L.nd1 = add(P.node1, 4 * n1);
-        L.b1 = add(tri ? P.bearing1 : nullptr, 24 * n1);
-        L.s1 = add(tri ? P.scale1 : nullptr, 4 * n1);
-        L.st1 = add(tri ? P.stereo1 : nullptr, n1);
-        L.d2 = add(P.desc2, 32 * n2);
-        L.a2 = add(check_orientation ? P.angle2 : nullptr, 4 * n2);
-        L.v2 = add(P.valid2, n2);
-        L.nd2 = add(P.node2, 4 * n2);
-        L.b2 = add(tri ? P.bearing2 : nullptr, 24 * n2);
-        L.st2 = add(tri ? P.stereo2 : nullptr, n2);
+        L.d1 = a.take(32 * n1);
+        L.a1 = a.take(4 * n1);
+        L.v1 = a.take(n1);
+        L.nd1 = a.take(4 * n1);
+        L.b1 = a.take(24 * n1);
+        L.s1 = a.take(4 * n1);
+        L.st1 = a.take(n1);
+        L.d2 = a.take(32 * n2);
+        L.a2 = a.take(4 * n2);
+        L.v2 = a.take(n2);
+        L.nd2 = a.take(4 * n2);
+        L.b2 = a.take(24 * n2);
+        L.st2 = a.take(n2);
         max_n1 = std::max(max_n1, P.n1);
         max_n2 = std::max(max_n2, P.n2);
     }
-    const size_t in_bytes = o, out_begin = o;
+    const size_t in_bytes = a.end, out_begin = a.end;
     for (int p = 0; p < n_problems; ++p) {
-        lay[p].mout = o; o += al(4 * (size_t)std::max(problems[p].n1, 1));
-        lay[p].nm = o; o += al(4);
+        lay[p].mout = a.take(4 * (size_t)problems[p].n1);
+        lay[p].nm = a.take(4);
     }
-    const size_t o_overflow = o;
-    o += al(4);
-    const size_t out_end = o;
+    const size_t o_overflow = a.take(4);
+    const size_t out_end = a.end;
     for (int p = 0; p < n_problems; ++p) {
-        lay[p].lists = o; o += al(8 * (size_t)cap * std::max(problems[p].n1, 1));
-        lay[p].llen = o; o += al(4 * (size_t)std::max(problems[p].n1, 1));
+        lay[p].lists = a.take(8 * (size_t)cap * problems[p].n1);
+        lay[p].llen = a.take(4 * (size_t)problems[p].n1);
     }
     const size_t rs_bytes = (size_t)std::max(max_n2, 1) * 6 + 16;
     if (rs_bytes > 200 * 1024) {
         b200::set_error("b200_match_pairs: %d keypoints per frame exceed the on-chip occupancy table", max_n2);
         return B200_ERR_CAPACITY;
     }
+    cudaStream_t st = m.stream;
     int rc;
-    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, o))) return rc;
-    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, out_end))) return rc;
-    unsigned char *hb = m.h_guided, *db = m.d_guided;
-    for (const Item& it : items)
-        if (it.bytes) std::memcpy(hb + it.off, it.src, it.bytes);
-    PairsDev* hg = reinterpret_cast<PairsDev*>(hb);
+    if ((rc = m.arena.reserve(a.end, out_end, st))) return rc;
+    b200::StagingArena& A = m.arena;
+    unsigned char *hb = A.h, *db = A.d;
+    PairsDev* hg = A.host<PairsDev>(0);
     for (int p = 0; p < n_problems; ++p) {
         const b200_pairs_problem_t& P = problems[p];
         const Lay& L = lay[p];
+        const size_t n1 = (size_t)P.n1, n2 = (size_t)P.n2;
+        A.put(L.d1, P.desc1, 32 * n1);
+        A.put(L.a1, check_orientation ? P.angle1 : nullptr, 4 * n1);
+        A.put(L.v1, P.valid1, n1);
+        A.put(L.nd1, P.node1, 4 * n1);
+        A.put(L.b1, tri ? P.bearing1 : nullptr, 24 * n1);
+        A.put(L.s1, tri ? P.scale1 : nullptr, 4 * n1);
+        A.put(L.st1, tri ? P.stereo1 : nullptr, n1);
+        A.put(L.d2, P.desc2, 32 * n2);
+        A.put(L.a2, check_orientation ? P.angle2 : nullptr, 4 * n2);
+        A.put(L.v2, P.valid2, n2);
+        A.put(L.nd2, P.node2, 4 * n2);
+        A.put(L.b2, tri ? P.bearing2 : nullptr, 24 * n2);
+        A.put(L.st2, tri ? P.stereo2 : nullptr, n2);
         PairsDev g{};
         g.n_queries = P.n1;
         g.n_train = P.n2;
@@ -2270,21 +2227,18 @@ int b200_match_pairs(b200_matcher_t h, int n_problems, b200_pairs_problem_t* pro
         g.owner = nullptr;
         hg[p] = g;
     }
-    cudaStream_t st = m.stream;
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(A.upload(in_bytes, st));
     B200_CUDA(cudaMemsetAsync(db + o_overflow, 0, 4, st));
-    const PairsDev* dg = reinterpret_cast<const PairsDev*>(db);
+    const PairsDev* dg = A.dev<const PairsDev>(0);
     b200::match::pairs_candidates_kernel<<<dim3(std::max(1, b200::ceil_div(max_n1, b200::match::kPairRows)), n_problems), b200::match::kPairRows, 0,
                                            st>>>(dg, variant, list_thr, check_orientation, (int*)(db + o_overflow));
     if (rs_bytes > 48 * 1024)
         B200_CUDA(cudaFuncSetAttribute(b200::match::guided_resolve_kernel<PairsDev>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rs_bytes));
     b200::match::guided_resolve_kernel<PairsDev><<<n_problems, 32, rs_bytes, st>>>(dg, tri ? 6 : 5, (unsigned)b200::match::kThrLow, lowe_ratio);
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpyAsync(hb + out_begin, db + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A.download(out_begin, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
-    m.last_h2d = in_bytes;
-    m.last_d2h = out_end - out_begin;
-    const int overflow = *reinterpret_cast<const int*>(hb + o_overflow);
+    const int overflow = *A.host<const int>(o_overflow);
     if (overflow > 0) {
         b200::set_error("b200_match_pairs: a row kept %d gated candidates, max_candidates is %d", overflow, cap);
         return B200_ERR_CAPACITY;
@@ -2346,22 +2300,17 @@ int b200_stereo_compute(b200_matcher_t h, b200_orb_t left, int frame_left, b200_
             return B200_ERR_INVALID;
         }
     if ((rc = b200_orb_sync(left)) || (rc = b200_orb_sync(right))) return rc;
-    auto al = [](size_t v) { return b200::round_up(v, (size_t)256); };
-    size_t o = al(sizeof(StereoDev));
-    const size_t o_kl = o; o += al(sizeof(b200_keypoint_t) * (size_t)n_left);
-    const size_t o_kr = o; o += al(sizeof(b200_keypoint_t) * (size_t)std::max(n_right, 1));
-    const size_t o_dl = o; o += al((size_t)32 * n_left);
-    const size_t o_dr = o; o += al((size_t)32 * std::max(n_right, 1));
-    const size_t in_bytes = o, out_begin = o;
-    const size_t o_x = o; o += al(4 * (size_t)n_left);
-    const size_t o_dep = o; o += al(4 * (size_t)n_left);
-    const size_t o_nk = o; o += al(4);
-    const size_t out_end = o;
-    const size_t o_best = o; o += al(4 * (size_t)n_left);
-    const size_t o_corr = o; o += al(4 * (size_t)n_left);
-    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, o))) return rc;
-    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, out_end))) return rc;
-    unsigned char *hb = m.h_guided, *db = m.d_guided;
+    b200::Layout a;
+    const size_t o_g = a.take<StereoDev>(1), o_kl = a.take<b200_keypoint_t>(n_left), o_kr = a.take<b200_keypoint_t>(n_right);
+    const size_t o_dl = a.take((size_t)32 * n_left), o_dr = a.take((size_t)32 * n_right);
+    const size_t in_bytes = a.end, out_begin = a.end;
+    const size_t o_x = a.take(4 * (size_t)n_left), o_dep = a.take(4 * (size_t)n_left), o_nk = a.take(4);
+    const size_t out_end = a.end;
+    const size_t o_best = a.take(4 * (size_t)n_left), o_corr = a.take(4 * (size_t)n_left);
+    cudaStream_t st = m.stream;
+    if ((rc = m.arena.reserve(a.end, out_end, st))) return rc;
+    b200::StagingArena& A = m.arena;
+    unsigned char *hb = A.h, *db = A.d;
     g.n_left = n_left;
     g.n_right = n_right;
     g.kl = (const b200_keypoint_t*)(db + o_kl);
@@ -2375,24 +2324,19 @@ int b200_stereo_compute(b200_matcher_t h, b200_orb_t left, int frame_left, b200_
     g.depth = (float*)(db + o_dep);
     g.corr = (int*)(db + o_corr);
     g.n_kept = (int*)(db + o_nk);
-    std::memcpy(hb, &g, sizeof(g));
-    std::memcpy(hb + o_kl, keypts_left, sizeof(b200_keypoint_t) * (size_t)n_left);
-    std::memcpy(hb + o_dl, descs_left, (size_t)32 * n_left);
-    if (n_right > 0) {
-        std::memcpy(hb + o_kr, keypts_right, sizeof(b200_keypoint_t) * (size_t)n_right);
-        std::memcpy(hb + o_dr, descs_right, (size_t)32 * n_right);
-    }
-    cudaStream_t st = m.stream;
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
-    const StereoDev* dg = reinterpret_cast<const StereoDev*>(db);
+    A.put(o_g, &g, sizeof(g));
+    A.put(o_kl, keypts_left, sizeof(b200_keypoint_t) * (size_t)n_left);
+    A.put(o_dl, descs_left, (size_t)32 * n_left);
+    A.put(o_kr, keypts_right, sizeof(b200_keypoint_t) * (size_t)n_right);
+    A.put(o_dr, descs_right, (size_t)32 * n_right);
+    B200_CUDA(A.upload(in_bytes, st));
+    const StereoDev* dg = A.dev<const StereoDev>(o_g);
     stereo_match_kernel<<<b200::ceil_div(n_left, kStereoRows), kStereoRows, 0, st>>>(dg);
     stereo_subpixel_kernel<<<b200::ceil_div(n_left, 4), 128, 0, st>>>(dg);
     stereo_median_kernel<<<1, 1024, 0, st>>>(dg);
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpyAsync(hb + out_begin, db + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A.download(out_begin, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
-    m.last_h2d = in_bytes;
-    m.last_d2h = out_end - out_begin;
     std::memcpy(stereo_x_right, hb + o_x, 4 * (size_t)n_left);
     std::memcpy(depths, hb + o_dep, 4 * (size_t)n_left);
     if (n_matched) *n_matched = *reinterpret_cast<const int*>(hb + o_nk);
@@ -2415,29 +2359,24 @@ int b200_landmark_descriptors(b200_matcher_t h, int n_landmarks, const uint8_t* 
     if (total > 0 && !descs) return B200_ERR_INVALID;
     auto& m = h->m;
     B200_CUDA(cudaSetDevice(m.device));
-    auto al = [](size_t v) { return b200::round_up(v, (size_t)256); };
-    size_t o = 0;
-    const size_t o_desc = o; o += al(32 * std::max(total, (size_t)1));
-    const size_t o_off = o; o += al(4 * ((size_t)n_landmarks + 1));
-    const size_t in_bytes = o, out_begin = o;
-    const size_t o_best = o; o += al(4 * (size_t)n_landmarks);
-    const size_t o_out = o; o += al(32 * (size_t)n_landmarks);
-    const size_t out_end = o;
-    int rc;
-    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, o))) return rc;
-    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, out_end))) return rc;
-    unsigned char *hb = m.h_guided, *db = m.d_guided;
-    if (total) std::memcpy(hb + o_desc, descs, 32 * total);
-    std::memcpy(hb + o_off, offsets, 4 * ((size_t)n_landmarks + 1));
+    b200::Layout a;
+    const size_t o_desc = a.take(32 * total), o_off = a.take(4 * ((size_t)n_landmarks + 1));
+    const size_t in_bytes = a.end, out_begin = a.end;
+    const size_t o_best = a.take(4 * (size_t)n_landmarks), o_out = a.take(32 * (size_t)n_landmarks);
+    const size_t out_end = a.end;
     cudaStream_t st = m.stream;
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    int rc;
+    if ((rc = m.arena.reserve(a.end, out_end, st))) return rc;
+    b200::StagingArena& A = m.arena;
+    unsigned char *hb = A.h, *db = A.d;
+    A.put(o_desc, descs, 32 * total);
+    A.put(o_off, offsets, 4 * ((size_t)n_landmarks + 1));
+    B200_CUDA(A.upload(in_bytes, st));
     b200::match::landmark_descriptor_kernel<<<b200::ceil_div(n_landmarks, 4), 128, 0, st>>>((const uint4*)(db + o_desc), (const int*)(db + o_off), n_landmarks,
                                                                                          (int*)(db + o_best), desc_out ? (uint4*)(db + o_out) : nullptr);
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpyAsync(hb + out_begin, db + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A.download(out_begin, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
-    m.last_h2d = in_bytes;
-    m.last_d2h = out_end - out_begin;
     std::memcpy(best_idx, hb + o_best, 4 * (size_t)n_landmarks);
     for (int l = 0; l < n_landmarks; ++l)
         if (best_idx[l] == -2) {
@@ -2465,35 +2404,28 @@ int b200_landmark_geometry(b200_matcher_t h, int n_landmarks, const double* pos_
     if (total > 0 && !cam_centers) return B200_ERR_INVALID;
     auto& m = h->m;
     B200_CUDA(cudaSetDevice(m.device));
-    auto al = [](size_t v) { return b200::round_up(v, (size_t)256); };
-    size_t o = 0;
-    const size_t o_p = o; o += al(24 * N);
-    const size_t o_off = o; o += al(4 * (N + 1));
-    const size_t o_c = o; o += al(24 * std::max(total, (size_t)1));
-    const size_t o_r = o; o += al(24 * N);
-    const size_t o_s = o; o += al(4 * N);
-    const size_t in_bytes = o, out_begin = o;
-    const size_t o_mn = o; o += al(24 * N);
-    const size_t o_mx = o; o += al(4 * N);
-    const size_t o_mi = o; o += al(4 * N);
-    const size_t out_end = o;
-    int rc;
-    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, o))) return rc;
-    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, out_end))) return rc;
-    unsigned char *hb = m.h_guided, *db = m.d_guided;
-    std::memcpy(hb + o_p, pos_w, 24 * N);
-    std::memcpy(hb + o_off, offsets, 4 * (N + 1));
-    if (total) std::memcpy(hb + o_c, cam_centers, 24 * total);
-    std::memcpy(hb + o_r, ref_center, 24 * N);
-    std::memcpy(hb + o_s, ref_scale_factor, 4 * N);
+    b200::Layout a;
+    const size_t o_p = a.take(24 * N), o_off = a.take(4 * (N + 1)), o_c = a.take(24 * total), o_r = a.take(24 * N), o_s = a.take(4 * N);
+    const size_t in_bytes = a.end, out_begin = a.end;
+    const size_t o_mn = a.take(24 * N), o_mx = a.take(4 * N), o_mi = a.take(4 * N);
+    const size_t out_end = a.end;
     cudaStream_t st = m.stream;
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    int rc;
+    if ((rc = m.arena.reserve(a.end, out_end, st))) return rc;
+    b200::StagingArena& A = m.arena;
+    unsigned char *hb = A.h, *db = A.d;
+    A.put(o_p, pos_w, 24 * N);
+    A.put(o_off, offsets, 4 * (N + 1));
+    A.put(o_c, cam_centers, 24 * total);
+    A.put(o_r, ref_center, 24 * N);
+    A.put(o_s, ref_scale_factor, 4 * N);
+    B200_CUDA(A.upload(in_bytes, st));
     b200::match::landmark_geometry_kernel<<<b200::ceil_div(n_landmarks, 128), 128, 0, st>>>(n_landmarks, (const double*)(db + o_p), (const int*)(db + o_off),
                                                                                          (const double*)(db + o_c), (const double*)(db + o_r),
                                                                                          (const float*)(db + o_s), inv_scale_factor_last,
                                                                                          (double*)(db + o_mn), (float*)(db + o_mx), (float*)(db + o_mi));
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpyAsync(hb + out_begin, db + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A.download(out_begin, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
     std::memcpy(mean_normal, hb + o_mn, 24 * N);
     std::memcpy(max_valid_dist, hb + o_mx, 4 * N);
@@ -2539,38 +2471,48 @@ int b200_depth_landmarks(b200_matcher_t h, int n_problems, b200_depth_landmarks_
     }
     // one pinned staging block: the problem table, then per problem its inputs (x, y, depth, octave, has_landmark, scale factors) and
     // its outputs (n_created, idx, pos_w, mean_normal, min / max valid distance)
-    auto al = [](size_t v) { return b200::round_up(v, (size_t)256); };
-    struct Lay { size_t in, out, n, lv; };
+    struct Lay { size_t x, y, depth, oct, has_lm, sf, n_created, idx, pos, nrm, lo, hi; };
     std::vector<Lay> lay(n_problems);
-    size_t o = al(sizeof(DepthLmDev) * (size_t)std::max(n_problems, 1));
+    auto staged = [&](int p) { return problems[p].status == B200_OK ? (size_t)problems[p].n_keypoints : 0; };
+    b200::Layout a;
+    a.take<DepthLmDev>(n_problems);  // at offset 0
     for (int p = 0; p < n_problems; ++p) {
-        const bool run = problems[p].status == B200_OK;
-        lay[p].n = run ? (size_t)problems[p].n_keypoints : 0;
-        lay[p].lv = run ? (size_t)problems[p].num_levels : 0;
-        lay[p].in = o;
-        o += 4 * al(4 * lay[p].n) + al(lay[p].n) + al(4 * lay[p].lv);
+        const size_t n = staged(p), lv = problems[p].status == B200_OK ? (size_t)problems[p].num_levels : 0;
+        Lay& L = lay[p];
+        L.x = a.take(4 * n);
+        L.y = a.take(4 * n);
+        L.depth = a.take(4 * n);
+        L.oct = a.take(4 * n);
+        L.has_lm = a.take(n);
+        L.sf = a.take(4 * lv);
     }
-    const size_t in_bytes = o;
+    const size_t in_bytes = a.end;
     for (int p = 0; p < n_problems; ++p) {
-        lay[p].out = o;
-        o += al(4) + al(4 * lay[p].n) + 2 * al(24 * lay[p].n) + 2 * al(4 * lay[p].n);
+        const size_t n = staged(p);
+        Lay& L = lay[p];
+        L.n_created = a.take(4);
+        L.idx = a.take(4 * n);
+        L.pos = a.take(24 * n);
+        L.nrm = a.take(24 * n);
+        L.lo = a.take(4 * n);
+        L.hi = a.take(4 * n);
     }
-    const size_t out_end = o;
+    const size_t out_end = a.end;
     auto& m = h->m;
     B200_CUDA(cudaSetDevice(m.device));
+    cudaStream_t st = m.stream;
     int rc;
-    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, out_end))) return rc;
-    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, out_end))) return rc;
-    unsigned char *hb = m.h_guided, *db = m.d_guided;
-    DepthLmDev* dev = reinterpret_cast<DepthLmDev*>(hb);
+    if ((rc = m.arena.reserve(out_end, out_end, st))) return rc;
+    b200::StagingArena& A = m.arena;
+    DepthLmDev* dev = A.host<DepthLmDev>(0);
     int npow_max = 1;
     for (int p = 0; p < n_problems; ++p) {
         const b200_depth_landmarks_problem_t& P = problems[p];
         DepthLmDev& D = dev[p];
         std::memset(&D, 0, sizeof(D));
         if (P.status != B200_OK) continue;  // n_created == nullptr: the kernel skips it
-        const size_t n = lay[p].n, a4 = al(4 * n);
-        size_t b = lay[p].in;
+        const Lay& L = lay[p];
+        const size_t n = (size_t)P.n_keypoints;
         D.mode = P.mode;
         D.n = P.n_keypoints;
         D.n_valid = nv[p];
@@ -2585,50 +2527,45 @@ int b200_depth_landmarks(b200_matcher_t h, int n_problems, b200_depth_landmarks_
         D.fx_inv = P.fx_inv; D.fy_inv = P.fy_inv; D.cx = P.cx; D.cy = P.cy; D.depth_thr = P.depth_thr;
         D.inv_last = P.inv_scale_factor_last;
         if (n) {
-            std::memcpy(hb + b, P.x, 4 * n);              D.x = (const float*)(db + b);      b += a4;
-            std::memcpy(hb + b, P.y, 4 * n);              D.y = (const float*)(db + b);      b += a4;
-            std::memcpy(hb + b, P.depth, 4 * n);          D.depth = (const float*)(db + b);  b += a4;
-            std::memcpy(hb + b, P.octave, 4 * n);         D.octave = (const int*)(db + b);   b += a4;
+            A.put(L.x, P.x, 4 * n);          D.x = A.dev<const float>(L.x);
+            A.put(L.y, P.y, 4 * n);          D.y = A.dev<const float>(L.y);
+            A.put(L.depth, P.depth, 4 * n);  D.depth = A.dev<const float>(L.depth);
+            A.put(L.oct, P.octave, 4 * n);   D.octave = A.dev<const int>(L.oct);
             if (P.has_landmark && P.mode == B200_DEPTH_LM_KEYFRAME) {
-                std::memcpy(hb + b, P.has_landmark, n);
-                D.has_lm = db + b;
+                A.put(L.has_lm, P.has_landmark, n);
+                D.has_lm = A.dev(L.has_lm);
             }
-            b += al(n);
         }
-        std::memcpy(hb + b, P.scale_factors, 4 * lay[p].lv);
-        D.sf = (const float*)(db + b);
-        size_t q = lay[p].out;
-        D.n_created = (int*)(db + q);          q += al(4);
-        D.out_idx = (int*)(db + q);            q += a4;
-        D.pos_w = (double*)(db + q);           q += al(24 * n);
-        D.mean_normal = (double*)(db + q);     q += al(24 * n);
-        D.min_valid = (float*)(db + q);        q += a4;
-        D.max_valid = (float*)(db + q);
+        A.put(L.sf, P.scale_factors, 4 * (size_t)P.num_levels);
+        D.sf = A.dev<const float>(L.sf);
+        D.n_created = A.dev<int>(L.n_created);
+        D.out_idx = A.dev<int>(L.idx);
+        D.pos_w = A.dev<double>(L.pos);
+        D.mean_normal = A.dev<double>(L.nrm);
+        D.min_valid = A.dev<float>(L.lo);
+        D.max_valid = A.dev<float>(L.hi);
     }
     if (n_problems == 0) return B200_OK;
-    cudaStream_t st = m.stream;
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
-    B200_CUDA(cudaMemsetAsync(db + in_bytes, 0, out_end - in_bytes, st));
+    B200_CUDA(A.upload(in_bytes, st));
+    B200_CUDA(cudaMemsetAsync(A.dev(in_bytes), 0, out_end - in_bytes, st));
     const size_t smem = sizeof(unsigned long long) * (size_t)npow_max;
     B200_CUDA(cudaFuncSetAttribute(b200::match::depth_landmarks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    b200::match::depth_landmarks_kernel<<<n_problems, b200::match::kDepthLmThreads, smem, st>>>((const DepthLmDev*)db);
+    b200::match::depth_landmarks_kernel<<<n_problems, b200::match::kDepthLmThreads, smem, st>>>(A.dev<const DepthLmDev>(0));
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpyAsync(hb + in_bytes, db + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A.download(in_bytes, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
     for (int p = 0; p < n_problems; ++p) {
         b200_depth_landmarks_problem_t& P = problems[p];
         if (P.status != B200_OK) continue;
-        const size_t n = lay[p].n, a4 = al(4 * n);
-        size_t q = lay[p].out;
-        int k = 0;
-        std::memcpy(&k, hb + q, 4);            q += al(4);
+        const Lay& L = lay[p];
+        const int k = *A.host<const int>(L.n_created);
         P.n_created = k;
         const size_t K = (size_t)k;
-        std::memcpy(P.created_idx, hb + q, 4 * K);      q += a4;
-        std::memcpy(P.pos_w, hb + q, 24 * K);           q += al(24 * n);
-        std::memcpy(P.mean_normal, hb + q, 24 * K);     q += al(24 * n);
-        std::memcpy(P.min_valid_dist, hb + q, 4 * K);   q += a4;
-        std::memcpy(P.max_valid_dist, hb + q, 4 * K);
+        std::memcpy(P.created_idx, A.host(L.idx), 4 * K);
+        std::memcpy(P.pos_w, A.host(L.pos), 24 * K);
+        std::memcpy(P.mean_normal, A.host(L.nrm), 24 * K);
+        std::memcpy(P.min_valid_dist, A.host(L.lo), 4 * K);
+        std::memcpy(P.max_valid_dist, A.host(L.hi), 4 * K);
     }
     return first_bad;
 }
@@ -2652,14 +2589,15 @@ int b200_hamming_matrix(b200_matcher_t h, const uint8_t* desc1, int n1, const ui
     if (!desc1 || !desc2 || !dist) return B200_ERR_INVALID;
     auto& m = h->m;
     B200_CUDA(cudaSetDevice(m.device));
-    const size_t o_d2 = b200::round_up((size_t)32 * n1, (size_t)256), o_out = o_d2 + b200::round_up((size_t)32 * n2, (size_t)256);
-    int rc = m.grow((void**)&m.d_stage, &m.stage_cap, o_out + sizeof(uint16_t) * (size_t)n1 * n2);
+    b200::Layout L;
+    const size_t o_d1 = L.take((size_t)32 * n1), o_d2 = L.take((size_t)32 * n2), o_out = L.take<uint16_t>((size_t)n1 * n2);
+    int rc = m.arena.reserve(L.end, 0, m.stream);
     if (rc) return rc;
-    unsigned char* s = m.d_stage;
-    B200_CUDA(cudaMemcpyAsync(s, desc1, (size_t)32 * n1, cudaMemcpyHostToDevice, m.stream));
+    unsigned char* s = m.arena.d;
+    B200_CUDA(cudaMemcpyAsync(s + o_d1, desc1, (size_t)32 * n1, cudaMemcpyHostToDevice, m.stream));
     B200_CUDA(cudaMemcpyAsync(s + o_d2, desc2, (size_t)32 * n2, cudaMemcpyHostToDevice, m.stream));
     b200::match::hamming_matrix_kernel<<<dim3(b200::ceil_div(n2, 64), b200::ceil_div(n1, 256)), 256, 0, m.stream>>>(
-        (const uint4*)s, n1, (const uint4*)(s + o_d2), n2, (unsigned short*)(s + o_out));
+        (const uint4*)(s + o_d1), n1, (const uint4*)(s + o_d2), n2, (unsigned short*)(s + o_out));
     B200_CUDA(cudaGetLastError());
     B200_CUDA(cudaMemcpyAsync(dist, s + o_out, sizeof(uint16_t) * (size_t)n1 * n2, cudaMemcpyDeviceToHost, m.stream));
     B200_CUDA(cudaStreamSynchronize(m.stream));
@@ -2776,29 +2714,6 @@ __global__ void __launch_bounds__(kClaimThreads) landmark_claim_kernel(const Tri
     }
 }
 
-// host-side staging: caller arrays are packed into one pinned buffer and go up in one copy
-struct Stage {
-    struct Item {
-        size_t off;
-        const void* src;
-        size_t bytes;
-    };
-    std::vector<Item> items;
-    size_t o = 0;
-    static size_t al(size_t v) { return round_up(v, (size_t)256); }
-    size_t add(const void* src, size_t bytes) {
-        const size_t at = o;
-        items.push_back({at, src, src ? bytes : 0});
-        o += al(std::max(bytes, (size_t)1));
-        return at;
-    }
-    size_t reserve(size_t bytes) {
-        const size_t at = o;
-        o += al(std::max(bytes, (size_t)1));
-        return at;
-    }
-};
-
 struct KfLay {
     size_t x, y, oct, xr, dep, b, sf, ls;
 };
@@ -2816,21 +2731,32 @@ bool kp_valid(const b200_tri_keyframe_t* K, int i) {
            && !(K->model == 1 && K->x_right && K->x_right[i] >= 0.0f);
 }
 
-KfLay stage_kf(Stage& s, const b200_tri_keyframe_t* K) {
+KfLay layout_kf(Layout& a, const b200_tri_keyframe_t* K) {
     const size_t n = (size_t)K->n_keypoints, nl = (size_t)K->num_levels;
     KfLay L;
-    L.x = s.add(K->x, 4 * n);
-    L.y = s.add(K->y, 4 * n);
-    L.oct = s.add(K->octave, 4 * n);
-    L.xr = s.add(K->x_right, 4 * n);
-    L.dep = s.add(K->depth, 4 * n);
-    L.b = s.add(K->bearings, 24 * n);
-    L.sf = s.add(K->scale_factors, 4 * nl);
-    L.ls = s.add(K->level_sigma_sq, 4 * nl);
+    L.x = a.take(4 * n);
+    L.y = a.take(4 * n);
+    L.oct = a.take(4 * n);
+    L.xr = a.take(4 * n);
+    L.dep = a.take(4 * n);
+    L.b = a.take(24 * n);
+    L.sf = a.take(4 * nl);
+    L.ls = a.take(4 * nl);
     return L;
 }
 
-TriKfDev make_kf(const b200_tri_keyframe_t* K, const KfLay& L, unsigned char* db) {
+// Stages the keyframe's arrays at L and returns its device view.
+TriKfDev make_kf(const b200_tri_keyframe_t* K, const KfLay& L, StagingArena& A) {
+    const size_t n = (size_t)K->n_keypoints, nl = (size_t)K->num_levels;
+    A.put(L.x, K->x, 4 * n);
+    A.put(L.y, K->y, 4 * n);
+    A.put(L.oct, K->octave, 4 * n);
+    A.put(L.xr, K->x_right, 4 * n);
+    A.put(L.dep, K->depth, 4 * n);
+    A.put(L.b, K->bearings, 24 * n);
+    A.put(L.sf, K->scale_factors, 4 * nl);
+    A.put(L.ls, K->level_sigma_sq, 4 * nl);
+    const unsigned char* db = A.d;
     TriKfDev d{};
     std::memcpy(d.pose_cw, K->pose_cw, sizeof(d.pose_cw));
     std::memcpy(d.pose_wc, K->pose_wc, sizeof(d.pose_wc));
@@ -2901,31 +2827,29 @@ int b200_triangulate_pairs(b200_matcher_t h, int n_problems, b200_triangulate_pr
         tp[p] = TriProblemDev{kf_row(P.keyfrm_1), kf_row(P.keyfrm_2), c.x, c.y, total};
         total += P.n_matches;
     }
-    Stage s;
-    const size_t o_kfs = s.reserve(sizeof(TriKfDev) * kf_list.size());
-    const size_t o_ps = s.reserve(sizeof(TriProblemDev) * (size_t)n_problems);
+    b200::Layout a;
+    const size_t o_kfs = a.take<TriKfDev>(kf_list.size());
+    const size_t o_ps = a.take<TriProblemDev>(n_problems);
     std::vector<KfLay> kl;
-    for (const b200_tri_keyframe_t* K : kf_list) kl.push_back(stage_kf(s, K));
+    for (const b200_tri_keyframe_t* K : kf_list) kl.push_back(layout_kf(a, K));
     // every problem's (idx_1, idx_2) rows, consecutive in problem order
-    const size_t o_matches = s.reserve(8 * (size_t)std::max(total, 1));
-    const size_t in_bytes = s.o, out_begin = s.o;
-    const size_t o_pos = s.reserve(24 * (size_t)std::max(total, 1));
-    const size_t o_ok = s.reserve((size_t)std::max(total, 1));
-    const size_t o_unconv = s.reserve(4);
-    const size_t out_end = s.o;
-    int rc;
-    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, s.o))) return rc;
-    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, s.o))) return rc;
-    unsigned char *hb = m.h_guided, *db = m.d_guided;
-    for (const Stage::Item& it : s.items)
-        if (it.bytes) std::memcpy(hb + it.off, it.src, it.bytes);
-    for (int p = 0; p < n_problems; ++p)
-        if (problems[p].n_matches) std::memcpy(hb + o_matches + 8 * (size_t)tp[p].begin, problems[p].matches, 8 * (size_t)problems[p].n_matches);
-    TriKfDev* hk = reinterpret_cast<TriKfDev*>(hb + o_kfs);
-    for (size_t r = 0; r < kf_list.size(); ++r) hk[r] = make_kf(kf_list[r], kl[r], db);
-    std::memcpy(hb + o_ps, tp.data(), sizeof(TriProblemDev) * (size_t)n_problems);
+    const size_t o_matches = a.take(8 * (size_t)total);
+    const size_t in_bytes = a.end, out_begin = a.end;
+    const size_t o_pos = a.take(24 * (size_t)total);
+    const size_t o_ok = a.take((size_t)total);
+    const size_t o_unconv = a.take(4);
+    const size_t out_end = a.end;
     cudaStream_t st = m.stream;
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    int rc;
+    if ((rc = m.arena.reserve(a.end, a.end, st))) return rc;
+    b200::StagingArena& A = m.arena;
+    unsigned char *hb = A.h, *db = A.d;
+    for (int p = 0; p < n_problems; ++p)
+        A.put(o_matches + 8 * (size_t)tp[p].begin, problems[p].matches, 8 * (size_t)problems[p].n_matches);
+    TriKfDev* hk = A.host<TriKfDev>(o_kfs);
+    for (size_t r = 0; r < kf_list.size(); ++r) hk[r] = make_kf(kf_list[r], kl[r], A);
+    A.put(o_ps, tp.data(), sizeof(TriProblemDev) * (size_t)n_problems);
+    B200_CUDA(A.upload(in_bytes, st));
     B200_CUDA(cudaMemsetAsync(db + o_unconv, 0, 4, st));
     if (total > 0) {
         triangulate_pairs_kernel<<<b200::ceil_div(total, 256), 256, 0, st>>>(
@@ -2933,10 +2857,8 @@ int b200_triangulate_pairs(b200_matcher_t h, int n_problems, b200_triangulate_pr
             (double*)(db + o_pos), db + o_ok, (int*)(db + o_unconv));
         B200_CUDA(cudaGetLastError());
     }
-    B200_CUDA(cudaMemcpyAsync(hb + out_begin, db + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A.download(out_begin, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
-    m.last_h2d = in_bytes;
-    m.last_d2h = out_end - out_begin;
     const int unconverged = *reinterpret_cast<const int*>(hb + o_unconv);
     if (unconverged > 0) {
         b200::set_error("b200_triangulate_pairs: the 4x4 Jacobi SVD did not converge within %d sweeps for %d matches", b200::tri::kMaxSweeps,
@@ -3007,14 +2929,14 @@ int b200_create_new_landmarks(b200_matcher_t h, int n_keyframes, b200_new_landma
         out.resize(K->n_keypoints);
         for (int i = 0; i < K->n_keypoints; ++i) out[i] = K->x_right[i] >= 0.0f;
     };
-    Stage s;
+    b200::Layout s;
     const size_t P_total = (size_t)n_ranks * n_kf;
-    const size_t o_pairs = s.reserve(sizeof(PairsDev) * P_total);
-    const size_t o_chain = s.reserve(sizeof(ChainKfDev) * n_kf);
+    const size_t o_pairs = s.take<PairsDev>(P_total);
+    const size_t o_chain = s.take<ChainKfDev>(n_kf);
     int n_views = 0;
     for (int k = 0; k < n_kf; ++k) n_views += 1 + problems[k].n_neighbours;
-    const size_t o_kfs = s.reserve(sizeof(TriKfDev) * n_views);
-    const size_t o_consts = s.reserve(8 * (size_t)n_views);
+    const size_t o_kfs = s.take<TriKfDev>(n_views);
+    const size_t o_consts = s.take(8 * (size_t)n_views);
     struct CurLay {
         KfLay kf;
         size_t desc, valid, node, scale, stereo;
@@ -3033,12 +2955,12 @@ int b200_create_new_landmarks(b200_matcher_t h, int n_keyframes, b200_new_landma
         for (size_t i = 0; i < n1; ++i) scale1[k][i] = C->scale_factors[C->octave[i]];
         stereo_of(C, stereo_cur[k]);
         CurLay& L = cl[k];
-        L.kf = stage_kf(s, C);
-        L.desc = s.add(P.desc, 32 * n1);
-        L.valid = s.add(P.valid, n1);
-        L.node = s.add(P.node, 4 * n1);
-        L.scale = s.add(scale1[k].data(), 4 * n1);
-        L.stereo = s.add(C->x_right ? stereo_cur[k].data() : nullptr, n1);
+        L.kf = layout_kf(s, C);
+        L.desc = s.take(32 * n1);
+        L.valid = s.take(n1);
+        L.node = s.take(4 * n1);
+        L.scale = s.take(4 * n1);
+        L.stereo = s.take(n1);
         stereo_nb[k].resize(P.n_neighbours);
         nl[k].resize(P.n_neighbours);
         for (int r = 0; r < P.n_neighbours; ++r) {
@@ -3046,21 +2968,21 @@ int b200_create_new_landmarks(b200_matcher_t h, int n_keyframes, b200_new_landma
             const size_t n2 = (size_t)N.keyfrm->n_keypoints;
             stereo_of(N.keyfrm, stereo_nb[k][r]);
             NbLay& M = nl[k][r];
-            M.kf = stage_kf(s, N.keyfrm);
-            M.desc = s.add(N.desc, 32 * n2);
-            M.valid = s.add(N.valid, n2);
-            M.node = s.add(N.node, 4 * n2);
-            M.stereo = s.add(N.keyfrm->x_right ? stereo_nb[k][r].data() : nullptr, n2);
+            M.kf = layout_kf(s, N.keyfrm);
+            M.desc = s.take(32 * n2);
+            M.valid = s.take(n2);
+            M.node = s.take(4 * n2);
+            M.stereo = s.take(n2);
         }
     }
-    const size_t in_bytes = s.o, out_begin = s.o;
+    const size_t in_bytes = s.end, out_begin = s.end;
     // outputs (one download): per problem match_out + n_matches, per keyframe the created list and counts, the two flags
     std::vector<size_t> o_mout(P_total), o_nm(P_total);
     for (int r = 0; r < n_ranks; ++r)
         for (int k = 0; k < n_kf; ++k) {
             const size_t q = (size_t)r * n_kf + k;
-            o_mout[q] = s.reserve(4 * (size_t)(r < problems[k].n_neighbours ? problems[k].keyfrm->n_keypoints : 0));
-            o_nm[q] = s.reserve(4);
+            o_mout[q] = s.take(4 * (size_t)(r < problems[k].n_neighbours ? problems[k].keyfrm->n_keypoints : 0));
+            o_nm[q] = s.take(4);
         }
     struct OutLay {
         size_t n_rank, n_created, rank, idx, pos;
@@ -3068,38 +2990,43 @@ int b200_create_new_landmarks(b200_matcher_t h, int n_keyframes, b200_new_landma
     std::vector<OutLay> ol(n_kf);
     for (int k = 0; k < n_kf; ++k) {
         const size_t n1 = (size_t)problems[k].keyfrm->n_keypoints;
-        ol[k].n_rank = s.reserve(4 * (size_t)std::max(problems[k].n_neighbours, 1));
-        ol[k].n_created = s.reserve(4);
-        ol[k].rank = s.reserve(4 * n1);
-        ol[k].idx = s.reserve(8 * n1);
-        ol[k].pos = s.reserve(24 * n1);
+        ol[k].n_rank = s.take(4 * (size_t)problems[k].n_neighbours);
+        ol[k].n_created = s.take(4);
+        ol[k].rank = s.take(4 * n1);
+        ol[k].idx = s.take(8 * n1);
+        ol[k].pos = s.take(24 * n1);
     }
-    const size_t o_overflow = s.reserve(4), o_unconv = s.reserve(4);
-    const size_t out_end = s.o;
+    const size_t o_overflow = s.take(4), o_unconv = s.take(4);
+    const size_t out_end = s.end;
     std::vector<size_t> o_lists(P_total), o_llen(P_total);
     for (int r = 0; r < n_ranks; ++r)
         for (int k = 0; k < n_kf; ++k) {
             const size_t q = (size_t)r * n_kf + k;
             const size_t n1 = r < problems[k].n_neighbours ? (size_t)problems[k].keyfrm->n_keypoints : 0;
-            o_lists[q] = s.reserve(8 * (size_t)cap * n1);
-            o_llen[q] = s.reserve(4 * n1);
+            o_lists[q] = s.take(8 * (size_t)cap * n1);
+            o_llen[q] = s.take(4 * n1);
         }
+    cudaStream_t st = m.stream;
     int rc;
-    if ((rc = m.grow((void**)&m.d_guided, &m.d_guided_cap, s.o))) return rc;
-    if ((rc = m.grow_pinned(&m.h_guided, &m.h_guided_cap, out_end))) return rc;
-    unsigned char *hb = m.h_guided, *db = m.d_guided;
-    for (const Stage::Item& it : s.items)
-        if (it.bytes) std::memcpy(hb + it.off, it.src, it.bytes);
-    TriKfDev* hk = reinterpret_cast<TriKfDev*>(hb + o_kfs);
-    float2* hc = reinterpret_cast<float2*>(hb + o_consts);
-    ChainKfDev* hch = reinterpret_cast<ChainKfDev*>(hb + o_chain);
-    PairsDev* hg = reinterpret_cast<PairsDev*>(hb + o_pairs);
+    if ((rc = m.arena.reserve(s.end, out_end, st))) return rc;
+    b200::StagingArena& A = m.arena;
+    unsigned char *hb = A.h, *db = A.d;
+    TriKfDev* hk = A.host<TriKfDev>(o_kfs);
+    float2* hc = A.host<float2>(o_consts);
+    ChainKfDev* hch = A.host<ChainKfDev>(o_chain);
+    PairsDev* hg = A.host<PairsDev>(o_pairs);
     int view = 0;
     for (int k = 0; k < n_kf; ++k) {
         const b200_new_landmarks_problem_t& P = problems[k];
         const b200_tri_keyframe_t* C = P.keyfrm;
+        const size_t n1 = (size_t)C->n_keypoints;
         const int cur = view++;
-        hk[cur] = make_kf(C, cl[k].kf, db);
+        hk[cur] = make_kf(C, cl[k].kf, A);
+        A.put(cl[k].desc, P.desc, 32 * n1);
+        A.put(cl[k].valid, P.valid, n1);
+        A.put(cl[k].node, P.node, 4 * n1);
+        A.put(cl[k].scale, scale1[k].data(), 4 * n1);
+        A.put(cl[k].stereo, C->x_right ? stereo_cur[k].data() : nullptr, n1);
         ChainKfDev K{};
         K.cur = cur;
         K.n_nb = P.n_neighbours;
@@ -3120,7 +3047,12 @@ int b200_create_new_landmarks(b200_matcher_t h, int n_keyframes, b200_new_landma
             if (r < P.n_neighbours) {
                 const b200_new_landmarks_neighbour_t& N = P.neighbours[r];
                 const NbLay& M = nl[k][r];
-                hk[view] = make_kf(N.keyfrm, M.kf, db);
+                const size_t n2 = (size_t)N.keyfrm->n_keypoints;
+                hk[view] = make_kf(N.keyfrm, M.kf, A);
+                A.put(M.desc, N.desc, 32 * n2);
+                A.put(M.valid, N.valid, n2);
+                A.put(M.node, N.node, 4 * n2);
+                A.put(M.stereo, N.keyfrm->x_right ? stereo_nb[k][r].data() : nullptr, n2);
                 hc[view] = tri_constants(C, N.keyfrm, rays_parallax_deg_thr);
                 ++view;
                 g.n_queries = C->n_keypoints;
@@ -3145,9 +3077,8 @@ int b200_create_new_landmarks(b200_matcher_t h, int n_keyframes, b200_new_landma
         }
         hch[k] = K;
     }
-    cudaStream_t st = m.stream;
-    const PairsDev* dg = reinterpret_cast<const PairsDev*>(db + o_pairs);
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    const PairsDev* dg = A.dev<const PairsDev>(o_pairs);
+    B200_CUDA(A.upload(in_bytes, st));
     B200_CUDA(cudaMemsetAsync(db + out_begin, 0, out_end - out_begin, st));
     b200::match::pairs_candidates_kernel<<<dim3(std::max(1, b200::ceil_div(max_n1, b200::match::kPairRows)), (unsigned)P_total),
                                            b200::match::kPairRows, 0, st>>>(dg, B200_PAIRS_TRIANGULATION, (unsigned)b200::match::kThrLow, 0,
@@ -3160,10 +3091,8 @@ int b200_create_new_landmarks(b200_matcher_t h, int n_keyframes, b200_new_landma
                                                               (int*)(db + o_unconv));
     }
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpyAsync(hb + out_begin, db + out_begin, out_end - out_begin, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A.download(out_begin, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
-    m.last_h2d = in_bytes;
-    m.last_d2h = out_end - out_begin;
     const int overflow = *reinterpret_cast<const int*>(hb + o_overflow);
     if (overflow > 0) {
         b200::set_error("b200_create_new_landmarks: a row kept %d gated candidates, max_candidates is %d", overflow, cap);

@@ -24,6 +24,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "staging.cuh"
 #include "track_chain.cuh"
 #include "util_trig.cuh"
 
@@ -2014,19 +2015,12 @@ int b200_frame_can_observe(b200_orb_t h, const b200_camera_intrinsics_t* cam, do
     a.ray_cos_thr = ray_cos_thr;
     a.log_scale_factor = log_scale_factor;
     a.num_levels = num_levels;
-    auto al = [](size_t v) { return b200::round_up(v, (size_t)256); };
     const size_t N = (size_t)n;
-    size_t o = 0;
-    const size_t o_p = o; o += al(24 * N);
-    const size_t o_n = o; o += al(24 * N);
-    const size_t o_lo = o; o += al(4 * N);
-    const size_t o_hi = o; o += al(4 * N);
-    const size_t o_ok = o; o += al(N);
-    const size_t o_rp = o; o += al(16 * N);
-    const size_t o_xr = o; o += al(4 * N);
-    const size_t o_lv = o; o += al(4 * N);
+    b200::Layout L;
+    const size_t o_p = L.take(24 * N), o_n = L.take(24 * N), o_lo = L.take(4 * N), o_hi = L.take(4 * N);
+    const size_t o_ok = L.take(N), o_rp = L.take(16 * N), o_xr = L.take(4 * N), o_lv = L.take(4 * N);
     unsigned char* d = nullptr;
-    B200_CUDA(cudaMallocAsync((void**)&d, o, ex.stream));
+    B200_CUDA(cudaMallocAsync((void**)&d, L.end, ex.stream));
     cudaStream_t st = ex.stream;
     cudaError_t e = cudaMemcpyAsync(d + o_p, pos_w, 24 * N, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d + o_n, mean_normal, 24 * N, cudaMemcpyHostToDevice, st);
@@ -2179,16 +2173,11 @@ int b200_rgbd_depths(b200_orb_t h, int n_frames, const b200_camera_intrinsics_t*
     B200_CUDA(cudaSetDevice(ex.prm.device));
     cudaStream_t st = ex.stream;
     const size_t F = (size_t)n_frames, M = F * (size_t)cap, map_bytes = row * (size_t)height;
-    auto al = [](size_t v) { return b200::round_up(v, (size_t)256); };
-    size_t o = 0;
-    const size_t o_map = o; o += al(map_bytes * F);
-    const size_t o_kp = o; o += al(sizeof(b200_keypoint_t) * M);
-    const size_t o_b = o; o += al(24 * M);
-    const size_t o_d = o; o += al(4 * M);
-    const size_t o_xr = o; o += al(4 * M);
-    const size_t o_n = o; o += al(4 * F);
+    b200::Layout L;
+    const size_t o_map = L.take(map_bytes * F), o_kp = L.take<b200_keypoint_t>(M), o_b = L.take(24 * M), o_d = L.take(4 * M);
+    const size_t o_xr = L.take(4 * M), o_n = L.take(4 * F);
     unsigned char* d = nullptr;
-    B200_CUDA(cudaMallocAsync((void**)&d, o, st));
+    B200_CUDA(cudaMallocAsync((void**)&d, L.end, st));
     const unsigned char* src = static_cast<const unsigned char*>(depth_maps);
     cudaError_t e = cudaSuccess;
     if (F == 1 || frame_stride == pitch * (size_t)height)

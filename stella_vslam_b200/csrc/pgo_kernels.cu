@@ -24,6 +24,7 @@
 
 #include "common.cuh"
 #include "sim3.cuh"
+#include "staging.cuh"
 
 namespace b200 {
 
@@ -541,15 +542,6 @@ __global__ void __launch_bounds__(256) pgo_export_kernel(const Sim3* __restrict_
 // ---------------------------------------------------------------------------------------------------------------
 // host driver
 // ---------------------------------------------------------------------------------------------------------------
-struct Arena {
-    size_t off = 0;
-    size_t take(size_t bytes) {
-        const size_t o = off;
-        off += round_up<size_t>(bytes ? bytes : 1, 256);
-        return o;
-    }
-};
-
 struct GraphGuard {
     cudaGraph_t g = nullptr;
     cudaGraphExec_t x = nullptr;
@@ -613,7 +605,7 @@ static int solve(b200_lba_t h, const b200_pose_graph_t* g, const Plan& P, int ma
     const auto t0 = std::chrono::steady_clock::now();
     const int nv = P.nv, ne = P.ne, np = g->n_points, nb = (int)P.blk_r.size();
     const bool want_pts = g->points_out && np > 0;
-    Arena A;
+    Layout A;
     // inputs (uploaded in one copy from the staging buffer, laid out identically)
     const size_t o_est = A.take(sizeof(Sim3) * nv), o_meas = A.take(sizeof(Sim3) * ne), o_ev = A.take(sizeof(int) * 2 * ne),
                  o_vpos = A.take(sizeof(int) * nv), o_ftile = A.take(sizeof(int) * P.nt), o_toff = A.take(sizeof(long long) * P.nt),
@@ -621,39 +613,37 @@ static int solve(b200_lba_t h, const b200_pose_graph_t* g, const Plan& P, int ma
                  o_bc = A.take(sizeof(int) * nb), o_bptr = A.take(sizeof(int) * (nb + 1)), o_bcon = A.take(sizeof(int) * P.blk_con.size()),
                  o_pts = A.take(sizeof(double) * 3 * (want_pts ? np : 0)), o_pref = A.take(sizeof(int) * (want_pts ? np : 0)),
                  o_ctl = A.take(sizeof(double) * 4);
-    const size_t in_bytes = A.off;
+    const size_t in_bytes = A.end;
     // outputs (downloaded in one copy)
     const size_t o_eout = A.take(sizeof(Sim3) * nv), o_pose = A.take(sizeof(double) * 16 * nv), o_pout = A.take(sizeof(double) * 3 * (want_pts ? np : 0)),
                  o_res = A.take(sizeof(double) * 4);
-    const size_t out_lo = o_eout, out_bytes = A.off - out_lo;
-    const size_t host_bytes = A.off;
+    const size_t out_lo = o_eout, out_hi = A.end;
     // device-only work buffers
     const size_t o_etr = A.take(sizeof(Sim3) * nv), o_einit = A.take(sizeof(Sim3) * nv), o_J = A.take(sizeof(double) * 98 * (size_t)ne),
                  o_err = A.take(sizeof(double) * 7 * (size_t)ne), o_chi = A.take(sizeof(double) * ne), o_blkH = A.take(sizeof(double) * 49 * (size_t)nb),
                  o_b = A.take(sizeof(double) * P.nt * kT), o_x = A.take(sizeof(double) * P.nt * kT), o_diag = A.take(sizeof(double) * kTT * (size_t)P.nt),
                  o_env = A.take(sizeof(double) * (size_t)P.env);
     cudaStream_t st;
-    unsigned char *db, *hb;
-    int rc = lba::borrow_buffers(h, A.off, host_bytes, &st, &db, &hb);
+    StagingArena* S;
+    int rc = lba::staging(h, A.end, out_hi, &st, &S);
     if (rc) return rc;
-
-    auto put = [&](size_t o, const void* src, size_t bytes) { if (bytes) memcpy(hb + o, src, bytes); };
-    put(o_est, g->estimate, sizeof(Sim3) * nv);
-    put(o_meas, g->e_meas, sizeof(Sim3) * ne);
+    unsigned char *db = S->d, *hb = S->h;
+    S->put(o_est, g->estimate, sizeof(Sim3) * nv);
+    S->put(o_meas, g->e_meas, sizeof(Sim3) * ne);
     int* ev = (int*)(hb + o_ev);
     for (int e = 0; e < ne; ++e) { ev[2 * e] = g->e_v1[e]; ev[2 * e + 1] = g->e_v2[e]; }
-    put(o_vpos, P.vpos.data(), sizeof(int) * nv);
-    put(o_ftile, P.ftile.data(), sizeof(int) * P.nt);
-    put(o_toff, P.tile_off.data(), sizeof(long long) * P.nt);
-    put(o_rptr, P.rows_ptr.data(), sizeof(int) * (P.nt + 1));
-    put(o_ridx, P.rows_idx.data(), sizeof(int) * P.rows_idx.size());
-    put(o_br, P.blk_r.data(), sizeof(int) * nb);
-    put(o_bc, P.blk_c.data(), sizeof(int) * nb);
-    put(o_bptr, P.blk_ptr.data(), sizeof(int) * (nb + 1));
-    put(o_bcon, P.blk_con.data(), sizeof(int) * P.blk_con.size());
+    S->put(o_vpos, P.vpos.data(), sizeof(int) * nv);
+    S->put(o_ftile, P.ftile.data(), sizeof(int) * P.nt);
+    S->put(o_toff, P.tile_off.data(), sizeof(long long) * P.nt);
+    S->put(o_rptr, P.rows_ptr.data(), sizeof(int) * (P.nt + 1));
+    S->put(o_ridx, P.rows_idx.data(), sizeof(int) * P.rows_idx.size());
+    S->put(o_br, P.blk_r.data(), sizeof(int) * nb);
+    S->put(o_bc, P.blk_c.data(), sizeof(int) * nb);
+    S->put(o_bptr, P.blk_ptr.data(), sizeof(int) * (nb + 1));
+    S->put(o_bcon, P.blk_con.data(), sizeof(int) * P.blk_con.size());
     if (want_pts) {
-        put(o_pts, g->points, sizeof(double) * 3 * np);
-        put(o_pref, g->point_ref, sizeof(int) * np);
+        S->put(o_pts, g->points, sizeof(double) * 3 * np);
+        S->put(o_pref, g->point_ref, sizeof(int) * np);
     }
     Dev d;
     d.est = (Sim3*)(db + o_est); d.meas = (Sim3*)(db + o_meas); d.est_trial = (Sim3*)(db + o_etr); d.est_init = (Sim3*)(db + o_einit);
@@ -672,7 +662,7 @@ static int solve(b200_lba_t h, const b200_pose_graph_t* g, const Plan& P, int ma
     GraphGuard Gf, Gs;
     for (cudaEvent_t& e : Gf.ev) B200_CUDA(cudaEventCreate(&e));
     int launches = 0, nodes_f = 0, nodes_s = 0;
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(S->upload(in_bytes, st));
     B200_CUDA(cudaMemcpyAsync(d.est_init, d.est, sizeof(Sim3) * nv, cudaMemcpyDeviceToDevice, st));
     rc = capture(st, Gf, launch_factor, d, P, &nodes_f);
     if (rc) return rc;
@@ -768,7 +758,7 @@ static int solve(b200_lba_t h, const b200_pose_graph_t* g, const Plan& P, int ma
     ++launches;
     B200_CUDA(cudaGetLastError());
     B200_CUDA(cudaMemcpyAsync(d.est_out, d.est, sizeof(Sim3) * nv, cudaMemcpyDeviceToDevice, st));
-    B200_CUDA(cudaMemcpyAsync(hb + out_lo, db + out_lo, out_bytes, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(S->download(out_lo, out_hi, st));
     B200_CUDA(cudaStreamSynchronize(st));
     memcpy(g->estimate_out, hb + o_eout, sizeof(Sim3) * nv);
     memcpy(g->pose_cw_out, hb + o_pose, sizeof(double) * 16 * nv);

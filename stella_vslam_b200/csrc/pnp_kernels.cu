@@ -16,6 +16,7 @@
 #include "common.cuh"
 #include "epnp.cuh"
 #include "ransac_host.cuh"
+#include "staging.cuh"
 #include "util_trig.cuh"
 
 namespace b200 {
@@ -204,7 +205,7 @@ int b200_pnp_ransac(b200_lba_t h, int n_problems, b200_pnp_problem_t* problems) 
         }
     }
     const size_t T = (size_t)std::max(total, 1LL), NH = (size_t)std::max(total_hyp, 1LL);
-    b200::Staging a;
+    b200::Layout a;
     const size_t o_probs = a.take(sizeof(ProblemDev) * n_problems), o_b = a.take(24 * T), o_p = a.take(24 * T), o_sf = a.take(4 * T);
     const size_t o_ms = a.take(16 * NH), o_hp = a.take(4 * NH);
     const size_t in_bytes = a.end;
@@ -212,9 +213,10 @@ int b200_pnp_ransac(b200_lba_t h, int n_problems, b200_pnp_problem_t* problems) 
     const size_t out_end = a.end;
     const size_t o_mc = a.take(4 * T), o_hyp = a.take(sizeof(HypDev) * NH), o_idx = a.take(4 * T);
     cudaStream_t st;
-    unsigned char *db, *hb;
-    int rc = b200::lba::borrow_buffers(h, a.end, out_end, &st, &db, &hb);
+    b200::StagingArena* A;
+    int rc = b200::lba::staging(h, a.end, out_end, &st, &A);
     if (rc) return rc;
+    unsigned char *db = A->d, *hb = A->h;
     std::memcpy(hb + o_probs, pd.data(), sizeof(ProblemDev) * n_problems);
     for (int q = 0; q < n_problems; ++q) {
         const b200_pnp_problem_t& P = problems[q];
@@ -227,7 +229,7 @@ int b200_pnp_ransac(b200_lba_t h, int n_problems, b200_pnp_problem_t* problems) 
         }
         b200::stage_min_sets(q, P.min_sets, 4, pd[q].n_hyp, 4 * (size_t)pd[q].hyp_off, pd[q].hyp_off, (int32_t*)(hb + o_ms), (int*)(hb + o_hp));
     }
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(A->upload(in_bytes, st));
     const double* d_b = (const double*)(db + o_b);
     const double* d_p = (const double*)(db + o_p);
     const float* d_mc = (const float*)(db + o_mc);
@@ -245,7 +247,7 @@ int b200_pnp_ransac(b200_lba_t h, int n_problems, b200_pnp_problem_t* problems) 
                                                                       (const HypDev*)(db + o_hyp), (int32_t*)(db + o_idx), db + o_fl,
                                                                       (ResultDev*)(db + o_res));
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpyAsync(hb + o_res, db + o_res, out_end - o_res, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A->download(o_res, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
     const ResultDev* res = reinterpret_cast<const ResultDev*>(hb + o_res);
     for (int q = 0; q < n_problems; ++q) {
@@ -281,13 +283,14 @@ int b200_epnp_compute_pose(b200_lba_t h, int n_problems, b200_epnp_problem_t* pr
         total += P.n;
         if (total > INT_MAX / 4) return B200_ERR_INVALID;
     }
-    b200::Staging a;
+    b200::Layout a;
     const size_t o_probs = a.take(sizeof(EpnpDev) * n_problems), o_b = a.take(24 * (size_t)total), o_p = a.take(24 * (size_t)total);
     const size_t bytes = a.end;
     cudaStream_t st;
-    unsigned char *db, *hb;
-    int rc = b200::lba::borrow_buffers(h, bytes, bytes, &st, &db, &hb);
+    b200::StagingArena* A;
+    int rc = b200::lba::staging(h, bytes, bytes, &st, &A);
     if (rc) return rc;
+    unsigned char *db = A->d, *hb = A->h;
     EpnpDev* E = reinterpret_cast<EpnpDev*>(hb + o_probs);
     size_t off = 0;
     for (int q = 0; q < n_problems; ++q) {
@@ -301,10 +304,10 @@ int b200_epnp_compute_pose(b200_lba_t h, int n_problems, b200_epnp_problem_t* pr
         std::memcpy(hb + o_p + 24 * off, P.points, 24 * (size_t)P.n);
         off += (size_t)P.n;
     }
-    B200_CUDA(cudaMemcpyAsync(db, hb, bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(A->upload(bytes, st));
     epnp_kernel<<<b200::ceil_div(n_problems, 64), 64, 0, st>>>(n_problems, (const double*)(db + o_b), (const double*)(db + o_p), (EpnpDev*)(db + o_probs));
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpyAsync(hb + o_probs, db + o_probs, sizeof(EpnpDev) * n_problems, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A->download(o_probs, o_probs + sizeof(EpnpDev) * n_problems, st));
     B200_CUDA(cudaStreamSynchronize(st));
     for (int q = 0; q < n_problems; ++q) {
         b200_epnp_problem_t& P = problems[q];

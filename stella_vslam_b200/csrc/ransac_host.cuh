@@ -1,6 +1,5 @@
-// ransac_host.cuh -- what b200_pnp_ransac, b200_essential_ransac and b200_twoview_ransac share: the staging layout, the minimal-set
-// check and copy, and the select kernels' inlier compaction.  Each entry point keeps its own problem checks, device structs and
-// selection rule.
+// ransac_host.cuh -- what b200_pnp_ransac, b200_essential_ransac and b200_twoview_ransac share: the minimal-set check and copy,
+// and the select kernels' inlier compaction.  Each entry point keeps its own problem checks, device structs and selection rule.
 #pragma once
 
 #include <climits>
@@ -10,16 +9,6 @@
 #include "common.cuh"
 
 namespace b200 {
-
-// Offsets of consecutive blocks in a staging arena, each block starting on a 256-byte boundary; `end` is the arena's size.
-struct Staging {
-    size_t end = 0;
-    size_t take(size_t bytes) {
-        const size_t o = end;
-        end = round_up(end + bytes, (size_t)256);
-        return o;
-    }
-};
 
 // A problem that runs RANSAC has max_num_iter within int, min_sets when it iterates, and every one of its set_size * max_num_iter
 // entries in [0, n).  Reports through set_error under fn's name.

@@ -26,6 +26,7 @@
 #include "common.cuh"
 #include "lm_common.cuh"
 #include "sim3.cuh"
+#include "staging.cuh"
 
 namespace b200 {
 
@@ -400,14 +401,14 @@ int b200_transform_optimize(b200_lba_t h, int n_problems, b200_transform_problem
     if (n_problems == 0) return B200_OK;
     size_t total = 0;
     for (int p = 0; p < n_problems; ++p) total += (size_t)problems[p].n_matches;
-    const size_t o_probs = 0, o_pairs = b200::round_up(o_probs + sizeof(Prob) * n_problems, (size_t)256);
-    const size_t in_bytes = o_pairs + sizeof(Pair) * total;
-    const size_t o_out = b200::round_up(in_bytes, (size_t)256), o_keep = o_out + sizeof(Out) * n_problems;
-    const size_t bytes = o_keep + total;
+    b200::Layout L;
+    const size_t o_probs = L.take<Prob>(n_problems), o_pairs = L.take<Pair>(total);
+    const size_t in_bytes = L.end;
+    const size_t o_out = L.take<Out>(n_problems), o_keep = L.take(total);
     cudaStream_t st;
-    unsigned char *d, *hs;
-    rc = b200::lba::borrow_buffers(h, bytes + 256, bytes + 256, &st, &d, &hs);
-    if (rc) return rc;
+    b200::StagingArena* A;
+    if ((rc = b200::lba::staging(h, L.end, L.end, &st, &A))) return rc;
+    unsigned char *d = A->d, *hs = A->h;
     Prob* hp = reinterpret_cast<Prob*>(hs + o_probs);
     Pair* hq = reinterpret_cast<Pair*>(hs + o_pairs);
     size_t off = 0;
@@ -439,11 +440,11 @@ int b200_transform_optimize(b200_lba_t h, int n_problems, b200_transform_problem
         off += (size_t)P.n_matches;
     }
     const float sqrt_chi_sq = std::sqrt(chi_sq);  // transform_optimizer.cc:23: the Huber delta is computed in float
-    B200_CUDA(cudaMemcpyAsync(d, hs, in_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(A->upload(in_bytes, st));
     transform_optimize_kernel<<<n_problems, kThreads, 0, st>>>((const Prob*)(d + o_probs), (const Pair*)(d + o_pairs), d + o_keep, (Out*)(d + o_out),
                                                               (double)sqrt_chi_sq, (double)chi_sq, num_iter);
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpyAsync(hs + o_out, d + o_out, bytes - o_out, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A->download(o_out, L.end, st));
     B200_CUDA(cudaStreamSynchronize(st));
     const Out* ho = reinterpret_cast<const Out*>(hs + o_out);
     off = 0;

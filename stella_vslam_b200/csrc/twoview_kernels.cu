@@ -24,6 +24,7 @@
 #include "common.cuh"
 #include "epnp.cuh"
 #include "ransac_host.cuh"
+#include "staging.cuh"
 #include "util_trig.cuh"  // util_cos, which essential_core.h (included below for its SVD pieces) calls in es_cos_angle_thr
 
 namespace b200 {
@@ -263,7 +264,7 @@ int b200_twoview_ransac(b200_lba_t h, int n_problems, b200_twoview_problem_t* pr
     }
     const size_t T = (size_t)std::max(total, 1LL), K1 = (size_t)std::max(total_k1, 1LL), K2 = (size_t)std::max(total_k2, 1LL);
     const size_t NH = (size_t)std::max(total_hyp, 1LL), NMS = (size_t)std::max(total_ms, 1LL);
-    b200::Staging a;
+    b200::Layout a;
     const size_t o_probs = a.take(sizeof(ProblemDev) * n_problems), o_k1 = a.take(8 * K1), o_k2 = a.take(8 * K2), o_mt = a.take(8 * T);
     const size_t o_ms = a.take(4 * NMS), o_hp = a.take(4 * NH);
     const size_t in_bytes = a.end;
@@ -273,9 +274,10 @@ int b200_twoview_ransac(b200_lba_t h, int n_problems, b200_twoview_problem_t* pr
     const size_t o_hyp = a.take(sizeof(HypDev) * NH), o_sc = a.take(sizeof(ScoreDev) * NH);
     const size_t o_idx = a.take(4 * T), o_mat = a.take(8 * 18 * T);
     cudaStream_t st;
-    unsigned char *db, *hb;
-    int rc = b200::lba::borrow_buffers(h, a.end, out_end, &st, &db, &hb);
+    b200::StagingArena* A;
+    int rc = b200::lba::staging(h, a.end, out_end, &st, &A);
     if (rc) return rc;
+    unsigned char *db = A->d, *hb = A->h;
     std::memcpy(hb + o_probs, pd.data(), sizeof(ProblemDev) * n_problems);
     for (int q = 0; q < n_problems; ++q) {
         const b200_twoview_problem_t& P = problems[q];
@@ -285,7 +287,7 @@ int b200_twoview_ransac(b200_lba_t h, int n_problems, b200_twoview_problem_t* pr
         if (D.n) std::memcpy(hb + o_mt + 8 * (size_t)D.match_off, P.matches_12, 8 * (size_t)D.n);
         b200::stage_min_sets(q, P.min_sets, D.set_size, D.n_hyp, (size_t)D.ms_off, D.hyp_off, (int32_t*)(hb + o_ms), (int*)(hb + o_hp));
     }
-    B200_CUDA(cudaMemcpyAsync(db, hb, in_bytes, cudaMemcpyHostToDevice, st));
+    B200_CUDA(A->upload(in_bytes, st));
     const ProblemDev* d_probs = (const ProblemDev*)(db + o_probs);
     const float* d_k1 = (const float*)(db + o_k1);
     const float* d_k2 = (const float*)(db + o_k2);
@@ -309,7 +311,7 @@ int b200_twoview_ransac(b200_lba_t h, int n_problems, b200_twoview_problem_t* pr
         (const HypDev*)(db + o_hyp), (const ScoreDev*)(db + o_sc), (int32_t*)(db + o_idx), (double*)(db + o_mat), db + o_fl,
         (ResultDev*)(db + o_res));
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpyAsync(hb + o_res, db + o_res, out_end - o_res, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(A->download(o_res, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
     const ResultDev* res = reinterpret_cast<const ResultDev*>(hb + o_res);
     for (int q = 0; q < n_problems; ++q) {
