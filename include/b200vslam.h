@@ -582,6 +582,49 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t matcher, b200_lba_t opt,
 int b200_track_stage_ms(b200_matcher_t matcher, int stage, float* ms);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Motion-model tracking on the device: module::frame_tracker::motion_based_track (module/frame_tracker.cc:20-59) with
+ * match::projection(0.9, true) for `n_frames` independent frames in ONE launch sequence, reading the extractor's results in HBM:
+ *   the predicted pose pose_cw = velocity * last_frm.get_pose_cw() (computed by the caller, :24); the frame starts with no landmarks
+ *   projection::match_current_and_last_frames (match/projection.cc:95-207): assume_forward / assume_backward from trans_lc (fp64,
+ *     reference order) against true_baseline (never for monocular setups), one query per entry of the last-frame table (reproject_to_image
+ *     of the camera model, octave window of the last keypoint, margin * scale_factors[last octave], 30-degree orientation gate, stereo
+ *     x_right gate, HAMMING_DIST_THR_HIGH)
+ *   when fewer than num_matches_thr matches: a second search at twice the margin on a frame without landmarks (:32-36); its result
+ *     replaces the first one.  Still short: the frame fails, its pose stays pose_cw and the matches of the last search are reported.
+ *   pose_optimizer::optimize (pose_optimizer_g2o.cc:38-175, the < 5 observations early return included) on the keypoints that carry a
+ *     landmark, then discard_outliers (:133-150): an outlier keypoint loses its landmark; tracked = n_valid >= num_matches_thr.
+ * prm: b200_track_params_t with margin = margin_last_frame_projection (20; 10 in the KITTI example), hamming_thr, max_candidates, the
+ * camera / bounds / grid / levels and the optimiser's trials; lowe_ratio, ray_cos_thr and log_scale_factor are not used.  The orientation
+ * check is always on (the reference constructs the matcher with it).  true_baseline = camera::base::true_baseline_.
+ * Errors as b200_track_local_map: B200_ERR_INVALID for bad parameters, an n_keypoints_in that disagrees with the extractor's count
+ * or a missing last_pose_cw in a non-monocular setup; B200_ERR_CAPACITY for a search-window overflow or an undersized kp_cap.
+ * One upload, one download and one stream synchronise per call; the retry decision and the choice of search stay on the device. */
+typedef struct b200_motion_track_frame {
+    int32_t frame;                     /* index into the extractor's last batch */
+    const double* pose_cw;             /* 16, row-major, predicted: velocity * last pose */
+    const double* last_pose_cw;        /* 16, last_frm pose after update_last_frame; may be NULL when monocular */
+    int32_t n_keypoints_in;            /* entries of kp_x_right (0 when NULL); must equal the frame's keypoint count */
+    const float* kp_x_right;           /* stereo_x_right_ of the current frame (b200_stereo_compute / b200_rgbd_depths), NULL = monocular */
+    int32_t n_landmarks;               /* last-frame table: keypoints with a landmark that is not will_be_erased, last-frame keypoint order */
+    const double* lm_pos_w;            /* 3 per entry */
+    const uint8_t* lm_desc;            /* 32 per entry: landmark::get_descriptor() */
+    const uint8_t* lm_octave;          /* last_frm undist_keypts_[idx].octave */
+    const float* lm_angle;             /* last_frm undist_keypts_[idx].angle */
+    const uint8_t* lm_has_observation; /* NULL = all have */
+    int32_t kp_cap;                    /* capacity of kp_landmark_out (>= the frame's keypoint count) */
+    int32_t* kp_landmark_out;          /* out, per keypoint: table row after discard_outliers, -1 none */
+    double pose_cw_out[16];            /* out */
+    int32_t n_keypoints, n_matches_first, n_matches, retried; /* out; n_matches = count of the search that decided */
+    uint32_t n_valid;                  /* out: discard_outliers' count */
+    int32_t tracked;                   /* out: motion_based_track's return value */
+} b200_motion_track_frame_t;
+int b200_motion_based_track(b200_orb_t orb, b200_matcher_t matcher, b200_lba_t opt, const b200_track_params_t* prm, double true_baseline,
+                            uint32_t num_matches_thr, int n_frames, b200_motion_track_frame_t* frames);
+/* Device time of the last b200_motion_based_track, per stage: 0 undistort + query build, 1 grid, 2 first search, 3 retry set-up + second
+ * search + choice, 4 edge build, 5 pose optimisation + scatter + discard, 6 whole chain (CUDA events on the stream). */
+int b200_motion_track_stage_ms(b200_matcher_t matcher, int stage, float* ms);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * New landmarks of the mapping module: module::two_view_triangulator (src/stella_vslam/module/two_view_triangulator.{h,cc}, with
  * solve::triangulator::triangulate, solve/triangulator.h:77-90, and data::triangulate_stereo, data/common.cc:192-260) and the
  * numeric chain of mapping_module::create_new_landmarks after the baseline test (mapping_module.cc, triangulate_with_two_keyframes).

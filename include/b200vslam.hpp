@@ -576,6 +576,33 @@ private:
     match::device_matcher m_;
     optimize::pose_optimizer opt_;
 };
+
+// module::frame_tracker::motion_based_track (module/frame_tracker.h, frame_tracker.cc:20-59) for a batch of frames that stay on the GPU
+// (b200_motion_based_track).  params.margin = margin_last_frame_projection; true_baseline = camera::base::true_baseline_.
+class frame_tracker {
+public:
+    frame_tracker(const feature::orb_extractor& extractor, const b200_track_params_t& params, double true_baseline, unsigned int num_matches_thr = 10,
+                  int device = 0)
+        : ex_(extractor), prm_(params), true_baseline_(true_baseline), num_matches_thr_(num_matches_thr), m_(device),
+          opt_(params.num_trials_robust, params.num_trials, params.num_each_iter, device) {}
+    void motion_based_track(std::vector<b200_motion_track_frame_t>& frames) {
+        check(b200_motion_based_track(ex_.handle(), m_.get(), opt_.handle(), &prm_, true_baseline_, num_matches_thr_, (int)frames.size(), frames.data()),
+              "b200_motion_based_track");
+    }
+    float stage_ms(int stage) const {
+        float ms = 0.f;
+        check(b200_motion_track_stage_ms(m_.get(), stage, &ms), "b200_motion_track_stage_ms");
+        return ms;
+    }
+
+private:
+    const feature::orb_extractor& ex_;
+    b200_track_params_t prm_;
+    double true_baseline_;
+    unsigned int num_matches_thr_;
+    match::device_matcher m_;
+    optimize::pose_optimizer opt_;
+};
 }  // namespace tracking
 
 namespace mapping {

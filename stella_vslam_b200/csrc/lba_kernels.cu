@@ -2476,7 +2476,7 @@ constexpr int kTrackEdgeThreads = 256;
 constexpr int kMatchedBias = 1 << 30;
 __global__ void __launch_bounds__(kTrackEdgeThreads) track_edges_kernel(chain::TrackShared sh, const chain::TrackFrameDev* __restrict__ frames,
                                                                         PoseProb* __restrict__ probs, PoseEdge* __restrict__ edges_all,
-                                                                        int* __restrict__ edge_kp_all) {
+                                                                        int* __restrict__ edge_kp_all, const int* __restrict__ gate) {
     __shared__ int warp_sum[kTrackEdgeThreads / 32];
     __shared__ int s_base;
     const chain::TrackFrameDev& F = frames[blockIdx.x];
@@ -2540,9 +2540,10 @@ __global__ void __launch_bounds__(kTrackEdgeThreads) track_edges_kernel(chain::T
         }
         __syncthreads();
     }
-    if (tid == 0) {
-        probs[blockIdx.x].n = s_base;
-        F.status[2] = s_base;
+    if (tid == 0) {  // a gated frame keeps its matches but gets no edge: pose_optimize_kernel returns before any iteration
+        const int n_edges = (!gate || gate[blockIdx.x]) ? s_base : 0;
+        probs[blockIdx.x].n = n_edges;
+        F.status[2] = n_edges;
     }
 }
 
@@ -2816,7 +2817,7 @@ namespace b200 {
 namespace chain {
 int track_stage_c(b200_lba_t opt, cudaStream_t st, const TrackShared& sh, const TrackFrameDev* d_frames, const TrackFrameDev* h_frames,
                   const double* const* pose_cw, int n_frames, int max_kp, int trials_robust, int trials, int each_iter, double* d_pose_out,
-                  unsigned* d_n_valid, cudaEvent_t ev_edges_done) {
+                  unsigned* d_n_valid, cudaEvent_t ev_edges_done, const int* d_gate) {
     using namespace b200::lba;
     if (!opt) return B200_ERR_INVALID;
     Solver& S = opt->s;
@@ -2847,7 +2848,7 @@ int track_stage_c(b200_lba_t opt, cudaStream_t st, const TrackShared& sh, const 
     unsigned char* d = S.arena.d;
     B200_CUDA(S.arena.upload(upload_bytes, st));
     PoseProb* dp = reinterpret_cast<PoseProb*>(d + o_probs);
-    track_edges_kernel<<<n_frames, kTrackEdgeThreads, 0, st>>>(sh, d_frames, dp, (PoseEdge*)(d + o_edges), (int*)(d + o_kp));
+    track_edges_kernel<<<n_frames, kTrackEdgeThreads, 0, st>>>(sh, d_frames, dp, (PoseEdge*)(d + o_edges), (int*)(d + o_kp), d_gate);
     if (ev_edges_done) B200_CUDA(cudaEventRecord(ev_edges_done, st));
     pose_optimize_kernel<<<n_frames, kPoseThreads, 0, st>>>(dp, (const PoseEdge*)(d + o_edges), d + o_level, d + o_flags, trials_robust, trials, each_iter,
                                                            d_pose_out, d_n_valid);

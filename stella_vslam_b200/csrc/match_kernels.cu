@@ -825,6 +825,69 @@ __global__ void track_set_counts_kernel(GuidedDev* __restrict__ gs, const chain:
     if (f < n) gs[f].n_train = frames[f].status[0];
 }
 
+// ---- b200_motion_based_track (frame_tracker.cc:20-59) --------------------------------------------------------------------------------
+// per-frame status words: [0] matches of the first search, [1] retried, [2] matches of the search that decided, [3] n_valid, [4] tracked
+constexpr int kMotionStat = 8;
+
+// One CTA per frame, after the first search: frame_tracker.cc:32-36 decides on the device whether the frame searches again.  The second
+// problem shares the grid, the query arrays and the candidate scratch of the first; it has its own occupancy (a frame without landmarks:
+// erase_landmarks), match_out and count.  (2 * margin) * scale_factors[l] = 2 * (margin * scale_factors[l]) exactly in float.
+__global__ void __launch_bounds__(128) motion_retry_kernel(const GuidedDev* __restrict__ g1, GuidedDev* __restrict__ g2,
+                                                           const chain::TrackFrameDev* __restrict__ frames, unsigned thr, int* __restrict__ stat) {
+    const int f = blockIdx.x;
+    const GuidedDev& a = g1[f];
+    const int n_first = *a.n_matches;
+    const bool retry = (unsigned)n_first < thr;
+    unsigned char* occ = g2[f].occupied;
+    if (threadIdx.x == 0) {
+        g2[f].n_train = a.n_train;
+        g2[f].n_queries = retry ? a.n_queries : 0;
+        stat[kMotionStat * f] = n_first;
+        stat[kMotionStat * f + 1] = retry ? 1 : 0;
+    }
+    if (!retry) return;
+    float* margin = frames[f].q_margin;
+    for (int q = threadIdx.x; q < a.n_queries; q += blockDim.x) margin[q] = __fmul_rn(2.f, margin[q]);
+    for (int i = threadIdx.x; i < a.n_train; i += blockDim.x) occ[i] = 0;
+}
+
+// after the second search: the result of the search that decided becomes the frame's match_out (the second replaces the first entirely)
+// and gate[f] = whether the pose optimisation runs (:38-41)
+__global__ void __launch_bounds__(128) motion_select_kernel(const GuidedDev* __restrict__ g1, const GuidedDev* __restrict__ g2, unsigned thr,
+                                                            int* __restrict__ stat, int* __restrict__ gate) {
+    const int f = blockIdx.y;
+    const bool retried = stat[kMotionStat * f + 1] != 0;
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q == 0) {
+        const int n = retried ? *g2[f].n_matches : *g1[f].n_matches;
+        stat[kMotionStat * f + 2] = n;
+        gate[f] = (unsigned)n >= thr ? 1 : 0;
+    }
+    if (retried && q < g1[f].n_queries) g1[f].match_out[q] = g2[f].match_out[q];
+}
+
+// discard_outliers (frame_tracker.cc:133-150) after stage C: an outlier keypoint loses its landmark; count the keypoints that keep one
+__global__ void __launch_bounds__(256) motion_discard_kernel(const chain::TrackFrameDev* __restrict__ frames, const int* __restrict__ gate, unsigned thr,
+                                                             int* __restrict__ stat) {
+    __shared__ int s_valid;
+    const chain::TrackFrameDev& F = frames[blockIdx.x];
+    if (threadIdx.x == 0) s_valid = 0;
+    __syncthreads();
+    const int n = F.status[0];
+    int valid = 0;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        if (F.kp_landmark_out[i] < 0) continue;
+        if (F.kp_outlier[i]) F.kp_landmark_out[i] = -1;
+        else ++valid;
+    }
+    if (valid) atomicAdd(&s_valid, valid);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        stat[kMotionStat * blockIdx.x + 3] = s_valid;
+        stat[kMotionStat * blockIdx.x + 4] = (gate[blockIdx.x] && (unsigned)s_valid >= thr) ? 1 : 0;
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // All-pairs matchers with greedy state other than brute_force_match:
 //   match::bow_tree::match_frame_and_keyframe   src/stella_vslam/match/bow_tree.cc:169-256   (variant 0)
@@ -1366,6 +1429,8 @@ struct Matcher {
     cudaEvent_t ev_t[3] = {nullptr, nullptr, nullptr};
     cudaEvent_t ev_track[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // b200_track_local_map stage boundaries
     bool track_timed = false;
+    cudaEvent_t ev_motion[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // b200_motion_based_track stage boundaries
+    bool motion_timed = false;
     int join() {  // the main stream waits for the side stream's resolve
         if (resolve_pending) {
             B200_CUDA(cudaStreamWaitEvent(stream, ev_resolved, 0));
@@ -1491,6 +1556,8 @@ int b200_matcher_destroy(b200_matcher_t h) {
         if (h->m.ev_t[i]) cudaEventDestroy(h->m.ev_t[i]);
     for (int i = 0; i < 7; ++i)
         if (h->m.ev_track[i]) cudaEventDestroy(h->m.ev_track[i]);
+    for (int i = 0; i < 7; ++i)
+        if (h->m.ev_motion[i]) cudaEventDestroy(h->m.ev_motion[i]);
     if (h->m.ev_topk) cudaEventDestroy(h->m.ev_topk);
     if (h->m.ev_resolved) cudaEventDestroy(h->m.ev_resolved);
     if (h->m.side_stream) cudaStreamDestroy(h->m.side_stream);
@@ -2105,6 +2172,321 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const
         F.n_matches = *reinterpret_cast<const int*>(hb + L.nm);
         F.n_valid = reinterpret_cast<const unsigned*>(hb + o_nvalid)[f];
         if (status[2] < 5) std::memcpy(F.pose_cw_out, F.pose_cw, sizeof(double) * 16);  // :116-118: returns before touching the pose
+        else std::memcpy(F.pose_cw_out, hb + o_pose + sizeof(double) * 16 * (size_t)f, sizeof(double) * 16);
+    }
+    return B200_OK;
+}
+
+int b200_motion_track_stage_ms(b200_matcher_t h, int stage, float* ms) {
+    if (!h || !ms || stage < 0 || stage > 6 || !h->m.motion_timed) return B200_ERR_INVALID;
+    if (stage == 6) B200_CUDA(cudaEventElapsedTime(ms, h->m.ev_motion[0], h->m.ev_motion[6]));
+    else B200_CUDA(cudaEventElapsedTime(ms, h->m.ev_motion[stage], h->m.ev_motion[stage + 1]));
+    return B200_OK;
+}
+
+// Motion-model tracking on the device (see include/b200vslam.h).  Arena of the matcher handle, as for b200_track_local_map:
+//   [TrackFrameDev x n][GuidedDev x n][GuidedDev x n (second search)][caller inputs]  -- mirrored in pinned memory, one upload
+//   [outputs]                                                                        -- one download
+//   [stage-A products, guided scratch, second-search buffers]
+int b200_motion_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const b200_track_params_t* prm, double true_baseline,
+                            uint32_t num_matches_thr, int n_frames, b200_motion_track_frame_t* frames) {
+    B200_RANGE("b200:track:motion");
+    using b200::chain::TrackFrameDev;
+    using b200::chain::TrackShared;
+    using b200::match::GuidedDev;
+    using b200::match::kMotionStat;
+    if (!orb || !h || !opt || !prm || n_frames < 0) return B200_ERR_INVALID;
+    if (n_frames == 0) return B200_OK;
+    if (!frames || !prm->scale_factors || !prm->inv_level_sigma_sq || prm->num_levels == 0 || prm->num_levels > 32 || prm->grid_cols <= 0
+        || prm->grid_rows <= 0 || (long long)prm->grid_cols * prm->grid_rows > (1 << 20) || !(prm->img_bounds[1] > prm->img_bounds[0])
+        || !(prm->img_bounds[3] > prm->img_bounds[2]) || !b200::chain::camera_valid(prm->cam) || prm->max_candidates < 0
+        || prm->num_trials_robust < 0 || prm->num_trials < 0 || prm->num_each_iter < 0 || std::isnan(true_baseline)) {
+        b200::set_error("b200_motion_based_track: invalid parameters");
+        return B200_ERR_INVALID;
+    }
+    auto& m = h->m;
+    const b200_keypoint_t* d_kps = nullptr;
+    const unsigned char* d_descs = nullptr;
+    const int* d_counts = nullptr;
+    int stride = 0, batch = 0, device = 0;
+    cudaStream_t st = nullptr;
+    int rc = b200::chain::orb_results(orb, &d_kps, &d_descs, &d_counts, &stride, &batch, &st, &device);
+    if (rc) return rc;
+    if (device != m.device) {
+        b200::set_error("b200_motion_based_track: extractor and matcher live on different devices");
+        return B200_ERR_INVALID;
+    }
+    B200_CUDA(cudaSetDevice(m.device));
+    const int cap = prm->max_candidates ? prm->max_candidates : 256;
+    struct Lay {
+        size_t xr, pos, desc, oct, ang, hobs;                                  // inputs
+        size_t klo, status, mout, nm;                                          // outputs
+        size_t und, tx, ty, tang, toct, occ, kout, qx, qy, qm, qxr, qlo, qhi, qval;  // stage A products
+        size_t cstart, citems, ccur, lists, llen, own;                         // guided scratch
+        size_t occ2, mout2, nm2;                                               // second search
+    };
+    std::vector<Lay> lay(n_frames);
+    int max_lm = 0;
+    b200::Layout a;
+    a.take<TrackFrameDev>(n_frames);  // at offset 0
+    const size_t o_gd = a.take<GuidedDev>(n_frames), o_gd2 = a.take<GuidedDev>(n_frames);
+    for (int f = 0; f < n_frames; ++f) {
+        const b200_motion_track_frame_t& F = frames[f];
+        if (F.frame < 0 || F.frame >= batch || !F.pose_cw || (!prm->monocular && !F.last_pose_cw) || F.n_landmarks < 0 || F.n_keypoints_in < 0
+            || F.kp_cap < 0 || (F.kp_x_right && F.n_keypoints_in > stride) || !F.kp_landmark_out
+            || (F.n_landmarks > 0 && (!F.lm_pos_w || !F.lm_desc || !F.lm_octave || !F.lm_angle))) {
+            b200::set_error("b200_motion_based_track: frame %d: bad frame index, sizes, null buffers or no last pose", f);
+            return B200_ERR_INVALID;
+        }
+        for (int l = 0; l < F.n_landmarks; ++l)
+            if (F.lm_octave[l] >= prm->num_levels) {  // scale_factors_.at(last_scale_level) (projection.cc:159)
+                b200::set_error("b200_motion_based_track: frame %d: octave %d of entry %d is not below num_levels", f, (int)F.lm_octave[l], l);
+                return B200_ERR_INVALID;
+            }
+        Lay& L = lay[f];
+        const size_t nk = (size_t)F.n_keypoints_in, nl = (size_t)F.n_landmarks;
+        L.xr = a.take(4 * nk);
+        L.pos = a.take(24 * nl);
+        L.desc = a.take(32 * nl);
+        L.oct = a.take(nl);
+        L.ang = a.take(4 * nl);
+        L.hobs = a.take(nl);
+        max_lm = std::max(max_lm, F.n_landmarks);
+    }
+    const size_t in_bytes = a.end, out_begin = a.end;
+    const size_t kc = (size_t)std::max(stride, 1);
+    for (int f = 0; f < n_frames; ++f) {
+        Lay& L = lay[f];
+        const size_t nl = (size_t)frames[f].n_landmarks;
+        L.klo = a.take(4 * kc);
+        L.status = a.take(16);
+        L.mout = a.take(4 * nl);
+        L.nm = a.take(4);
+    }
+    const size_t o_pose = a.take(8 * 16 * (size_t)n_frames);
+    const size_t o_nvalid = a.take(4 * (size_t)n_frames);
+    const size_t o_stat = a.take(4 * kMotionStat * (size_t)n_frames);
+    const size_t o_gate = a.take(4 * (size_t)n_frames);
+    const size_t o_overflow = a.take(4);
+    const size_t out_end = a.end;
+    const size_t cells = (size_t)prm->grid_cols * prm->grid_rows;
+    for (int f = 0; f < n_frames; ++f) {
+        Lay& L = lay[f];
+        const size_t nl = (size_t)frames[f].n_landmarks;
+        L.und = a.take(sizeof(b200_keypoint_t) * kc);
+        L.tx = a.take(4 * kc);
+        L.ty = a.take(4 * kc);
+        L.tang = a.take(4 * kc);
+        L.toct = a.take(kc);
+        L.occ = a.take(kc);
+        L.kout = a.take(kc);
+        L.qx = a.take(4 * nl);
+        L.qy = a.take(4 * nl);
+        L.qm = a.take(4 * nl);
+        L.qxr = a.take(4 * nl);
+        L.qlo = a.take(nl);
+        L.qhi = a.take(nl);
+        L.qval = a.take(nl);
+        L.cstart = a.take(4 * (cells + 1));
+        L.citems = a.take(4 * kc);
+        L.ccur = a.take(4 * cells);
+        L.lists = a.take(8 * (size_t)cap * nl);
+        L.llen = a.take(4 * nl);
+        L.own = a.take(4 * kc);
+        L.occ2 = a.take(kc);
+        L.mout2 = a.take(4 * nl);
+        L.nm2 = a.take(4);
+    }
+    const size_t rs_bytes = kc * 6 + 16;
+    if (rs_bytes > 200 * 1024) {
+        b200::set_error("b200_motion_based_track: %d keypoints per frame exceed the on-chip occupancy table", stride);
+        return B200_ERR_CAPACITY;
+    }
+    if ((rc = m.arena.reserve(a.end, out_end, m.stream))) return rc;
+    for (int i = 0; i < 7; ++i)
+        if (!m.ev_motion[i]) B200_CUDA(cudaEventCreate(&m.ev_motion[i]));
+    b200::StagingArena& A = m.arena;
+    unsigned char *hb = A.h, *db = A.d;
+    TrackFrameDev* hf = A.host<TrackFrameDev>(0);
+    GuidedDev* hg = A.host<GuidedDev>(o_gd);
+    GuidedDev* hg2 = A.host<GuidedDev>(o_gd2);
+    TrackShared sh{};
+    sh.model = prm->cam.model;
+    sh.fx = prm->cam.fx; sh.fy = prm->cam.fy; sh.cx = prm->cam.cx; sh.cy = prm->cam.cy;
+    sh.k1 = prm->cam.k1; sh.k2 = prm->cam.k2; sh.p1 = prm->cam.p1; sh.p2 = prm->cam.p2; sh.k3 = prm->cam.k3;
+    sh.k4 = prm->cam.k4; sh.distortion = prm->cam.distortion;
+    sh.cols = prm->cam.cols; sh.rows = prm->cam.rows;
+    sh.fxb = prm->focal_x_baseline;
+    sh.min_x = prm->img_bounds[0]; sh.max_x = prm->img_bounds[1]; sh.min_y = prm->img_bounds[2]; sh.max_y = prm->img_bounds[3];
+    sh.margin = prm->margin;
+    sh.delta = prm->monocular ? std::sqrt(5.99146f) : std::sqrt(7.81473f);  // pose_optimizer_g2o.cc:73-88
+    sh.num_levels = prm->num_levels;
+    for (unsigned l = 0; l < 32; ++l) {
+        sh.scale_factors[l] = prm->scale_factors[std::min(l, prm->num_levels - 1)];
+        sh.inv_level_sigma_sq[l] = prm->inv_level_sigma_sq[std::min(l, prm->num_levels - 1)];
+    }
+    sh.monocular = prm->monocular ? 1 : 0;
+    sh.true_baseline = true_baseline;
+    std::vector<const double*> poses(n_frames);
+    for (int f = 0; f < n_frames; ++f) {
+        const b200_motion_track_frame_t& F = frames[f];
+        const Lay& L = lay[f];
+        const size_t nk = (size_t)F.n_keypoints_in, nl = (size_t)F.n_landmarks;
+        A.put(L.xr, F.kp_x_right, 4 * nk);
+        A.put(L.pos, F.lm_pos_w, 24 * nl);
+        A.put(L.desc, F.lm_desc, 32 * nl);
+        A.put(L.oct, F.lm_octave, nl);
+        A.put(L.ang, F.lm_angle, 4 * nl);
+        A.put(L.hobs, F.lm_has_observation, nl);
+        poses[f] = F.pose_cw;
+        TrackFrameDev t{};
+        t.kps = d_kps + (size_t)F.frame * stride;
+        t.n_kp = d_counts + F.frame;
+        t.kp_cap = stride;
+        t.n_kp_in = F.n_keypoints_in;
+        t.n_lm = F.n_landmarks;
+        t.kp_x_right = F.kp_x_right ? (const float*)(db + L.xr) : nullptr;
+        t.kp_landmark = nullptr;  // frame_tracker.cc:27: the frame starts without landmarks
+        t.pos_w = (const double*)(db + L.pos);
+        t.lm_has_obs = F.lm_has_observation ? db + L.hobs : nullptr;
+        t.lm_octave = db + L.oct;
+        const double* P = F.pose_cw;
+        for (int r = 0; r < 3; ++r) {
+            for (int c = 0; c < 3; ++c) t.Rt[3 * r + c] = P[4 * r + c];
+            t.Rt[9 + r] = P[4 * r + 3];
+        }
+        for (int r = 0; r < 3; ++r) t.twc[r] = -(t.Rt[r] * t.Rt[9] + t.Rt[3 + r] * t.Rt[10] + t.Rt[6 + r] * t.Rt[11]);
+        if (F.last_pose_cw) {
+            const double* Q = F.last_pose_cw;
+            for (int r = 0; r < 3; ++r) {
+                for (int c = 0; c < 3; ++c) t.last_Rt[3 * r + c] = Q[4 * r + c];
+                t.last_Rt[9 + r] = Q[4 * r + 3];
+            }
+        }
+        t.undist = (b200_keypoint_t*)(db + L.und);
+        t.t_x = (float*)(db + L.tx);
+        t.t_y = (float*)(db + L.ty);
+        t.t_angle = (float*)(db + L.tang);
+        t.t_octave = db + L.toct;
+        t.occupied = db + L.occ;
+        t.q_x = (float*)(db + L.qx);
+        t.q_y = (float*)(db + L.qy);
+        t.q_margin = (float*)(db + L.qm);
+        t.q_xr = (float*)(db + L.qxr);
+        t.q_lo = (signed char*)(db + L.qlo);
+        t.q_hi = (signed char*)(db + L.qhi);
+        t.q_valid = db + L.qval;
+        t.match_out = (const int*)(db + L.mout);
+        t.kp_landmark_out = (int*)(db + L.klo);
+        t.kp_outlier = db + L.kout;
+        t.status = (int*)(db + L.status);
+        hf[f] = t;
+        GuidedDev g{};
+        g.n_train = 0;  // set on the device from the extractor's counter
+        g.n_queries = F.n_landmarks;
+        g.grid_cols = prm->grid_cols;
+        g.grid_rows = prm->grid_rows;
+        g.cap = cap;
+        g.min_x = sh.min_x; g.max_x = sh.max_x; g.min_y = sh.min_y; g.max_y = sh.max_y;
+        g.t_x = t.t_x;
+        g.t_y = t.t_y;
+        g.t_angle = t.t_angle;
+        g.t_x_right = t.kp_x_right;
+        g.t_octave = t.t_octave;
+        g.t_desc = reinterpret_cast<const uint4*>(d_descs + (size_t)F.frame * stride * 32);
+        g.q_desc = (const uint4*)(db + L.desc);
+        g.q_x = t.q_x;
+        g.q_y = t.q_y;
+        g.q_margin = t.q_margin;
+        g.q_x_right = t.q_xr;
+        g.q_angle = (const float*)(db + L.ang);
+        g.q_min_level = t.q_lo;
+        g.q_max_level = t.q_hi;
+        g.q_valid = t.q_valid;
+        g.q_reproj = nullptr;
+        g.inv_level_sigma_sq = nullptr;
+        g.do_reproj = 0;
+        g.owner = (int*)(db + L.own);
+        g.cell_start = (int*)(db + L.cstart);
+        g.cell_items = (int*)(db + L.citems);
+        g.cell_cursor = (int*)(db + L.ccur);
+        g.lists = (uint2*)(db + L.lists);
+        g.list_len = (int*)(db + L.llen);
+        g.occupied = t.occupied;
+        g.match_out = (int*)(db + L.mout);
+        g.n_matches = (int*)(db + L.nm);
+        hg[f] = g;
+        g.n_queries = 0;  // both counts are set by motion_retry_kernel
+        g.occupied = db + L.occ2;
+        g.match_out = (int*)(db + L.mout2);
+        g.n_matches = (int*)(db + L.nm2);
+        hg2[f] = g;
+    }
+    if ((rc = m.join())) return rc;
+    B200_CUDA(cudaEventRecord(m.ev_motion[0], st));
+    B200_CUDA(A.upload(in_bytes, st));
+    B200_CUDA(cudaMemsetAsync(db + out_begin, 0, out_end - out_begin, st));
+    const TrackFrameDev* df = A.dev<const TrackFrameDev>(0);
+    GuidedDev* dg = A.dev<GuidedDev>(o_gd);
+    GuidedDev* dg2 = A.dev<GuidedDev>(o_gd2);
+    int* d_stat = (int*)(db + o_stat);
+    int* d_gate = (int*)(db + o_gate);
+    const unsigned thr = num_matches_thr;
+    const dim3 q_grid(std::max(1, b200::ceil_div(max_lm, 128)), n_frames);
+    const float lowe = 0.9f;  // projection(0.9, true): mode 1 has no ratio test
+    if ((rc = b200::chain::motion_stage_a(st, sh, df, n_frames, stride, max_lm))) return rc;
+    b200::match::track_set_counts_kernel<<<b200::ceil_div(n_frames, 128), 128, 0, st>>>(dg, df, n_frames);
+    B200_CUDA(cudaEventRecord(m.ev_motion[1], st));
+    b200::match::guided_grid_kernel<<<n_frames, 1024, 0, st>>>(dg);
+    B200_CUDA(cudaEventRecord(m.ev_motion[2], st));
+    if (rs_bytes > 48 * 1024)
+        B200_CUDA(cudaFuncSetAttribute(b200::match::guided_resolve_kernel<GuidedDev>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rs_bytes));
+    b200::match::guided_candidates_kernel<<<q_grid, 128, 0, st>>>(dg, B200_GUIDED_LAST_FRAME, 1, (int*)(db + o_overflow));
+    b200::match::guided_resolve_kernel<GuidedDev><<<n_frames, 32, rs_bytes, st>>>(dg, B200_GUIDED_LAST_FRAME, prm->hamming_thr, lowe);
+    B200_CUDA(cudaEventRecord(m.ev_motion[3], st));
+    b200::match::motion_retry_kernel<<<n_frames, 128, 0, st>>>(dg, dg2, df, thr, d_stat);
+    b200::match::guided_candidates_kernel<<<q_grid, 128, 0, st>>>(dg2, B200_GUIDED_LAST_FRAME, 1, (int*)(db + o_overflow));
+    b200::match::guided_resolve_kernel<GuidedDev><<<n_frames, 32, rs_bytes, st>>>(dg2, B200_GUIDED_LAST_FRAME, prm->hamming_thr, lowe);
+    b200::match::motion_select_kernel<<<q_grid, 128, 0, st>>>(dg, dg2, thr, d_stat, d_gate);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaEventRecord(m.ev_motion[4], st));
+    if ((rc = b200::chain::track_stage_c(opt, st, sh, df, hf, poses.data(), n_frames, stride, prm->num_trials_robust, prm->num_trials, prm->num_each_iter,
+                                         (double*)(db + o_pose), (unsigned*)(db + o_nvalid), m.ev_motion[5], d_gate)))
+        return rc;
+    b200::match::motion_discard_kernel<<<n_frames, 256, 0, st>>>(df, d_gate, thr, d_stat);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaEventRecord(m.ev_motion[6], st));
+    B200_CUDA(A.download(out_begin, out_end, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    m.motion_timed = true;
+    const int overflow = *reinterpret_cast<const int*>(hb + o_overflow);
+    if (overflow > 0) {
+        b200::set_error("b200_motion_based_track: a search window returned %d keypoints, max_candidates is %d", overflow, cap);
+        return B200_ERR_CAPACITY;
+    }
+    for (int f = 0; f < n_frames; ++f) {
+        b200_motion_track_frame_t& F = frames[f];
+        const Lay& L = lay[f];
+        const int* status = reinterpret_cast<const int*>(hb + L.status);
+        const int nk = status[0];
+        if (status[1]) {
+            b200::set_error("b200_motion_based_track: frame %d has %d keypoints, the caller's per-keypoint arrays have %d", f, nk, F.n_keypoints_in);
+            return B200_ERR_INVALID;
+        }
+        if (nk > F.kp_cap) {
+            b200::set_error("b200_motion_based_track: frame %d has %d keypoints, kp_cap is %d", f, nk, F.kp_cap);
+            return B200_ERR_CAPACITY;
+        }
+        const int* ms = reinterpret_cast<const int*>(hb + o_stat) + kMotionStat * (size_t)f;
+        F.n_keypoints = nk;
+        std::memcpy(F.kp_landmark_out, hb + L.klo, 4 * (size_t)nk);
+        F.n_matches_first = ms[0];
+        F.retried = ms[1];
+        F.n_matches = ms[2];
+        F.n_valid = (uint32_t)ms[3];
+        F.tracked = ms[4];
+        // a failed frame or fewer than 5 edges (pose_optimizer_g2o.cc:116-118): the predicted pose stays
+        if (status[2] < 5) std::memcpy(F.pose_cw_out, F.pose_cw, sizeof(double) * 16);
         else std::memcpy(F.pose_cw_out, hb + o_pose + sizeof(double) * 16 * (size_t)f, sizeof(double) * 16);
     }
     return B200_OK;

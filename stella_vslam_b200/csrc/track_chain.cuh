@@ -1,6 +1,7 @@
-// track_chain.cuh -- internal interfaces of b200_track_local_map (include/b200vslam.h): the chain is driven from match_kernels.cu,
-// stage A (undistort + can_observe + query build) lives in orb_kernels.cu (same device functions and -fmad=false as the stage-by-stage
-// ABI), stage C (edge build + pose optimisation) in lba_kernels.cu.  Plain device pointers, no handles' internals cross a TU.
+// track_chain.cuh -- internal interfaces of b200_track_local_map and b200_motion_based_track (include/b200vslam.h): both chains are
+// driven from match_kernels.cu, stage A (undistort + can_observe or the last-frame reprojection + query build) lives in orb_kernels.cu
+// (same device functions and -fmad=false as the stage-by-stage ABI), stage C (edge build + pose optimisation) in lba_kernels.cu.  Plain
+// device pointers, no handles' internals cross a TU.
 #pragma once
 
 #include <cmath>
@@ -27,6 +28,9 @@ struct TrackShared {  // by-value kernel parameter
     float ray_cos_thr, log_scale_factor, margin, delta;
     unsigned num_levels;
     float scale_factors[32], inv_level_sigma_sq[32];
+    // b200_motion_based_track: projection.cc:108-116
+    int monocular;
+    double true_baseline;
 };
 
 struct TrackFrameDev {  // one frame; every pointer is a device pointer
@@ -55,18 +59,25 @@ struct TrackFrameDev {  // one frame; every pointer is a device pointer
     // stage C
     int* kp_landmark_out;
     unsigned char* kp_outlier;
-    int* status;  // [0] keypoint count, [1] != 0: n_kp_in disagrees with the extractor's count
+    int* status;  // [0] keypoint count, [1] != 0: n_kp_in disagrees with the extractor's count, [2] edges of stage C
+    // b200_motion_based_track only (null / unused in the local-map chain)
+    float* t_angle;                   // stage A: angle of every keypoint, for the orientation gate
+    const unsigned char* lm_octave;   // last-frame table: octave of the last frame's keypoint
+    double last_Rt[12];               // last frame: rot_cw row-major, then trans_cw
 };
 
 // orb_kernels.cu: device views of the extractor's last batch + the stream its work is ordered on
 int orb_results(b200_orb_t orb, const b200_keypoint_t** d_kps, const unsigned char** d_descs, const int** d_counts, int* stride, int* batch,
                 cudaStream_t* stream, int* device);
 int track_stage_a(cudaStream_t st, const TrackShared& sh, const TrackFrameDev* d_frames, int n_frames, int max_kp, int max_lm);
+// the same keypoint kernel (with t_angle), then one query per last-frame table entry (projection.cc:95-160)
+int motion_stage_a(cudaStream_t st, const TrackShared& sh, const TrackFrameDev* d_frames, int n_frames, int max_kp, int max_lm);
 // lba_kernels.cu: builds one edge per keypoint that carries a landmark (keypoint order), runs pose_optimizer::optimize for every frame and
 // scatters the flags back to keypoint indexing.  h_frames = the host copy of d_frames; pose_out / n_valid are device pointers.
+// d_gate: null, or per frame 0 = apply the matches but build no edge (the pose stays, no flag is set).
 int track_stage_c(b200_lba_t opt, cudaStream_t st, const TrackShared& sh, const TrackFrameDev* d_frames, const TrackFrameDev* h_frames,
                   const double* const* pose_cw, int n_frames, int max_kp, int trials_robust, int trials, int each_iter, double* d_pose_out,
-                  unsigned* d_n_valid, cudaEvent_t ev_edges_done);
+                  unsigned* d_n_valid, cudaEvent_t ev_edges_done, const int* d_gate = nullptr);
 
 }  // namespace chain
 }  // namespace b200

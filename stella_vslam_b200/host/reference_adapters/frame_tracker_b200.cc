@@ -1,0 +1,145 @@
+// module::frame_tracker::motion_based_track (module/frame_tracker.cc:20-59) as one device call: the last frame's landmarks are projected
+// into curr_frm, matched (a second time at twice the margin when short), the pose optimised and the outliers discarded by
+// b200_motion_based_track -- the frame's keypoints and descriptors are read where the GPU extractor left them, only the last-frame table
+// goes up and the landmark slots / pose come back.
+//
+// Call site (tracking_module::track_current_frame, tracking_module.cc:333-355, USE_B200):
+//     succeeded = frame_tracker_.motion_based_track(curr_frm_, last_frm_, twist_);
+//         -> succeeded = motion_based_track_b200(curr_frm_, last_frm_, twist_, extractor_left_, margin_last_frame_projection_,
+//                                                num_matches_thr);
+// The landmarks curr_frm now carries are the ones track_local_map_b200 (track_local_map_b200.cc) then finds in its kp_landmark table:
+// they are skipped by the local-map search and become edges of its pose optimisation, as in the reference.
+// Precondition: `extractor` is the (left) feature::orb_extractor whose LAST extract() produced curr_frm (true in system.cc:380-395:
+// one extract per frame, frame constructed from its outputs), so frame 0 of its last batch is this frame.
+#include "stella_vslam/camera/base.h"
+#include "stella_vslam/camera/fisheye.h"
+#include "stella_vslam/camera/perspective.h"
+#include "stella_vslam/camera/radial_division.h"
+#include "stella_vslam/data/frame.h"
+#include "stella_vslam/data/landmark.h"
+#include "stella_vslam/feature/orb_extractor.h"
+#include "stella_vslam/feature/orb_params.h"
+
+#include <cstring>
+#include <stdexcept>
+
+#include "b200vslam.h"
+
+namespace stella_vslam {
+namespace feature {
+b200_orb_t b200_handle_of(const orb_extractor* self);  // orb_extractor_b200.cc
+}
+
+// Returns what frame_tracker::motion_based_track returns.  curr_frm leaves with the predicted pose velocity * last pose and the matches
+// of the last search when tracking failed before the pose optimisation, else with the optimised pose and the inlier landmarks.
+bool motion_based_track_b200(data::frame& curr_frm, const data::frame& last_frm, const Mat44_t& velocity, const feature::orb_extractor* extractor,
+                             float margin, unsigned int num_matches_thr) {
+    const b200_orb_t orb = feature::b200_handle_of(extractor);
+    if (!orb) throw std::runtime_error("motion_based_track_b200: the extractor has not extracted a frame yet");
+    static thread_local b200_matcher_t matcher = nullptr;
+    static thread_local b200_lba_t opt = nullptr;
+    if (!matcher && b200_matcher_create(0, &matcher) != B200_OK) throw std::runtime_error(b200_last_error());
+    if (!opt && b200_lba_create(0, &opt) != B200_OK) throw std::runtime_error(b200_last_error());
+
+    // ---- the last-frame table: keypoints of last_frm with a landmark that is not will_be_erased, in keypoint order (projection.cc:120-128)
+    const auto& last_kps = last_frm.frm_obs_.undist_keypts_;
+    std::vector<std::shared_ptr<data::landmark>> table;
+    std::vector<double> pos;
+    std::vector<uint8_t> desc, octave, has_obs;
+    std::vector<float> angle;
+    for (unsigned int idx = 0; idx < last_kps.size(); ++idx) {
+        const auto& lm = last_frm.get_landmark(idx);
+        if (!lm || lm->will_be_erased()) continue;
+        const Vec3_t p = lm->get_pos_in_world();
+        pos.insert(pos.end(), {p(0), p(1), p(2)});
+        const cv::Mat d = lm->get_descriptor();
+        desc.insert(desc.end(), d.ptr<uint8_t>(), d.ptr<uint8_t>() + 32);
+        octave.push_back(static_cast<uint8_t>(last_kps[idx].octave));
+        angle.push_back(last_kps[idx].angle);
+        has_obs.push_back(lm->has_observation() ? 1 : 0);
+        table.push_back(lm);
+    }
+
+    b200_track_params_t prm{};
+    const auto* cam = curr_frm.camera_;
+    switch (cam->model_type_) {  // model codes of b200_camera_intrinsics_t, as in track_local_map_b200.cc
+        case camera::model_type_t::Perspective: {
+            const auto* p = static_cast<const camera::perspective*>(cam);
+            prm.cam.model = 0;
+            prm.cam.fx = p->fx_; prm.cam.fy = p->fy_; prm.cam.cx = p->cx_; prm.cam.cy = p->cy_;
+            prm.cam.k1 = p->k1_; prm.cam.k2 = p->k2_; prm.cam.p1 = p->p1_; prm.cam.p2 = p->p2_; prm.cam.k3 = p->k3_;
+            break;
+        }
+        case camera::model_type_t::Fisheye: {
+            const auto* p = static_cast<const camera::fisheye*>(cam);
+            prm.cam.model = 2;
+            prm.cam.fx = p->fx_; prm.cam.fy = p->fy_; prm.cam.cx = p->cx_; prm.cam.cy = p->cy_;
+            prm.cam.k1 = p->k1_; prm.cam.k2 = p->k2_; prm.cam.k3 = p->k3_; prm.cam.k4 = p->k4_;
+            break;
+        }
+        case camera::model_type_t::RadialDivision: {
+            const auto* p = static_cast<const camera::radial_division*>(cam);
+            prm.cam.model = 3;
+            prm.cam.fx = p->fx_; prm.cam.fy = p->fy_; prm.cam.cx = p->cx_; prm.cam.cy = p->cy_;
+            prm.cam.distortion = p->distortion_;
+            break;
+        }
+        default:
+            prm.cam.model = 1;  // equirectangular
+            break;
+    }
+    prm.cam.cols = cam->cols_;
+    prm.cam.rows = cam->rows_;
+    prm.focal_x_baseline = cam->focal_x_baseline_;
+    prm.monocular = cam->setup_type_ == camera::setup_type_t::Monocular ? 1 : 0;
+    prm.img_bounds[0] = cam->img_bounds_.min_x_; prm.img_bounds[1] = cam->img_bounds_.max_x_;
+    prm.img_bounds[2] = cam->img_bounds_.min_y_; prm.img_bounds[3] = cam->img_bounds_.max_y_;
+    prm.grid_cols = static_cast<int32_t>(curr_frm.frm_obs_.num_grid_cols_);
+    prm.grid_rows = static_cast<int32_t>(curr_frm.frm_obs_.num_grid_rows_);
+    const auto* op = curr_frm.orb_params_;
+    prm.num_levels = op->num_levels_;
+    prm.log_scale_factor = op->log_scale_factor_;
+    prm.scale_factors = op->scale_factors_.data();
+    prm.inv_level_sigma_sq = op->inv_level_sigma_sq_.data();
+    prm.margin = margin;       // margin_last_frame_projection
+    prm.lowe_ratio = 0.9f;     // match::projection projection_matcher(0.9, true) (:21); mode 1 has no ratio test
+    prm.hamming_thr = 100;     // HAMMING_DIST_THR_HIGH
+    prm.num_trials_robust = 2; prm.num_trials = 2; prm.num_each_iter = 10;  // pose_optimizer_factory.h:18-47
+
+    const Mat44_t pose_cw = velocity * last_frm.get_pose_cw();  // :24
+    const Mat44_t last_pose_cw = last_frm.get_pose_cw();
+    double pose[16], last_pose[16];
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) {
+            pose[4 * r + c] = pose_cw(r, c);
+            last_pose[4 * r + c] = last_pose_cw(r, c);
+        }
+    const unsigned int num_keypts = curr_frm.frm_obs_.undist_keypts_.size();
+    std::vector<int32_t> kp_landmark_out(num_keypts + 1, -1);
+    b200_motion_track_frame_t f{};
+    f.frame = 0;
+    f.pose_cw = pose;
+    f.last_pose_cw = last_pose;
+    const bool stereo = !curr_frm.frm_obs_.stereo_x_right_.empty();
+    f.n_keypoints_in = stereo ? static_cast<int32_t>(num_keypts) : 0;
+    f.kp_x_right = stereo ? curr_frm.frm_obs_.stereo_x_right_.data() : nullptr;
+    f.n_landmarks = static_cast<int32_t>(table.size());
+    f.lm_pos_w = pos.data(); f.lm_desc = desc.data(); f.lm_octave = octave.data(); f.lm_angle = angle.data(); f.lm_has_observation = has_obs.data();
+    f.kp_cap = static_cast<int32_t>(num_keypts);
+    f.kp_landmark_out = kp_landmark_out.data();
+    if (b200_motion_based_track(orb, matcher, opt, &prm, cam->true_baseline_, num_matches_thr, 1, &f) != B200_OK)
+        throw std::runtime_error(b200_last_error());
+    if (static_cast<unsigned int>(f.n_keypoints) != num_keypts) throw std::runtime_error("motion_based_track_b200: the extractor's last frame is not curr_frm");
+
+    // ---- write-back: the frame starts without landmarks (:27) and carries what survived the search and discard_outliers
+    curr_frm.erase_landmarks();
+    for (unsigned int idx = 0; idx < num_keypts; ++idx)
+        if (kp_landmark_out[idx] >= 0) curr_frm.add_landmark(table[kp_landmark_out[idx]], idx);
+    Mat44_t out;
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) out(r, c) = f.pose_cw_out[4 * r + c];
+    curr_frm.set_pose_cw(out);
+    return f.tracked != 0;
+}
+
+}  // namespace stella_vslam

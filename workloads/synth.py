@@ -569,6 +569,80 @@ def make_tracking_frame(kps, desc, camera, scale_factors, seed=0, stereo=False, 
                                has_observation=has_obs))
 
 
+
+def make_motion_frame(kps, desc, camera, scale_factors, seed=0, stereo=False, motion="forward", true_baseline=None, landmark_frac=0.7,
+                      clutter_frac=0.2, rotated_frac=0.05, no_obs_frac=0.05, pixel_sigma=0.7, shift_px=0.0, rot_deg=0.2, trans_m=0.02, max_flips=25):
+    """The last-frame table of frame_tracker::motion_based_track for one extracted frame (keypoints taken as undistorted).  Most keypoints
+    get an entry whose landmark lies at a random depth along the keypoint's ray under a true pose (descriptor = the keypoint's with a few
+    flipped bits, octave = the keypoint's, angle within a few degrees of it), plus `rotated_frac` entries turned 40-180 degrees (rejected by
+    the 30-degree orientation gate), clutter entries (random descriptors and positions) and `no_obs_frac` entries without observations,
+    in a shuffled (last-frame keypoint) order.  The predicted pose is the true pose turned about the camera's y axis so that reprojections
+    move by about `shift_px` pixels (between margin and 2 * margin: the first search falls short and the second succeeds; beyond 2 * margin
+    both fail), then perturbed by rot_deg / trans_m.  The last pose sees the current camera centre moved by twice true_baseline along its
+    optical axis ("forward"), against it ("backward") or sideways.  Perspective-family and equirectangular cameras."""
+    rng = np.random.default_rng(seed)
+    n_kp = len(kps)
+    sf = np.asarray(scale_factors, np.float64)
+    equirect = camera.get("model", "perspective") == "equirectangular"
+    fx, fy, cx, cy = camera.get("fx", 1.0), camera.get("fy", 1.0), camera.get("cx", 0.0), camera.get("cy", 0.0)
+    if true_baseline is None:
+        true_baseline = camera.get("fxb", 0.0) / fx if fx else 0.0
+    Rcw = _rot_y(0.2 * rng.standard_normal()) @ _rodrigues(0.05 * rng.standard_normal(3))
+    tcw = rng.normal(0, 1.0, 3)
+
+    def back_project(uu, vv, depth):
+        if equirect:                                                 # camera/equirectangular.cc:42-49: pixel -> bearing
+            lon, lat = (uu / camera["cols"] - 0.5) * 2 * np.pi, -(vv / camera["rows"] - 0.5) * np.pi
+            return np.stack([np.cos(lat) * np.sin(lon), -np.sin(lat), np.cos(lat) * np.cos(lon)], 1) * depth[:, None]
+        return np.stack([(uu - cx) / fx * depth, (vv - cy) / fy * depth, depth], 1)
+
+    pick = np.nonzero(rng.random(n_kp) < landmark_frac)[0]
+    z = rng.uniform(4, 40, len(pick))
+    u = kps["x"][pick].astype(np.float64) + pixel_sigma * rng.standard_normal(len(pick))
+    v = kps["y"][pick].astype(np.float64) + pixel_sigma * rng.standard_normal(len(pick))
+    n_cl = int(clutter_frac * len(pick))
+    zc = rng.uniform(4, 60, n_cl) if equirect else rng.uniform(-10, 60, n_cl)
+    uc, vc = rng.uniform(-200, camera["cols"] + 200, n_cl), rng.uniform(-100, camera["rows"] + 100, n_cl)
+    if equirect:
+        uc, vc = np.clip(uc, 0, camera["cols"] - 1), np.clip(vc, 0, camera["rows"] - 1)
+    pc = np.concatenate([back_project(u, v, z), back_project(uc, vc, zc)])
+    pw = (pc - tcw) @ Rcw
+    n_lm = len(pw)
+    ldesc = rng.integers(0, 256, (n_lm, 32), dtype=np.uint8)
+    for j, k in enumerate(pick):
+        row = desc[k].copy()
+        for b in rng.choice(256, int(rng.integers(0, max_flips + 1)), replace=False):
+            row[b >> 3] ^= np.uint8(1 << (b & 7))
+        ldesc[j] = row
+    octave = np.concatenate([kps["octave"][pick].astype(np.int64), rng.integers(0, len(sf), n_cl)]).astype(np.uint8)
+    angle = np.concatenate([kps["angle"][pick].astype(np.float64) + rng.uniform(-8, 8, len(pick)), rng.uniform(0, 360, n_cl)])
+    turned = rng.random(n_lm) < rotated_frac
+    angle[turned] += rng.uniform(40, 180, turned.sum()) * rng.choice([-1, 1], turned.sum())
+    angle = np.mod(angle, 360.0).astype(np.float32)
+    has_obs = (rng.random(n_lm) >= no_obs_frac).astype(np.uint8)
+    perm = rng.permutation(n_lm)
+    kp_x_right = None
+    if stereo:
+        kp_x_right = np.full(n_kp, -1.0, np.float32)
+        zk = np.full(n_kp, np.nan)
+        zk[pick] = z
+        ok = ~np.isnan(zk) & (rng.random(n_kp) < 0.8)
+        kp_x_right[ok] = (kps["x"][ok] - camera["fxb"] / zk[ok] + 0.5 * rng.standard_normal(ok.sum())).astype(np.float32)
+    turn = shift_px * 2 * np.pi / camera["cols"] if equirect else np.arctan(shift_px / fx)
+    dR = _rodrigues(np.deg2rad(rot_deg) * rng.standard_normal(3) / np.sqrt(3)) @ _rot_y(turn)
+    pose = np.eye(4)
+    pose[:3, :3] = dR @ Rcw
+    pose[:3, 3] = dR @ tcw + trans_m * rng.standard_normal(3) / np.sqrt(3)
+    gt = np.eye(4)
+    gt[:3, :3], gt[:3, 3] = Rcw, tcw
+    axis = {"forward": np.array([0.0, 0.0, 1.0]), "backward": np.array([0.0, 0.0, -1.0]), "sideways": np.array([1.0, 0.0, 0.0])}[motion]
+    step = 2.0 * true_baseline if true_baseline > 0 else 0.1
+    center_last = -Rcw.T @ tcw - Rcw.T @ (step * axis)             # trans_lc = R_cw (c_curr - c_last) = step * axis
+    last = np.eye(4)
+    last[:3, :3], last[:3, 3] = Rcw, -Rcw @ center_last
+    return dict(pose_cw=pose, last_pose_cw=last, gt_pose_cw=gt, kp_x_right=kp_x_right, true_baseline=float(true_baseline),
+                table=dict(pos_w=pw[perm], desc=ldesc[perm], octave=octave[perm], angle=angle[perm], has_observation=has_obs[perm]))
+
 def make_mapping_problem(seed, n_neighbours=10, n_keypoints=2000, model="perspective", stereo=False, num_levels=8, scale_factor=1.2):
     """A current keyframe and `n_neighbours` ordered covisibilities for the mapping module's landmark creation
     (mapping_module::create_new_landmarks, two_view_triangulator).  Returns (cur, neighbours): keyframe dicts in the shape of
