@@ -625,6 +625,51 @@ int b200_motion_based_track(b200_orb_t orb, b200_matcher_t matcher, b200_lba_t o
 int b200_motion_track_stage_ms(b200_matcher_t matcher, int stage, float* ms);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Robust-match tracking on the device: module::frame_tracker::robust_match_based_track (module/frame_tracker.cc:97-131) with
+ * match::robust(lowe_ratio, true)::match_frame_and_keyframe (match/robust.cc:195-230) for `n_frames` independent frames in ONE launch
+ * sequence, reading the extractor's results in HBM:
+ *   undistortion and bearings of the frame's keypoints (the four camera models of b200_keypoints_undistort)
+ *   robust::brute_force_match (robust.cc:232-328): the frame is side 1, the reference keyframe side 2 (its keypoints whose landmark
+ *     exists and is not will_be_erased, kf_valid); HAMMING_DIST_THR_LOW, the orientation check on; pairs sorted by frame keypoint
+ *   essential_solver::find_via_ransac(1000, true) with the five-point set on the pairs' bearings; its 1 000 minimal sets are drawn on the
+ *     device from the frame's engine, bit-identical to b200_draw_min_sets
+ *   n_inliers = the inlier count, 0 when the solution is not valid; applied = n_inliers >= num_matches_thr (:105-108)
+ *   when applied: set_landmarks (every inlier pair gives its frame keypoint the keyframe keypoint's landmark, every other keypoint none),
+ *     the pose last_pose_cw, pose_optimizer::optimize (the < 5 observations early return included), then discard_outliers (:133-150):
+ *     an outlier keypoint loses its landmark; tracked = n_valid >= num_matches_thr.
+ * prm: b200_track_params_t with lowe_ratio = 0.8 (robust(0.8, true)), the camera, levels and the optimiser's trials; margin,
+ * hamming_thr, grid, max_candidates, ray_cos_thr and log_scale_factor are not used.
+ * When applied is 0 the reference returns before it touches the frame: kp_landmark_out and pose_cw_out are not written, n_valid and
+ * tracked are 0.  B200_ERR_INVALID, with nothing written, for bad parameters, a null required pointer, an n_keypoints_in that
+ * disagrees with the extractor's count or a kp_cap below it.  One upload, one download and one stream synchronise per call. */
+typedef struct b200_robust_track_frame {
+    int32_t frame;                      /* index into the extractor's last batch */
+    const double* last_pose_cw;         /* 16, row-major: last_frm.get_pose_cw(), the optimisation's initial pose (:115) */
+    int32_t n_keypoints_in;             /* entries of kp_x_right (0 when NULL); must equal the frame's keypoint count */
+    const float* kp_x_right;            /* stereo_x_right_ of the current frame, NULL = monocular */
+    const struct b200_mt19937* engine;  /* the solver's engine (b200_mt19937_seed); NULL = default-constructed, create_random_engine(true) */
+    int32_t n_kf_keypoints;             /* reference keyframe, in its keypoint order: */
+    const uint8_t* kf_desc;             /* 32 per keypoint: frm_obs_.descriptors_ */
+    const float* kf_angle;              /* undist_keypts_[i].angle */
+    const double* kf_bearings;          /* 3 per keypoint: frm_obs_.bearings_ */
+    const uint8_t* kf_valid;            /* 1 = the keypoint has a landmark that is not will_be_erased */
+    const double* kf_pos_w;             /* 3 per keypoint: its landmark's position (read for valid keypoints only) */
+    int32_t kp_cap;                     /* capacity of kp_landmark_out (>= the frame's keypoint count) */
+    int32_t* kp_landmark_out;           /* out when applied, per keypoint: the keyframe keypoint whose landmark it carries, -1 none */
+    double pose_cw_out[16];             /* out when applied */
+    int32_t n_keypoints, n_matches;     /* out; n_matches = brute_force_match's count */
+    int32_t essential_valid, status;    /* out: solution_is_valid(), and B200_OK or B200_ERR_INVALID as b200_essential_problem_t.status */
+    int32_t n_inliers, applied;         /* out: match_frame_and_keyframe's return value; n_inliers >= num_matches_thr */
+    uint32_t n_valid;                   /* out: discard_outliers' count */
+    int32_t tracked;                    /* out: robust_match_based_track's return value */
+} b200_robust_track_frame_t;
+int b200_robust_match_based_track(b200_orb_t orb, b200_matcher_t matcher, b200_lba_t opt, const b200_track_params_t* prm, uint32_t num_matches_thr,
+                                  int n_frames, b200_robust_track_frame_t* frames);
+/* Device time of the last b200_robust_match_based_track, per stage: 0 undistort + bearings, 1 brute force, 2 sampler, 3 essential,
+ * 4 edge build, 5 pose optimisation + discard, 6 whole chain (CUDA events on the stream). */
+int b200_robust_track_stage_ms(b200_matcher_t matcher, int stage, float* ms);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * New landmarks of the mapping module: module::two_view_triangulator (src/stella_vslam/module/two_view_triangulator.{h,cc}, with
  * solve::triangulator::triangulate, solve/triangulator.h:77-90, and data::triangulate_stereo, data/common.cc:192-260) and the
  * numeric chain of mapping_module::create_new_landmarks after the baseline test (mapping_module.cc, triangulate_with_two_keyframes).
@@ -810,7 +855,8 @@ typedef struct b200_epnp_problem {
 int b200_epnp_compute_pose(b200_lba_t h, int n_problems, b200_epnp_problem_t* problems);
 
 /* std::mt19937 as libstdc++ implements it, and util::create_random_array(4, 0, n - 1, engine) as find_via_ransac draws its minimal
- * sets (std::uniform_int_distribution<unsigned>, sort, unique, std::shuffle).  Host only.  The draws reproduce a reference built
+ * sets (std::uniform_int_distribution<unsigned>, sort, unique, std::shuffle), on the host (b200_draw_min_sets_batch: the same sampler on
+ * the device).  The draws reproduce a reference built
  * against libstdc++ (GCC 11 or later: Lemire's nearly divisionless uniform_int_distribution). */
 typedef struct b200_mt19937 {
     uint32_t state[624];
@@ -825,6 +871,12 @@ int b200_pnp_draw_min_sets(b200_mt19937_t* engine, uint32_t n_matches, uint32_t 
 /* max_num_iter calls of util::create_random_array(set_size, 0, n_matches - 1, engine) (out: max_num_iter x set_size), continuing the
  * engine's state.  B200_ERR_INVALID for a null engine, set_size outside [1, 65535] or n_matches < set_size. */
 int b200_draw_min_sets(b200_mt19937_t* engine, uint32_t set_size, uint32_t n_matches, uint32_t max_num_iter, int32_t* out);
+/* The device sampler of b200_robust_match_based_track for n_engines engines on the handle's stream: engine p (engines NULL: every
+ * engine default-constructed) makes max_num_iter calls of util::create_random_array(set_size, 0, n_matches[p] - 1) into
+ * out + p * max_num_iter * set_size, the same draws as b200_draw_min_sets; the engines are not advanced.  B200_ERR_INVALID for
+ * set_size outside [1, 8] or an n_matches below set_size. */
+int b200_draw_min_sets_batch(b200_lba_t h, int n_engines, const b200_mt19937_t* engines, uint32_t set_size, const uint32_t* n_matches,
+                             uint32_t max_num_iter, int32_t* out);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Robust matching's essential matrix: solve::essential_solver::find_via_ransac (src/stella_vslam/solve/essential_solver.cc) with the

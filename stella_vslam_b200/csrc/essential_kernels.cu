@@ -1,8 +1,9 @@
 // essential_kernels.cu -- solve::essential_solver (src/stella_vslam/solve/essential_solver.cc) on the device: find_via_ransac with the
 // five-point minimal set for many problems in one launch sequence on the b200_lba_t handle's stream.  The minimal sets are drawn on the
-// host (random_array.cu).
+// host (random_array.cu), or on the device in the robust-match tracking chain (match_kernels.cu).
 //
-// find_via_ransac is split in three launches:
+// find_via_ransac is split in three launches (enqueue_ransac, essential_ransac.cuh), which read each problem's match count and whether it
+// runs from device memory:
 //   essential_hypothesis_kernel  one thread per (problem, iteration): compute_E_21_minimal on the minimal set (essential_core.h),
 //                                up to ten candidates written to scratch in eigenvalue order;
 //   essential_score_kernel       one thread per (problem, iteration, candidate slot): check_inliers, the float cost accumulated over
@@ -19,6 +20,7 @@
 
 #include "common.cuh"
 #include "epnp.cuh"
+#include "essential_ransac.cuh"
 #include "ransac_host.cuh"
 #include "staging.cuh"
 #include "util_trig.cuh"
@@ -35,34 +37,6 @@ using tri::ds;
 
 #include "essential_core.cuh"
 
-constexpr int kMinSet = 5;
-constexpr int kMaxCand = 10;
-
-struct ProblemDev {
-    int n;          // matches
-    int match_off;  // first row in the concatenated bearings / flags
-    int hyp_off;    // first iteration in the concatenated minimal sets
-    int n_hyp;      // max_num_iter (0 on the early return)
-    int runs;       // 0: find_via_ransac returns before drawing (n < min_set_size)
-    int recompute;
-};
-
-struct HypDev {
-    int count;  // candidates written
-    int flags;  // ES_STATUS_* bits
-};
-
-struct ScoreDev {
-    float cost;
-    unsigned num_inliers;
-};
-
-struct ResultDev {
-    double E[9];
-    float best_cost;
-    int valid, best_iter, best_candidate, num_inliers, status;
-};
-
 __global__ void __launch_bounds__(32) essential_hypothesis_kernel(int n_hyp_total, const int* __restrict__ hyp_problem,
                                                                    const ProblemDev* __restrict__ probs, const double* __restrict__ b1,
                                                                    const double* __restrict__ b2, const int32_t* __restrict__ min_sets,
@@ -72,8 +46,10 @@ __global__ void __launch_bounds__(32) essential_hypothesis_kernel(int n_hyp_tota
     const ProblemDev P = probs[hyp_problem[h]];
     HypDev out;
     out.flags = 0;
-    out.count = es_minimal(b1 + 3 * (size_t)P.match_off, b2 + 3 * (size_t)P.match_off, min_sets + kMinSet * (size_t)h,
-                           cand + 9 * kMaxCand * (size_t)h, &out.flags);
+    out.count = 0;
+    if (P.runs)
+        out.count = es_minimal(b1 + 3 * (size_t)P.match_off, b2 + 3 * (size_t)P.match_off, min_sets + kMinSet * (size_t)h,
+                               cand + 9 * kMaxCand * (size_t)h, &out.flags);
     hyps[h] = out;
 }
 
@@ -149,6 +125,21 @@ __global__ void __launch_bounds__(64) essential_select_kernel(int n_problems, co
     results[q] = r;
 }
 
+int enqueue_ransac(cudaStream_t st, int n_problems, int n_hyp, const RansacDev& d) {
+    if (n_hyp > 0) {
+        // 32-thread blocks: one problem of 1 000 iterations spreads over 32 SMs rather than 8 (the tracker's fallback is one problem)
+        essential_hypothesis_kernel<<<b200::ceil_div(n_hyp, 32), 32, 0, st>>>(n_hyp, d.hyp_problem, d.probs, d.b1, d.b2, d.min_sets, d.cand, d.hyps);
+        B200_CUDA(cudaGetLastError());
+        const long long slots = (long long)n_hyp * kMaxCand;
+        essential_score_kernel<<<(unsigned)((slots + 63) / 64), 64, 0, st>>>(slots, d.hyp_problem, d.probs, d.b1, d.b2, d.cand, d.hyps, d.scores);
+        B200_CUDA(cudaGetLastError());
+    }
+    essential_select_kernel<<<b200::ceil_div(n_problems, 64), 64, 0, st>>>(n_problems, d.probs, d.b1, d.b2, d.cand, d.hyps, d.scores, d.idx, d.mat,
+                                                                          d.flags, d.results);
+    B200_CUDA(cudaGetLastError());
+    return B200_OK;
+}
+
 }  // namespace ess
 }  // namespace b200
 
@@ -210,24 +201,10 @@ int b200_essential_ransac(b200_lba_t h, int n_problems, b200_essential_problem_t
                              (int*)(hb + o_hp));
     }
     B200_CUDA(A->upload(in_bytes, st));
-    const double* d_b1 = (const double*)(db + o_b1);
-    const double* d_b2 = (const double*)(db + o_b2);
-    if (total_hyp > 0) {
-        // 32-thread blocks: one problem of 1 000 iterations spreads over 32 SMs rather than 8 (the tracker's fallback is one problem)
-        essential_hypothesis_kernel<<<b200::ceil_div((int)total_hyp, 32), 32, 0, st>>>(
-            (int)total_hyp, (const int*)(db + o_hp), (const ProblemDev*)(db + o_probs), d_b1, d_b2, (const int32_t*)(db + o_ms),
-            (double*)(db + o_cand), (HypDev*)(db + o_hyp));
-        B200_CUDA(cudaGetLastError());
-        const long long slots = total_hyp * kMaxCand;
-        essential_score_kernel<<<(unsigned)((slots + 63) / 64), 64, 0, st>>>(slots, (const int*)(db + o_hp), (const ProblemDev*)(db + o_probs),
-                                                                                d_b1, d_b2, (const double*)(db + o_cand),
-                                                                                (const HypDev*)(db + o_hyp), (ScoreDev*)(db + o_sc));
-        B200_CUDA(cudaGetLastError());
-    }
-    essential_select_kernel<<<b200::ceil_div(n_problems, 64), 64, 0, st>>>(
-        n_problems, (const ProblemDev*)(db + o_probs), d_b1, d_b2, (const double*)(db + o_cand), (const HypDev*)(db + o_hyp),
-        (const ScoreDev*)(db + o_sc), (int32_t*)(db + o_idx), (double*)(db + o_mat), db + o_fl, (ResultDev*)(db + o_res));
-    B200_CUDA(cudaGetLastError());
+    const RansacDev dev{(const int*)(db + o_hp), (const ProblemDev*)(db + o_probs), (const double*)(db + o_b1), (const double*)(db + o_b2),
+                        (const int32_t*)(db + o_ms), (double*)(db + o_cand), (HypDev*)(db + o_hyp), (ScoreDev*)(db + o_sc), (int32_t*)(db + o_idx),
+                        (double*)(db + o_mat), db + o_fl, (ResultDev*)(db + o_res)};
+    if ((rc = enqueue_ransac(st, n_problems, (int)total_hyp, dev))) return rc;
     B200_CUDA(A->download(o_res, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
     const ResultDev* res = reinterpret_cast<const ResultDev*>(hb + o_res);

@@ -1628,6 +1628,7 @@ __global__ void __launch_bounds__(128) track_keypoints_kernel(chain::TrackShared
     if (i == 0) {
         F.status[0] = n;
         F.status[1] = ((F.kp_x_right || F.kp_landmark) && F.n_kp_in != n) ? 1 : 0;
+        if (F.count_out) *F.count_out = n;
     }
     if (i >= n) return;
     const b200_keypoint_t kp = F.kps[i];
@@ -1641,6 +1642,7 @@ __global__ void __launch_bounds__(128) track_keypoints_kernel(chain::TrackShared
     o.response = (sh.model == 1) ? kp.response : 0.f;
     o.octave = kp.octave;
     F.undist[i] = o;
+    if (F.bearings) point_to_bearing(cam_of(sh), ux, uy, F.bearings + 3 * (size_t)i);
     F.t_x[i] = ux;
     F.t_y[i] = uy;
     F.t_octave[i] = (unsigned char)kp.octave;
@@ -1731,6 +1733,12 @@ namespace chain {
 int track_stage_a(cudaStream_t st, const TrackShared& sh, const TrackFrameDev* d_frames, int n_frames, int max_kp, int max_lm) {
     if (max_kp > 0) orb::track_keypoints_kernel<<<dim3(ceil_div(max_kp, 128), n_frames), 128, 0, st>>>(sh, d_frames);
     if (max_lm > 0) orb::track_landmarks_kernel<<<dim3(ceil_div(max_lm, 128), n_frames), 128, 0, st>>>(sh, d_frames);
+    B200_CUDA(cudaGetLastError());
+    return B200_OK;
+}
+
+int robust_stage_a(cudaStream_t st, const TrackShared& sh, const TrackFrameDev* d_frames, int n_frames, int max_kp) {
+    if (max_kp > 0) orb::track_keypoints_kernel<<<dim3(ceil_div(max_kp, 128), n_frames), 128, 0, st>>>(sh, d_frames);
     B200_CUDA(cudaGetLastError());
     return B200_OK;
 }

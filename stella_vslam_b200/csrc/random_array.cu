@@ -1,85 +1,53 @@
-// random_array.cu -- the minimal-set sampler of the RANSAC solvers, on the host: std::mt19937 and util::create_random_array
-// (src/stella_vslam/util/random_array.cc) as libstdc++ evaluates them.  The solvers draw their minimal sets here, in draw order, and
-// pass them to b200_pnp_ransac, b200_essential_ransac and b200_twoview_ransac.
+// random_array.cu -- the minimal-set sampler of the RANSAC solvers: std::mt19937 and util::create_random_array
+// (src/stella_vslam/util/random_array.cc) as libstdc++ evaluates them (random_array.cuh).  The solvers draw their minimal sets here on
+// the host, in draw order, and pass them to b200_pnp_ransac, b200_essential_ransac and b200_twoview_ransac; the device sampler draws
+// them where the match count is only known on the device (b200_robust_match_based_track).
+#include <climits>
 #include <cstdint>
+#include <cstring>
 #include <vector>
 
 #include "common.cuh"
+#include "random_array.cuh"
+#include "staging.cuh"
+#include "track_chain.cuh"
 
 namespace b200 {
-namespace {
+namespace rnd {
 
-void mt_twist(b200_mt19937_t* e) {
-    uint32_t* x = e->state;
-    for (int k = 0; k < 624; ++k) {
-        const uint32_t y = (x[k] & 0x80000000u) | (x[(k + 1) % 624] & 0x7fffffffu);
-        x[k] = x[(k + 397) % 624] ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
+// One warp per engine: max_num_iter calls of create_random_array(set_size, 0, n[p] - 1) for every problem p with n[p] >= set_size, the
+// engine's state in shared memory.  engines == null: default-constructed engines (seed 5489), built here.
+__global__ void __launch_bounds__(32) draw_min_sets_kernel(const b200_mt19937_t* __restrict__ engines, const int* __restrict__ n, uint32_t set_size,
+                                                           uint32_t max_num_iter, int32_t* __restrict__ out) {
+    __shared__ uint32_t x[624];
+    const int p = blockIdx.x;
+    const int np = n[p];
+    if (np < (int)set_size) return;
+    MtRef e{x, 624u, threadIdx.x, 32u};
+    if (engines) {
+        for (int k = threadIdx.x; k < 624; k += 32) x[k] = engines[p].state[k];
+        e.index = engines[p].index;
+    } else if (threadIdx.x == 0) {
+        x[0] = 5489u;
+        for (uint32_t i = 1; i < 624; ++i) x[i] = 1812433253u * (x[i - 1] ^ (x[i - 1] >> 30)) + i;
     }
-    e->index = 0;
+    __syncwarp();
+    uint32_t v[scratch_size(kMaxDeviceSet)];
+    int32_t* o = out + (size_t)p * max_num_iter * set_size;
+    for (uint32_t it = 0; it < max_num_iter; ++it) create_random_array(e, set_size, (uint32_t)np, v, o + (size_t)set_size * it);
 }
 
-uint32_t mt_next(b200_mt19937_t* e) {
-    if (e->index >= 624) mt_twist(e);
-    uint32_t y = e->state[e->index++];
-    y ^= y >> 11;
-    y ^= (y << 7) & 0x9d2c5680u;
-    y ^= (y << 15) & 0xefc60000u;
-    y ^= y >> 18;
-    return y;
-}
+}  // namespace rnd
 
-// uniform_int_distribution{0, range - 1} on a 32-bit engine: Lemire's nearly divisionless method (libstdc++ _S_nd)
-uint32_t uniform_below(b200_mt19937_t* e, uint32_t range) {
-    uint64_t product = (uint64_t)mt_next(e) * range;
-    uint32_t low = (uint32_t)product;
-    if (low < range) {
-        const uint32_t threshold = (uint32_t)(0u - range) % range;
-        while (low < threshold) {
-            product = (uint64_t)mt_next(e) * range;
-            low = (uint32_t)product;
-        }
-    }
-    return (uint32_t)(product >> 32);
+namespace chain {
+int draw_min_sets(cudaStream_t st, int n_problems, const b200_mt19937_t* d_engines, const int* d_n, uint32_t set_size, uint32_t max_num_iter,
+                  int32_t* d_out) {
+    if (set_size < 1 || set_size > rnd::kMaxDeviceSet) return B200_ERR_INVALID;
+    if (n_problems > 0 && max_num_iter > 0) rnd::draw_min_sets_kernel<<<n_problems, 32, 0, st>>>(d_engines, d_n, set_size, max_num_iter, d_out);
+    B200_CUDA(cudaGetLastError());
+    return B200_OK;
 }
-
-// util::create_random_array(set_size, 0, n - 1, engine): make_size = size_t(set_size * 1.2) draws of uniform_int_distribution<unsigned>,
-// sort + unique (truncated to set_size), repeated until set_size remain, then std::shuffle.
-void create_random_array(b200_mt19937_t* e, uint32_t set_size, uint32_t n, uint32_t* v, int32_t* out) {
-    const size_t make_size = (size_t)(set_size * 1.2);
-    size_t size = 0;
-    while (size != set_size) {
-        while (size < make_size) v[size++] = uniform_below(e, n);
-        for (size_t i = 1; i < size; ++i)
-            for (size_t j = i; j > 0 && v[j - 1] > v[j]; --j) {
-                const uint32_t t = v[j];
-                v[j] = v[j - 1];
-                v[j - 1] = t;
-            }
-        size_t u = 0;
-        for (size_t i = 0; i < size; ++i)
-            if (u == 0 || v[u - 1] != v[i]) v[u++] = v[i];
-        size = u < set_size ? u : set_size;
-    }
-    // std::shuffle: with a 32-bit engine and set_size^2 <= 2^32 - 1, swap positions come in pairs from one draw
-    uint32_t t;
-    size_t i = 1;
-    if (set_size % 2 == 0) {
-        const uint32_t d = uniform_below(e, 2);
-        t = v[i], v[i] = v[d], v[d] = t;
-        ++i;
-    }
-    while (i < set_size) {
-        const uint32_t r = (uint32_t)i + 1;
-        const uint32_t x = uniform_below(e, r * (r + 1));
-        t = v[i], v[i] = v[x / (r + 1)], v[x / (r + 1)] = t;
-        ++i;
-        t = v[i], v[i] = v[x % (r + 1)], v[x % (r + 1)] = t;
-        ++i;
-    }
-    for (uint32_t k = 0; k < set_size; ++k) out[k] = (int32_t)v[k];
-}
-
-}  // namespace
+}  // namespace chain
 }  // namespace b200
 
 extern "C" {
@@ -116,18 +84,58 @@ int b200_mt19937_seed(b200_mt19937_t* e, const uint32_t* seed_seq, int n_seed) {
     return B200_OK;
 }
 
-uint32_t b200_mt19937_next(b200_mt19937_t* e) { return e ? b200::mt_next(e) : 0u; }
+uint32_t b200_mt19937_next(b200_mt19937_t* e) {
+    if (!e) return 0u;
+    b200::rnd::MtRef r{e->state, e->index, 0, 1};
+    const uint32_t y = b200::rnd::mt_next(r);
+    e->index = r.index;
+    return y;
+}
 
 int b200_draw_min_sets(b200_mt19937_t* e, uint32_t set_size, uint32_t n_matches, uint32_t max_num_iter, int32_t* out) {
     // set_size <= 65535 keeps set_size^2 within the engine's range (the paired shuffle) and the products below in 32 bits
     if (!e || set_size < 1 || set_size > 65535u || n_matches < set_size || (max_num_iter > 0 && !out)) return B200_ERR_INVALID;
-    std::vector<uint32_t> v((size_t)(set_size * 1.2) + set_size);
-    for (uint32_t it = 0; it < max_num_iter; ++it) b200::create_random_array(e, set_size, n_matches, v.data(), out + (size_t)set_size * it);
+    std::vector<uint32_t> v(b200::rnd::scratch_size(set_size));
+    b200::rnd::MtRef r{e->state, e->index, 0, 1};
+    for (uint32_t it = 0; it < max_num_iter; ++it) b200::rnd::create_random_array(r, set_size, n_matches, v.data(), out + (size_t)set_size * it);
+    e->index = r.index;
     return B200_OK;
 }
 
 int b200_pnp_draw_min_sets(b200_mt19937_t* e, uint32_t n_matches, uint32_t max_num_iter, int32_t* out) {
     return b200_draw_min_sets(e, 4, n_matches, max_num_iter, out);
+}
+
+int b200_draw_min_sets_batch(b200_lba_t h, int n_engines, const b200_mt19937_t* engines, uint32_t set_size, const uint32_t* n_matches,
+                             uint32_t max_num_iter, int32_t* out) {
+    B200_RANGE("b200:random:draw_min_sets_batch");
+    if (!h || n_engines < 0 || set_size < 1 || set_size > b200::rnd::kMaxDeviceSet || max_num_iter > (1u << 24)) return B200_ERR_INVALID;
+    if (n_engines == 0 || max_num_iter == 0) return B200_OK;
+    if (!n_matches || !out) return B200_ERR_INVALID;
+    for (int p = 0; p < n_engines; ++p)
+        if (n_matches[p] < set_size || n_matches[p] > (uint32_t)INT32_MAX || (engines && engines[p].index > 624u)) {
+            b200::set_error("b200_draw_min_sets_batch: engine %d: n_matches %u below the set size or a bad engine index", p, n_matches[p]);
+            return B200_ERR_INVALID;
+        }
+    const size_t out_bytes = sizeof(int32_t) * set_size * (size_t)max_num_iter * n_engines;
+    b200::Layout a;
+    const size_t o_eng = a.take<b200_mt19937_t>(engines ? n_engines : 0), o_n = a.take<int>(n_engines);
+    const size_t in_bytes = a.end;
+    const size_t o_out = a.take(out_bytes);
+    cudaStream_t st;
+    b200::StagingArena* A;
+    int rc = b200::lba::staging(h, a.end, a.end, &st, &A);
+    if (rc) return rc;
+    if (engines) A->put(o_eng, engines, sizeof(b200_mt19937_t) * n_engines);
+    A->put(o_n, n_matches, sizeof(int) * n_engines);
+    B200_CUDA(A->upload(in_bytes, st));
+    if ((rc = b200::chain::draw_min_sets(st, n_engines, engines ? A->dev<const b200_mt19937_t>(o_eng) : nullptr, A->dev<const int>(o_n), set_size,
+                                         max_num_iter, A->dev<int32_t>(o_out))))
+        return rc;
+    B200_CUDA(A->download(o_out, o_out + out_bytes, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    std::memcpy(out, A->host(o_out), out_bytes);
+    return B200_OK;
 }
 
 }  // extern "C"

@@ -1,7 +1,8 @@
-// track_chain.cuh -- internal interfaces of b200_track_local_map and b200_motion_based_track (include/b200vslam.h): both chains are
-// driven from match_kernels.cu, stage A (undistort + can_observe or the last-frame reprojection + query build) lives in orb_kernels.cu
-// (same device functions and -fmad=false as the stage-by-stage ABI), stage C (edge build + pose optimisation) in lba_kernels.cu.  Plain
-// device pointers, no handles' internals cross a TU.
+// track_chain.cuh -- internal interfaces of b200_track_local_map, b200_motion_based_track and b200_robust_match_based_track
+// (include/b200vslam.h): the chains are driven from match_kernels.cu, stage A (undistort + bearings, can_observe or the last-frame
+// reprojection + query build) lives in orb_kernels.cu (same device functions and -fmad=false as the stage-by-stage ABI), stage C (edge
+// build + pose optimisation) in lba_kernels.cu, the robust chain's minimal-set sampler in random_array.cu and its RANSAC in
+// essential_kernels.cu (essential_ransac.cuh).  Plain device pointers, no handles' internals cross a TU.
 #pragma once
 
 #include <cmath>
@@ -64,6 +65,9 @@ struct TrackFrameDev {  // one frame; every pointer is a device pointer
     float* t_angle;                   // stage A: angle of every keypoint, for the orientation gate
     const unsigned char* lm_octave;   // last-frame table: octave of the last frame's keypoint
     double last_Rt[12];               // last frame: rot_cw row-major, then trans_cw
+    // b200_robust_match_based_track only (null in the other chains)
+    double* bearings;                 // stage A: bearing of every keypoint (3 doubles)
+    int* count_out;                   // stage A: the keypoint count again, in the per-frame array the brute-force matcher reads
 };
 
 // orb_kernels.cu: device views of the extractor's last batch + the stream its work is ordered on
@@ -72,6 +76,13 @@ int orb_results(b200_orb_t orb, const b200_keypoint_t** d_kps, const unsigned ch
 int track_stage_a(cudaStream_t st, const TrackShared& sh, const TrackFrameDev* d_frames, int n_frames, int max_kp, int max_lm);
 // the same keypoint kernel (with t_angle), then one query per last-frame table entry (projection.cc:95-160)
 int motion_stage_a(cudaStream_t st, const TrackShared& sh, const TrackFrameDev* d_frames, int n_frames, int max_kp, int max_lm);
+// the same keypoint kernel with the bearings and count_out (camera::base::convert_keypoints_to_bearings after the undistortion)
+int robust_stage_a(cudaStream_t st, const TrackShared& sh, const TrackFrameDev* d_frames, int n_frames, int max_kp);
+// random_array.cu: for every problem p with d_n[p] >= set_size (<= rnd::kMaxDeviceSet), max_num_iter calls of
+// util::create_random_array(set_size, 0, d_n[p] - 1) from engine p (d_engines null: default-constructed engines) into
+// d_out + p * max_num_iter * set_size.  One warp per problem.
+int draw_min_sets(cudaStream_t st, int n_problems, const b200_mt19937_t* d_engines, const int* d_n, uint32_t set_size, uint32_t max_num_iter,
+                  int32_t* d_out);
 // lba_kernels.cu: builds one edge per keypoint that carries a landmark (keypoint order), runs pose_optimizer::optimize for every frame and
 // scatters the flags back to keypoint indexing.  h_frames = the host copy of d_frames; pose_out / n_valid are device pointers.
 // d_gate: null, or per frame 0 = apply the matches but build no edge (the pose stays, no flag is set).

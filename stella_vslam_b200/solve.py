@@ -58,6 +58,7 @@ def _L():
         L.b200_mt19937_next.argtypes = [C.POINTER(Mt19937)]
         L.b200_mt19937_next.restype = C.c_uint32
         L.b200_draw_min_sets.argtypes = [C.POINTER(Mt19937), C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_int32)]
+        L.b200_draw_min_sets_batch.argtypes = [vp, C.c_int, C.POINTER(Mt19937), C.c_uint32, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(C.c_int32)]
         L.b200_essential_ransac.argtypes = [vp, C.c_int, C.POINTER(EssentialProblem)]
         L.b200_twoview_ransac.argtypes = [vp, C.c_int, C.POINTER(TwoviewProblem)]
         L._pnp_bound = True
@@ -97,6 +98,23 @@ def draw_min_sets(n_matches, max_num_iter, engine=None, set_size=4):
     out = np.zeros((max(int(max_num_iter), 1), max(k, 1)), np.int32)
     check(_L().b200_draw_min_sets(C.byref(e), k, int(n_matches), int(max_num_iter), out.ctypes.data_as(C.POINTER(C.c_int32))))
     return out[:int(max_num_iter)]
+
+
+def draw_min_sets_batch(n_matches, max_num_iter, engines=None, set_size=5, device=0):
+    """The device sampler (b200_draw_min_sets_batch): engine p (engines None: default-constructed ones) draws max_num_iter minimal sets
+    from n_matches[p] matches, (len(n_matches), max_num_iter, set_size) int32.  The engines are not advanced."""
+    nm = np.ascontiguousarray(np.asarray(n_matches, np.uint32).reshape(-1))
+    n = len(nm)
+    k, it = int(set_size), int(max_num_iter)
+    arr = None
+    if engines is not None:
+        arr = (Mt19937 * max(n, 1))()
+        for i, e in enumerate(engines):
+            arr[i] = e
+    out = np.zeros((max(n, 1), max(it, 1), max(k, 1)), np.int32)
+    check(_L().b200_draw_min_sets_batch(_handle(device), n, arr, k, nm.ctypes.data_as(C.POINTER(C.c_uint32)), it,
+                                        out.ctypes.data_as(C.POINTER(C.c_int32))))
+    return out[:n, :it, :k]
 
 
 def _run_batch(entry, StructT, pack, problems, device):

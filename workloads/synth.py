@@ -643,6 +643,80 @@ def make_motion_frame(kps, desc, camera, scale_factors, seed=0, stereo=False, mo
     return dict(pose_cw=pose, last_pose_cw=last, gt_pose_cw=gt, kp_x_right=kp_x_right, true_baseline=float(true_baseline),
                 table=dict(pos_w=pw[perm], desc=ldesc[perm], octave=octave[perm], angle=angle[perm], has_observation=has_obs[perm]))
 
+def make_robust_frame(kps, desc, camera, seed=0, stereo=False, landmark_frac=0.6, clutter_frac=0.2, rotated_frac=0.05, erased_frac=0.05,
+                      wrong_depth_frac=0.1, max_flips=20, baseline_m=0.5, rot_deg=2.0, trans_m=0.05, kf_keypoints=None):
+    """The reference keyframe of frame_tracker::robust_match_based_track for one extracted frame (keypoints taken as undistorted), under a
+    known relative pose.  A `landmark_frac` share of the frame's keypoints get a landmark at a random depth along their ray under the true
+    pose; each is a keyframe keypoint (bearing of the landmark seen from the keyframe, descriptor = the frame keypoint's with a few flipped
+    bits, angle within a few degrees of it).  Among them: `rotated_frac` turned 40-180 degrees (rejected by the orientation check),
+    `erased_frac` whose landmark is will_be_erased (kf_valid 0) and `wrong_depth_frac` whose landmark sits at another depth along the
+    keyframe's ray (the pair fits the epipolar geometry, the pose optimisation rejects it).  Clutter keypoints have random descriptors,
+    bearings and positions.  The keyframe's keypoints come in a shuffled order.  last_pose_cw is the true pose perturbed by rot_deg /
+    trans_m; the keyframe sits baseline_m away.  kf_keypoints caps the keyframe's size.  Perspective-family and equirectangular cameras."""
+    rng = np.random.default_rng(seed)
+    n_kp = len(kps)
+    equirect = camera.get("model", "perspective") == "equirectangular"
+    fx, fy, cx, cy = camera.get("fx", 1.0), camera.get("fy", 1.0), camera.get("cx", 0.0), camera.get("cy", 0.0)
+    u, v = kps["x"].astype(np.float64), kps["y"].astype(np.float64)
+    if equirect:                                                     # camera/equirectangular.cc:42-49
+        lon, lat = (u / camera["cols"] - 0.5) * 2 * np.pi, -(v / camera["rows"] - 0.5) * np.pi
+        rays = np.stack([np.cos(lat) * np.sin(lon), -np.sin(lat), np.cos(lat) * np.cos(lon)], 1)
+    else:
+        rays = np.stack([(u - cx) / fx, (v - cy) / fy, np.ones(n_kp)], 1)
+    Rcw = _rot_y(0.3 * rng.standard_normal()) @ _rodrigues(0.05 * rng.standard_normal(3))
+    tcw = rng.normal(0, 1.0, 3)
+    dRk = _rodrigues(np.deg2rad(3.0) * rng.standard_normal(3) / np.sqrt(3))
+    Rkw = dRk @ Rcw
+    tkw = dRk @ tcw + baseline_m * np.array([1.0, 0.2 * rng.standard_normal(), 0.1 * rng.standard_normal()])
+    pick = np.nonzero(rng.random(n_kp) < landmark_frac)[0]
+    depth = rng.uniform(4, 30, len(pick))
+    pc = rays[pick] * depth[:, None]                                 # perspective: z = depth; equirectangular: range = depth
+    pw = (pc - tcw) @ Rcw
+    pk = pw @ Rkw.T + tkw
+    kb = pk / np.linalg.norm(pk, axis=1, keepdims=True)
+    wrong = rng.random(len(pick)) < wrong_depth_frac
+    scale = rng.uniform(1.3, 2.5, wrong.sum()) * rng.choice([1 / 1.8, 1.0], wrong.sum())
+    pw[wrong] = ((pk[wrong] * scale[:, None]) - tkw) @ Rkw          # along the keyframe's ray, at another depth
+    kdesc = np.empty((len(pick), 32), np.uint8)
+    for j, k in enumerate(pick):
+        row = desc[k].copy()
+        for b in rng.choice(256, int(rng.integers(0, max_flips + 1)), replace=False):
+            row[b >> 3] ^= np.uint8(1 << (b & 7))
+        kdesc[j] = row
+    kang = kps["angle"][pick].astype(np.float64) + rng.uniform(-6, 6, len(pick))
+    turned = rng.random(len(pick)) < rotated_frac
+    kang[turned] += rng.uniform(40, 180, turned.sum()) * rng.choice([-1, 1], turned.sum())
+    n_cl = int(clutter_frac * len(pick))
+    cb = rng.normal(0, 1, (n_cl, 3))
+    cb[:, 2] = np.abs(cb[:, 2]) + 1.0
+    cb /= np.linalg.norm(cb, axis=1, keepdims=True)
+    cpw = ((cb * rng.uniform(4, 30, n_cl)[:, None]) - tkw) @ Rkw
+    desc_all = np.concatenate([kdesc, rng.integers(0, 256, (n_cl, 32), dtype=np.uint8)])
+    ang_all = np.mod(np.concatenate([kang, rng.uniform(0, 360, n_cl)]), 360.0).astype(np.float32)
+    bear_all = np.concatenate([kb, cb])
+    pos_all = np.concatenate([pw, cpw])
+    valid = (rng.random(len(desc_all)) >= erased_frac).astype(np.uint8)
+    perm = rng.permutation(len(desc_all))
+    if kf_keypoints is not None:
+        perm = perm[:int(kf_keypoints)]
+    pos_all = pos_all[perm]
+    pos_all[valid[perm] == 0] = 0.0                                  # not read for keypoints without a live landmark
+    kp_x_right = None
+    if stereo:
+        kp_x_right = np.full(n_kp, -1.0, np.float32)
+        zk = np.full(n_kp, np.nan)
+        zk[pick] = pc[:, 2]
+        ok = ~np.isnan(zk) & (rng.random(n_kp) < 0.8)
+        kp_x_right[ok] = (kps["x"][ok] - camera["fxb"] / zk[ok] + 0.5 * rng.standard_normal(ok.sum())).astype(np.float32)
+    gt = np.eye(4)
+    gt[:3, :3], gt[:3, 3] = Rcw, tcw
+    dR = _rodrigues(np.deg2rad(rot_deg) * rng.standard_normal(3) / np.sqrt(3))
+    last = np.eye(4)
+    last[:3, :3], last[:3, 3] = dR @ Rcw, dR @ tcw + trans_m * rng.standard_normal(3) / np.sqrt(3)
+    return dict(last_pose_cw=last, gt_pose_cw=gt, kp_x_right=kp_x_right,
+                keyframe=dict(desc=desc_all[perm], angle=ang_all[perm], bearings=bear_all[perm], valid=valid[perm], pos_w=pos_all))
+
+
 def make_mapping_problem(seed, n_neighbours=10, n_keypoints=2000, model="perspective", stereo=False, num_levels=8, scale_factor=1.2):
     """A current keyframe and `n_neighbours` ordered covisibilities for the mapping module's landmark creation
     (mapping_module::create_new_landmarks, two_view_triangulator).  Returns (cur, neighbours): keyframe dicts in the shape of
