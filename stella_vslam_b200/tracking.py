@@ -91,6 +91,22 @@ def _track_params(extractor, camera, margin, lowe_ratio, hamming_thr, ray_cos_th
     return p, (sf, isig)
 
 
+def _default_kp_cap(extractor):
+    """The extractor's largest keypoint count at its last image size."""
+    b, h, w = extractor._shape
+    return lib().b200_orb_max_keypoints(extractor._h, w, h)
+
+
+def _stage_ms(fn, names, device):
+    """{name: ms} of the calling thread's matcher's last call of one chain, read with fn (b200_*_stage_ms)."""
+    out = {}
+    for i, nm in enumerate(names):
+        v = C.c_float()
+        check(fn(match._matcher(device), i, C.byref(v)))
+        out[nm] = v.value
+    return out
+
+
 def camera_intrinsics(camera):
     """b200_camera_intrinsics_t of a camera dict (perspective, equirectangular, fisheye or radial_division; see _lib.camera_intrinsics)."""
     return _lib.camera_intrinsics(camera)
@@ -150,8 +166,7 @@ class local_map_tracker:
     def track(self, frames, kp_cap=None):
         """Returns, per frame: dict(observable bool (n_lm,), kp_landmark int32 (n_kp,), kp_outlier bool (n_kp,), pose_cw (4,4), n_matches, n_valid)."""
         if kp_cap is None:
-            b, h, w = self.extractor._shape
-            kp_cap = lib().b200_orb_max_keypoints(self.extractor._h, w, h)
+            kp_cap = _default_kp_cap(self.extractor)
         packed = self.pack(frames, kp_cap)
         self.run_packed(packed)
         res = []
@@ -163,12 +178,7 @@ class local_map_tracker:
         return res
 
     def stage_ms(self):
-        out = {}
-        for i, nm in enumerate(self.STAGES):
-            v = C.c_float()
-            check(self._L.b200_track_stage_ms(match._matcher(self.device), i, C.byref(v)))
-            out[nm] = v.value
-        return out
+        return _stage_ms(self._L.b200_track_stage_ms, self.STAGES, self.device)
 
 
 class frame_tracker:
@@ -233,8 +243,7 @@ class frame_tracker:
         """Returns, per frame: dict(kp_landmark int32 (n_kp,) after discard_outliers, pose_cw (4,4), n_keypoints, n_matches_first, n_matches,
         retried, n_valid, tracked)."""
         if kp_cap is None:
-            b, h, w = self.extractor._shape
-            kp_cap = lib().b200_orb_max_keypoints(self.extractor._h, w, h)
+            kp_cap = _default_kp_cap(self.extractor)
         packed = self.pack(frames, kp_cap)
         self.run_packed(packed)
         res = []
@@ -246,12 +255,7 @@ class frame_tracker:
         return res
 
     def stage_ms(self):
-        out = {}
-        for i, nm in enumerate(self.STAGES):
-            v = C.c_float()
-            check(self._L.b200_motion_track_stage_ms(match._matcher(self.device), i, C.byref(v)))
-            out[nm] = v.value
-        return out
+        return _stage_ms(self._L.b200_motion_track_stage_ms, self.STAGES, self.device)
 
     def pack_robust(self, frames, kp_cap):
         """frames: dicts(frame, last_pose_cw (4,4), keyframe=dict(desc (n, 32), angle, bearings (n, 3), valid, pos_w (n, 3)) [, kp_x_right]
@@ -295,8 +299,7 @@ class frame_tracker:
         """Returns, per frame: dict(kp_landmark int32 (n_kp,) after discard_outliers and pose_cw (4,4) -- both None when not applied (the
         reference leaves the frame as it was) --, n_keypoints, n_matches, essential_valid, status, n_inliers, applied, n_valid, tracked)."""
         if kp_cap is None:
-            b, h, w = self.extractor._shape
-            kp_cap = lib().b200_orb_max_keypoints(self.extractor._h, w, h)
+            kp_cap = _default_kp_cap(self.extractor)
         packed = self.pack_robust(frames, kp_cap)
         self.run_robust_packed(packed)
         res = []
@@ -310,9 +313,4 @@ class frame_tracker:
         return res
 
     def robust_stage_ms(self):
-        out = {}
-        for i, nm in enumerate(self.ROBUST_STAGES):
-            v = C.c_float()
-            check(self._L.b200_robust_track_stage_ms(match._matcher(self.device), i, C.byref(v)))
-            out[nm] = v.value
-        return out
+        return _stage_ms(self._L.b200_robust_track_stage_ms, self.ROBUST_STAGES, self.device)

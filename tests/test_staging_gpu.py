@@ -1,13 +1,13 @@
 """One staging arena per handle serves every host-buffer entry point that runs on it.  On one matcher handle and on one local-BA
 handle, calls of growing and then shrinking size, interleaved across those entry points, must give bit for bit what the same call
-gives on a fresh handle."""
+gives on a fresh handle.  The tracking chains also share the matcher's arena, and each keeps its own stage timer and parameter checks."""
 import contextlib
 import ctypes as C
 
 import numpy as np
 import pytest
 
-from stella_vslam_b200 import _lib, mapping, match, optimize, solve
+from stella_vslam_b200 import _lib, feature, mapping, match, optimize, solve, tracking
 from workloads import synth
 
 pytestmark = pytest.mark.gpu
@@ -154,3 +154,94 @@ def test_lba_arena_shared_across_entry_points():
         for call, w in zip(reversed(calls), reversed(want)):
             with _lba_handle(h):
                 _same(call(), w)
+
+
+KITTI = dict(model="perspective", fx=718.856, fy=718.856, cx=607.1928, cy=185.2157, fxb=386.1448, cols=1241.0, rows=376.0, setup="stereo")
+
+
+@pytest.fixture(scope="module")
+def chains():
+    """64 extracted KITTI-sized stereo frames with a local map, a last-frame table and a reference keyframe each, and the trackers."""
+    ex = feature.orb_extractor(feature.orb_params(), 2000, max_batch=64)
+    imgs = [synth.make_frame(1241, 376, seed=s) for s in range(200, 208)]
+    kps, descs = ex.extract_batch(np.stack([imgs[i % 8] for i in range(64)]))
+    sf = ex.orb_params_.scale_factors_
+    local = [dict(synth.make_tracking_frame(kps[i], descs[i], KITTI, sf, seed=70 + i, stereo=True), frame=i) for i in range(64)]
+    motion = [dict(synth.make_motion_frame(kps[i], descs[i], KITTI, sf, seed=170 + i, stereo=True), frame=i) for i in range(64)]
+    robust = [dict(synth.make_robust_frame(kps[i], descs[i], KITTI, seed=300 + i, stereo=True), frame=i) for i in range(64)]
+    return dict(ex=ex, local=local, motion=motion, robust=robust, lm=tracking.local_map_tracker(ex, KITTI),
+                ft=tracking.frame_tracker(ex, KITTI, use_fixed_seed=True))
+
+
+def _robust_frames(c, n):
+    # a fresh engine per call: the draws depend only on the frame
+    return [dict(fr, engine=solve.mt19937([i, 7])) for i, fr in enumerate(c["robust"][:n])]
+
+
+def _chain_calls(c):
+    calls = []
+    for n in (1, 8, 64, 2):
+        calls += [lambda n=n: c["lm"].track(c["local"][:n]), lambda n=n: c["ft"].motion_based_track(c["motion"][:n]),
+                  lambda n=n: c["ft"].robust_match_based_track(_robust_frames(c, n))]
+    return calls
+
+
+def test_tracking_chains_share_the_matcher_arena(chains):
+    calls = _chain_calls(chains)
+    want = []
+    for call in calls:
+        with _matcher_handle():
+            want.append(call())
+    assert sum(r["tracked"] for r in want[-4]) >= 32  # the 64-frame robust call tracks
+    with _matcher_handle() as h:
+        for call, w in zip(calls, want):
+            with _matcher_handle(h):
+                _same(call(), w)
+        for call, w in zip(reversed(calls), reversed(want)):
+            with _matcher_handle(h):
+                _same(call(), w)
+
+
+def test_chain_stage_timers_are_separate(chains):
+    c = chains
+    lm, ft = c["lm"], c["ft"]
+    runs = dict(local=lambda: lm.track(c["local"][:2]), motion=lambda: ft.motion_based_track(c["motion"][:2]),
+                robust=lambda: ft.robust_match_based_track(_robust_frames(c, 2)))
+    timers = dict(local=lm.stage_ms, motion=ft.stage_ms, robust=ft.robust_stage_ms)
+    with _matcher_handle():
+        started = set()
+        for name in ("local", "motion", "robust"):
+            for other in timers:
+                if other not in started:  # a chain's timer is unset until its own first call
+                    with pytest.raises(_lib.B200Error):
+                        timers[other]()
+            runs[name]()
+            started.add(name)
+        for name in runs:
+            read = timers[name]()
+            assert len(read) == 7
+            for other in runs:
+                if other != name:
+                    runs[other]()
+            assert timers[name]() == read, name
+
+
+def test_chain_parameter_checks(chains):
+    c = chains
+    ex = c["ex"]
+    with _matcher_handle():
+        for grid in ((0, 48), (64, 0)):
+            with pytest.raises(_lib.B200Error):
+                tracking.local_map_tracker(ex, KITTI, grid=grid).track(c["local"][:1])
+            with pytest.raises(_lib.B200Error):
+                tracking.frame_tracker(ex, KITTI, grid=grid).motion_based_track(c["motion"][:1])
+        # the robust chain runs no guided search: it reads neither the grid nor max_candidates
+        free = tracking.frame_tracker(ex, KITTI, grid=(0, 0), max_candidates=-1, use_fixed_seed=True)
+        _same(free.robust_match_based_track(_robust_frames(c, 2)), c["ft"].robust_match_based_track(_robust_frames(c, 2)))
+        with pytest.raises(_lib.B200Error):
+            tracking.frame_tracker(ex, KITTI, true_baseline=float("nan")).motion_based_track(c["motion"][:1])
+        nan_ratio = tracking.frame_tracker(ex, KITTI, use_fixed_seed=True)
+        nan_ratio._prm.lowe_ratio = float("nan")
+        with pytest.raises(_lib.B200Error):
+            nan_ratio.robust_match_based_track(_robust_frames(c, 1))
+        _same(nan_ratio.motion_based_track(c["motion"][:2]), c["ft"].motion_based_track(c["motion"][:2]))  # the motion chain does not read it
