@@ -947,6 +947,75 @@ typedef struct b200_twoview_problem {
  * keypoints or a min_sets entry outside [0, n_matches) of a problem that runs RANSAC. */
 int b200_twoview_ransac(b200_lba_t h, int n_problems, b200_twoview_problem_t* problems);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Monocular initialisation: initialize::perspective::initialize (src/stella_vslam/initialize/perspective.cc) and
+ * initialize::bearing_vector::initialize (bearing_vector.cc) for many frame pairs in one launch sequence on the b200_lba_t handle's
+ * stream: the H and F RANSAC of b200_twoview_ransac (perspective, fisheye, radial division) or the E RANSAC of b200_essential_ransac
+ * (equirectangular), all with recompute = false; the rel_cost_H choice; homography_solver::decompose (8 hypotheses) or the
+ * essential_solver::decompose of E = K2^T F K1 or of E (4 hypotheses); base::triangulate with the midpoint triangulation for every
+ * hypothesis; base::find_most_plausible_pose.  Float exactly where the reference stores float, fp64 elsewhere, in the CPU
+ * restatement's evaluation order (csrc/initialize_core.h).  Deviations (DESIGN.md section 8): sums run left to right; Jacobi sweeps
+ * are bounded and set status; points that are not triangulated are zeros (the reference leaves them uninitialised); a point behind
+ * a camera whose parallax is small is scored with its projection (the reference reads an unset pixel there).
+ * ---------------------------------------------------------------------------------------------------------------- */
+#define B200_INIT_MODEL_NONE 0
+#define B200_INIT_MODEL_H 1
+#define B200_INIT_MODEL_F 2
+#define B200_INIT_MODEL_E 3
+/* Where an attempt stopped.  NO_MODEL and DECOMPOSE leave rot / trans untouched; the rejections of find_most_plausible_pose zero them
+ * (base.cc:59-60), as the reference does. */
+#define B200_INIT_STAGE_NO_MODEL 0          /* neither RANSAC gave a usable model */
+#define B200_INIT_STAGE_DECOMPOSE 1         /* homography_solver::decompose's rank test failed */
+#define B200_INIT_STAGE_MIN_VALID 2         /* the largest nums_valid is below min_num_valid_pts */
+#define B200_INIT_STAGE_AMBIGUOUS 3         /* more than one hypothesis has 0.8 * max < nums_valid */
+#define B200_INIT_STAGE_PARALLAX 4          /* the winner's parallax_cos exceeds cos(parallax_deg_thr) */
+#define B200_INIT_STAGE_MIN_TRIANGULATED 5  /* the winner triangulated fewer than min_num_triangulated points */
+#define B200_INIT_STAGE_SUCCEEDED 6
+typedef struct b200_init_problem {
+    b200_camera_intrinsics_t cam_ref, cam_cur; /* models 0, 2, 3: perspective path (K = fx fy cx cy); 1 (both views): bearing_vector */
+    float img_bounds_ref[4], img_bounds_cur[4]; /* min_x, max_x, min_y, max_y (unused by model 1) */
+    int32_t n_ref, n_cur;                       /* keypoints of each frame */
+    const float* undist_ref;                    /* n_ref x 2: frm_obs_.undist_keypts_[i].pt */
+    const double* bearings_ref;                 /* n_ref x 3: frm_obs_.bearings_ */
+    const float* undist_cur;                    /* n_cur x 2 */
+    const double* bearings_cur;                 /* n_cur x 3 */
+    const int32_t* ref_matches_with_cur;        /* n_ref: the current keypoint matched to ref keypoint i, negative for none */
+    uint32_t num_ransac_iters;                  /* default 100 (module/initializer.cc) */
+    uint32_t min_num_triangulated;              /* default 50 */
+    uint32_t min_num_valid_pts;                 /* default 50 */
+    float parallax_deg_thr;                     /* default 1.0; cos(parallax_deg_thr / 180 * pi) is taken in double on the host */
+    float reproj_err_thr;                       /* default 4.0 */
+    /* minimal sets of util::create_random_array in draw order (b200_draw_min_sets), each drawn from its solver's own engine; needed
+     * only by a problem whose RANSAC runs (8 or more matches on the perspective path, 5 or more on the bearing-vector path) */
+    const int32_t* min_sets_H;                  /* num_ransac_iters x 4 (perspective path) */
+    const int32_t* min_sets_F;                  /* num_ransac_iters x 8 (perspective path) */
+    const int32_t* min_sets_E;                  /* num_ransac_iters x 5 (bearing-vector path) */
+    /* out */
+    int32_t status;                             /* B200_OK, or B200_ERR_INVALID when a RealSchur or a Jacobi SVD did not converge */
+    int32_t succeeded;                          /* initialize()'s return value */
+    int32_t model;                              /* B200_INIT_MODEL_*: the model reconstructed with (NONE when no model was usable) */
+    int32_t stage;                              /* B200_INIT_STAGE_* */
+    int32_t n_matches;                          /* ref_cur_matches_.size() */
+    float cost_H, cost_F, cost_E;               /* get_best_cost() of each solver that was constructed (0 otherwise) */
+    int32_t valid_H, valid_F, valid_E;          /* solution_is_valid() */
+    int32_t num_inliers_H, num_inliers_F, num_inliers_E;
+    int32_t n_hypotheses;                       /* 8 (H), 4 (F, E); 0 when find_most_plausible_pose did not run */
+    int32_t nums_valid[8];                      /* per hypothesis: base::triangulate's return value */
+    int32_t num_triangulated[8];
+    float parallax_cos[8];
+    double rot_ref_to_cur[9];                   /* row-major get_rotation_ref_to_cur(); see the stages above */
+    double trans_ref_to_cur[3];
+    double* triangulated_pts;                   /* n_ref x 3, written when succeeded: get_triangulated_pts() */
+    uint8_t* triangulated_flags;                /* n_ref, written when succeeded: get_triangulated_flags() */
+    uint8_t* inlier_flags;                      /* NULL or n_ref entries: the chosen solver's get_inlier_matches() in its first n_matches,
+                                                   written when a model was chosen */
+} b200_init_problem_t;
+/* initialize(cur_frm, ref_matches_with_cur) for every problem: one upload, the RANSAC launches, the model choice and decomposition,
+ * the triangulation of every hypothesis and the selection, one download.  B200_ERR_INVALID (nothing written) for a null handle or
+ * required pointer, a negative count, a camera model outside 0-3, model 1 on one view only, non-finite intrinsics of models 2 and 3, a
+ * match index at or above n_cur, num_ransac_iters above INT_MAX or a minimal-set index outside [0, n_matches). */
+int b200_initialize(b200_lba_t h, int n_problems, b200_init_problem_t* problems);
+
 /* ----------------------------------------------------------------------------------------------------------------
  * Pose-graph optimisation (optimize::graph_optimizer, optimize/graph_optimizer.cc:254-302): the Sim3 essential graph of a loop
  * closure, g2o's Levenberg-Marquardt with numeric central-difference Jacobians (delta 1e-9) and the terminate action, on the handle's

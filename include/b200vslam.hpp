@@ -13,6 +13,7 @@
 //   b200::util::stereo_rectifier          <-> stella_vslam::util::stereo_rectifier          (util/stereo_rectifier.h:14-46)
 //   b200::solve::pnp_solver               <-> stella_vslam::solve::pnp_solver               (solve/pnp_solver.h:13-142)
 //   b200::solve::essential_solver         <-> stella_vslam::solve::essential_solver         (solve/essential_solver.h)
+//   b200::initialize::perspective / bearing_vector <-> stella_vslam::initialize::perspective / bearing_vector (initialize/*.h)
 //   b200::module::depth_landmarks         <-> the depth branches of module::keyframe_inserter and module::initializer
 #pragma once
 
@@ -913,4 +914,151 @@ private:
 };
 
 }  // namespace solve
+}  // namespace b200
+
+namespace b200 {
+namespace initialize {
+
+// One frame as the initialisers read it: the camera (b200_camera_intrinsics_t model codes), its image bounds (min_x, max_x, min_y,
+// max_y), every undistorted keypoint (n x 2) and bearing (n x 3).
+struct frame {
+    b200_camera_intrinsics_t camera{};
+    float img_bounds[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    std::vector<float> undist_keypts;
+    std::vector<double> bearings;
+};
+
+// initialize() for many frame pairs in one call (b200_initialize); the problems' out fields are filled
+inline void initialize_batch(b200_lba_t h, std::vector<b200_init_problem_t>& problems) {
+    check(b200_initialize(h, (int)problems.size(), problems.data()), "b200_initialize");
+}
+
+// initialize::base (initialize/base.h) with initialize() of perspective (models 0, 2, 3) or bearing_vector (model 1).  Each attempt
+// constructs its solvers' engines afresh (util::create_random_engine) and draws only for a RANSAC that runs; a Jacobi SVD or RealSchur
+// that hits its bound does not throw (the reference returns normally): status() then reports B200_ERR_INVALID.  R and t are left as
+// the reference leaves base's members: zeroed once find_most_plausible_pose has run and rejected, untouched when RANSAC or the
+// decomposition failed first.  The initialiser owns a b200_lba_t handle unless one is given.
+class base {
+public:
+    base(const frame& ref_frm, bool bearing, unsigned int num_ransac_iters, unsigned int min_num_triangulated, unsigned int min_num_valid_pts,
+         float parallax_deg_thr, float reproj_err_thr, bool use_fixed_seed, b200_lba_t handle)
+        : ref_(ref_frm), bearing_(bearing), num_ransac_iters_(num_ransac_iters), min_num_triangulated_(min_num_triangulated),
+          min_num_valid_pts_(min_num_valid_pts), parallax_deg_thr_(parallax_deg_thr), reproj_err_thr_(reproj_err_thr),
+          use_fixed_seed_(use_fixed_seed), h_(handle) {
+        if ((ref_.camera.model == 1) != bearing_)
+            throw std::invalid_argument(bearing_ ? "bearing_vector: needs an equirectangular camera" : "perspective: cannot get a camera matrix");
+        if (ref_.undist_keypts.size() / 2 != ref_.bearings.size() / 3) throw std::invalid_argument("initialize: one bearing per keypoint");
+    }
+    virtual ~base() {
+        if (own_) b200_lba_destroy(h_);
+    }
+    base(const base&) = delete;
+    base& operator=(const base&) = delete;
+
+    bool initialize(const frame& cur_frm, const std::vector<int>& ref_matches_with_cur) {
+        const size_t n_ref = ref_.undist_keypts.size() / 2;
+        if (ref_matches_with_cur.size() != n_ref) throw std::invalid_argument("initialize: one match entry per ref keypoint");
+        if (!h_) {
+            check(b200_lba_create(0, &h_), "b200_lba_create");
+            own_ = true;
+        }
+        uint32_t n = 0;
+        for (int m : ref_matches_with_cur) n += m >= 0;
+        std::vector<int32_t> sets_H, sets_F, sets_E;
+        b200_mt19937_t engine;
+        if (bearing_) {
+            if (n >= 5) {
+                solve::create_random_engine(engine, use_fixed_seed_);
+                sets_E = solve::draw_min_sets(engine, 5, n, num_ransac_iters_);
+            }
+        } else if (n >= 8) {
+            solve::create_random_engine(engine, use_fixed_seed_);
+            sets_H = solve::draw_min_sets(engine, 4, n, num_ransac_iters_);
+            solve::create_random_engine(engine, use_fixed_seed_);
+            sets_F = solve::draw_min_sets(engine, 8, n, num_ransac_iters_);
+        }
+        const std::vector<int32_t> matches(ref_matches_with_cur.begin(), ref_matches_with_cur.end());
+        std::vector<double> pts(3 * n_ref);
+        std::vector<uint8_t> flags(n_ref);
+        b200_init_problem_t P{};
+        P.cam_ref = ref_.camera;
+        P.cam_cur = cur_frm.camera;
+        for (int k = 0; k < 4; ++k) {
+            P.img_bounds_ref[k] = ref_.img_bounds[k];
+            P.img_bounds_cur[k] = cur_frm.img_bounds[k];
+        }
+        P.n_ref = (int32_t)n_ref;
+        P.n_cur = (int32_t)(cur_frm.undist_keypts.size() / 2);
+        P.undist_ref = ref_.undist_keypts.data();
+        P.bearings_ref = ref_.bearings.data();
+        P.undist_cur = cur_frm.undist_keypts.data();
+        P.bearings_cur = cur_frm.bearings.data();
+        P.ref_matches_with_cur = matches.data();
+        P.num_ransac_iters = num_ransac_iters_;
+        P.min_num_triangulated = min_num_triangulated_;
+        P.min_num_valid_pts = min_num_valid_pts_;
+        P.parallax_deg_thr = parallax_deg_thr_;
+        P.reproj_err_thr = reproj_err_thr_;
+        P.min_sets_H = sets_H.empty() ? nullptr : sets_H.data();
+        P.min_sets_F = sets_F.empty() ? nullptr : sets_F.data();
+        P.min_sets_E = sets_E.empty() ? nullptr : sets_E.data();
+        P.triangulated_pts = pts.data();
+        P.triangulated_flags = flags.data();
+        check(b200_initialize(h_, 1, &P), "b200_initialize");
+        status_ = P.status;
+        stage_ = P.stage;
+        model_ = P.model;
+        if (P.n_hypotheses > 0) {
+            for (int k = 0; k < 9; ++k) rot_ref_to_cur_[k] = P.rot_ref_to_cur[k];
+            for (int k = 0; k < 3; ++k) trans_ref_to_cur_[k] = P.trans_ref_to_cur[k];
+        }
+        if (P.succeeded) {
+            triangulated_pts_ = pts;
+            is_triangulated_.assign(flags.begin(), flags.end());
+        }
+        return P.succeeded != 0;
+    }
+
+    const double* get_rotation_ref_to_cur() const { return rot_ref_to_cur_; }  // row-major
+    const double* get_translation_ref_to_cur() const { return trans_ref_to_cur_; }
+    const std::vector<double>& get_triangulated_pts() const { return triangulated_pts_; }  // n_ref x 3
+    std::vector<bool> get_triangulated_flags() const { return is_triangulated_; }
+    int status() const { return status_; }
+    int stage() const { return stage_; }  // B200_INIT_STAGE_* of the last attempt
+    int model() const { return model_; }  // B200_INIT_MODEL_*
+
+private:
+    frame ref_;
+    bool bearing_;
+    unsigned int num_ransac_iters_, min_num_triangulated_, min_num_valid_pts_;
+    float parallax_deg_thr_, reproj_err_thr_;
+    bool use_fixed_seed_;
+    b200_lba_t h_ = nullptr;
+    bool own_ = false;
+    int status_ = B200_OK, stage_ = B200_INIT_STAGE_NO_MODEL, model_ = B200_INIT_MODEL_NONE;
+    double rot_ref_to_cur_[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};  // base.h: Mat33_t::Identity(), Vec3_t::Zero()
+    double trans_ref_to_cur_[3] = {0, 0, 0};
+    std::vector<double> triangulated_pts_;
+    std::vector<bool> is_triangulated_;
+};
+
+// initialize::perspective (initialize/perspective.h): H and F RANSAC and the reconstruction with the model rel_cost_H picks
+class perspective final : public base {
+public:
+    explicit perspective(const frame& ref_frm, unsigned int num_ransac_iters = 100, unsigned int min_num_triangulated = 50,
+                         unsigned int min_num_valid_pts = 50, float parallax_deg_thr = 1.0f, float reproj_err_thr = 4.0f, bool use_fixed_seed = false,
+                         b200_lba_t handle = nullptr)
+        : base(ref_frm, false, num_ransac_iters, min_num_triangulated, min_num_valid_pts, parallax_deg_thr, reproj_err_thr, use_fixed_seed, handle) {}
+};
+
+// initialize::bearing_vector (initialize/bearing_vector.h): E RANSAC and its reconstruction (equirectangular cameras)
+class bearing_vector final : public base {
+public:
+    explicit bearing_vector(const frame& ref_frm, unsigned int num_ransac_iters = 100, unsigned int min_num_triangulated = 50,
+                            unsigned int min_num_valid_pts = 50, float parallax_deg_thr = 1.0f, float reproj_err_thr = 4.0f,
+                            bool use_fixed_seed = false, b200_lba_t handle = nullptr)
+        : base(ref_frm, true, num_ransac_iters, min_num_triangulated, min_num_valid_pts, parallax_deg_thr, reproj_err_thr, use_fixed_seed, handle) {}
+};
+
+}  // namespace initialize
 }  // namespace b200

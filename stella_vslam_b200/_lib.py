@@ -162,7 +162,7 @@ SYMBOLS = [
     "b200_rectifier_create", "b200_rectifier_destroy", "b200_rectifier_set_stream", "b200_rectifier_maps", "b200_stereo_rectify",
     "b200_stereo_rectify_device",
     "b200_pnp_ransac", "b200_epnp_compute_pose", "b200_mt19937_seed", "b200_mt19937_next", "b200_pnp_draw_min_sets",
-    "b200_draw_min_sets", "b200_essential_ransac", "b200_twoview_ransac",
+    "b200_draw_min_sets", "b200_essential_ransac", "b200_twoview_ransac", "b200_initialize",
     "b200_graph_optimize", "b200_pgo_envelope", "b200_transform_optimize",
 ]
 

@@ -25,6 +25,8 @@ SOURCES = {
     "pnp_kernels.cu": [],
     "essential_kernels.cu": [],
     "twoview_kernels.cu": [],
+    # reproject_to_image (camera_model.cuh) is plain double arithmetic that must not be contracted, as in orb_kernels.cu
+    "initialize_kernels.cu": ["-fmad=false"],
     # the pose-graph Jacobian is a central difference at delta 1e-9: no contraction on either side, as in tests/pgo_oracle.c
     "pgo_kernels.cu": ["-fmad=false", "-Xcompiler", "-ffp-contract=off"],
     # the transform optimiser's Jacobian is the same central difference (tests/transform_oracle.c)

@@ -2,7 +2,7 @@
 // fundamental_solver.cc) on the device: find_via_ransac for many problems of either model in one launch sequence on the b200_lba_t
 // handle's stream.
 //
-// find_via_ransac is split in four launches:
+// find_via_ransac is split in four launches (enqueue_ransac, twoview_ransac.cuh):
 //   twoview_normalize_kernel   one CTA per (problem, frame): solve::normalize.  Thread 0 forms the float centroid and L1 deviation in
 //                              keypoint order (the sums are sequential in the reference) and the transform; every thread then
 //                              scales its keypoints;
@@ -25,6 +25,7 @@
 #include "epnp.cuh"
 #include "ransac_host.cuh"
 #include "staging.cuh"
+#include "twoview_ransac.cuh"
 #include "util_trig.cuh"  // util_cos, which essential_core.h (included below for its SVD pieces) calls in es_cos_angle_thr
 
 namespace b200 {
@@ -44,44 +45,6 @@ __device__ __forceinline__ float tv_fd(float a, float b) { return __fdiv_rn(a, b
 
 #include "essential_core.cuh"
 #include "twoview_core.h"
-
-constexpr int kMinRows = 8;  // both models return early below 8 matches (H: min_set_size * 2)
-
-struct ProblemDev {
-    int model;
-    int n;          // matches
-    int match_off;  // first match in the concatenated matches / flags
-    int n1, kp1_off, n2, kp2_off;
-    int set_size;   // 4 (H) or 8 (F)
-    int hyp_off;    // first iteration in the concatenated iterations
-    int ms_off;     // first entry in the concatenated minimal sets
-    int n_hyp;      // max_num_iter (0 on the early return)
-    int runs;       // 0: find_via_ransac returns before drawing (n < 8)
-    int recompute;
-    float sigma;
-};
-
-struct NormDev {
-    double T1[9];  // transform_1
-    double D2[9];  // transform_2.inverse() (H) or transform_2.transpose() (F)
-};
-
-struct HypDev {
-    double M[9];  // the denormalised estimate
-    int ok;       // 0: H's minimal set was degenerate (the iteration is skipped)
-    int status;   // ES_STATUS_SVD
-};
-
-struct ScoreDev {
-    float cost;
-    unsigned num_inliers;
-};
-
-struct ResultDev {
-    double M[9];
-    float best_cost;
-    int valid, best_iter, num_inliers, status;
-};
 
 __global__ void __launch_bounds__(128) twoview_normalize_kernel(const ProblemDev* __restrict__ probs, const float* __restrict__ kp1,
                                                                  const float* __restrict__ kp2, float* __restrict__ kn1,
@@ -216,6 +179,23 @@ __global__ void __launch_bounds__(64) twoview_select_kernel(int n_problems, cons
     results[q] = r;
 }
 
+int enqueue_ransac(cudaStream_t st, int n_problems, int n_hyp, const RansacDev& d) {
+    twoview_normalize_kernel<<<2 * n_problems, 128, 0, st>>>(d.probs, d.kp1, d.kp2, d.kn1, d.kn2, d.norms);
+    B200_CUDA(cudaGetLastError());
+    if (n_hyp > 0) {
+        // 32-thread blocks: one attempt's 100 iterations spread over 4 SMs rather than 1
+        twoview_hypothesis_kernel<<<b200::ceil_div(n_hyp, 32), 32, 0, st>>>(n_hyp, d.hyp_problem, d.probs, d.norms, d.kn1, d.kn2, d.matches,
+                                                                            d.min_sets, d.hyps);
+        B200_CUDA(cudaGetLastError());
+        twoview_score_kernel<<<b200::ceil_div(n_hyp, 4), 128, 0, st>>>(n_hyp, d.hyp_problem, d.probs, d.kp1, d.kp2, d.matches, d.hyps, d.scores);
+        B200_CUDA(cudaGetLastError());
+    }
+    twoview_select_kernel<<<b200::ceil_div(n_problems, 64), 64, 0, st>>>(n_problems, d.probs, d.norms, d.kp1, d.kp2, d.kn1, d.kn2, d.matches,
+                                                                        d.hyps, d.scores, d.idx, d.mat, d.flags, d.results);
+    B200_CUDA(cudaGetLastError());
+    return B200_OK;
+}
+
 }  // namespace twoview
 }  // namespace b200
 
@@ -288,29 +268,11 @@ int b200_twoview_ransac(b200_lba_t h, int n_problems, b200_twoview_problem_t* pr
         b200::stage_min_sets(q, P.min_sets, D.set_size, D.n_hyp, (size_t)D.ms_off, D.hyp_off, (int32_t*)(hb + o_ms), (int*)(hb + o_hp));
     }
     B200_CUDA(A->upload(in_bytes, st));
-    const ProblemDev* d_probs = (const ProblemDev*)(db + o_probs);
-    const float* d_k1 = (const float*)(db + o_k1);
-    const float* d_k2 = (const float*)(db + o_k2);
-    const int32_t* d_mt = (const int32_t*)(db + o_mt);
-    const int* d_hp = (const int*)(db + o_hp);
-    twoview_normalize_kernel<<<2 * n_problems, 128, 0, st>>>(d_probs, d_k1, d_k2, (float*)(db + o_n1), (float*)(db + o_n2),
-                                                              (NormDev*)(db + o_norm));
-    B200_CUDA(cudaGetLastError());
-    if (total_hyp > 0) {
-        // 32-thread blocks: one attempt's 100 iterations spread over 4 SMs rather than 1
-        twoview_hypothesis_kernel<<<b200::ceil_div((int)total_hyp, 32), 32, 0, st>>>(
-            (int)total_hyp, d_hp, d_probs, (const NormDev*)(db + o_norm), (const float*)(db + o_n1), (const float*)(db + o_n2), d_mt,
-            (const int32_t*)(db + o_ms), (HypDev*)(db + o_hyp));
-        B200_CUDA(cudaGetLastError());
-        twoview_score_kernel<<<b200::ceil_div((int)total_hyp, 4), 128, 0, st>>>((int)total_hyp, d_hp, d_probs, d_k1, d_k2, d_mt,
-                                                                                (const HypDev*)(db + o_hyp), (ScoreDev*)(db + o_sc));
-        B200_CUDA(cudaGetLastError());
-    }
-    twoview_select_kernel<<<b200::ceil_div(n_problems, 64), 64, 0, st>>>(
-        n_problems, d_probs, (const NormDev*)(db + o_norm), d_k1, d_k2, (const float*)(db + o_n1), (const float*)(db + o_n2), d_mt,
-        (const HypDev*)(db + o_hyp), (const ScoreDev*)(db + o_sc), (int32_t*)(db + o_idx), (double*)(db + o_mat), db + o_fl,
-        (ResultDev*)(db + o_res));
-    B200_CUDA(cudaGetLastError());
+    const RansacDev dev{(const ProblemDev*)(db + o_probs), (const float*)(db + o_k1), (const float*)(db + o_k2), (const int32_t*)(db + o_mt),
+                        (const int32_t*)(db + o_ms), (const int*)(db + o_hp), (float*)(db + o_n1), (float*)(db + o_n2), (NormDev*)(db + o_norm),
+                        (HypDev*)(db + o_hyp), (ScoreDev*)(db + o_sc), (int32_t*)(db + o_idx), (double*)(db + o_mat), db + o_fl,
+                        (ResultDev*)(db + o_res)};
+    if ((rc = enqueue_ransac(st, n_problems, (int)total_hyp, dev))) return rc;
     B200_CUDA(A->download(o_res, out_end, st));
     B200_CUDA(cudaStreamSynchronize(st));
     const ResultDev* res = reinterpret_cast<const ResultDev*>(hb + o_res);

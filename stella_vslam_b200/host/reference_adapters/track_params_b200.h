@@ -13,42 +13,47 @@
 
 namespace stella_vslam {
 
-inline void fill_track_params(const data::frame& curr_frm, b200_track_params_t& prm) {
-    const auto* cam = curr_frm.camera_;
-    // model codes of b200_camera_intrinsics_t: 0 perspective, 1 equirectangular, 2 fisheye, 3 radial division (the double members;
-    // the fisheye undistortion rounds them to float on the device as cv_cam_matrix_ / cv_dist_params_ do)
+// b200_camera_intrinsics_t and image bounds (min_x, max_x, min_y, max_y) of a camera, shared with the initialiser's adapter
+// (initialize_b200.cc).  Model codes: 0 perspective, 1 equirectangular, 2 fisheye, 3 radial division (the double members; the fisheye
+// undistortion rounds them to float on the device as cv_cam_matrix_ / cv_dist_params_ do).
+inline void fill_camera_intrinsics(const camera::base* cam, b200_camera_intrinsics_t& ci, float* img_bounds) {
     switch (cam->model_type_) {
         case camera::model_type_t::Perspective: {
             const auto* p = static_cast<const camera::perspective*>(cam);
-            prm.cam.model = 0;
-            prm.cam.fx = p->fx_; prm.cam.fy = p->fy_; prm.cam.cx = p->cx_; prm.cam.cy = p->cy_;
-            prm.cam.k1 = p->k1_; prm.cam.k2 = p->k2_; prm.cam.p1 = p->p1_; prm.cam.p2 = p->p2_; prm.cam.k3 = p->k3_;
+            ci.model = 0;
+            ci.fx = p->fx_; ci.fy = p->fy_; ci.cx = p->cx_; ci.cy = p->cy_;
+            ci.k1 = p->k1_; ci.k2 = p->k2_; ci.p1 = p->p1_; ci.p2 = p->p2_; ci.k3 = p->k3_;
             break;
         }
         case camera::model_type_t::Fisheye: {
             const auto* p = static_cast<const camera::fisheye*>(cam);
-            prm.cam.model = 2;
-            prm.cam.fx = p->fx_; prm.cam.fy = p->fy_; prm.cam.cx = p->cx_; prm.cam.cy = p->cy_;
-            prm.cam.k1 = p->k1_; prm.cam.k2 = p->k2_; prm.cam.k3 = p->k3_; prm.cam.k4 = p->k4_;
+            ci.model = 2;
+            ci.fx = p->fx_; ci.fy = p->fy_; ci.cx = p->cx_; ci.cy = p->cy_;
+            ci.k1 = p->k1_; ci.k2 = p->k2_; ci.k3 = p->k3_; ci.k4 = p->k4_;
             break;
         }
         case camera::model_type_t::RadialDivision: {
             const auto* p = static_cast<const camera::radial_division*>(cam);
-            prm.cam.model = 3;
-            prm.cam.fx = p->fx_; prm.cam.fy = p->fy_; prm.cam.cx = p->cx_; prm.cam.cy = p->cy_;
-            prm.cam.distortion = p->distortion_;
+            ci.model = 3;
+            ci.fx = p->fx_; ci.fy = p->fy_; ci.cx = p->cx_; ci.cy = p->cy_;
+            ci.distortion = p->distortion_;
             break;
         }
         default:
-            prm.cam.model = 1;  // equirectangular
+            ci.model = 1;  // equirectangular
             break;
     }
-    prm.cam.cols = cam->cols_;
-    prm.cam.rows = cam->rows_;
+    ci.cols = cam->cols_;
+    ci.rows = cam->rows_;
+    img_bounds[0] = cam->img_bounds_.min_x_; img_bounds[1] = cam->img_bounds_.max_x_;
+    img_bounds[2] = cam->img_bounds_.min_y_; img_bounds[3] = cam->img_bounds_.max_y_;
+}
+
+inline void fill_track_params(const data::frame& curr_frm, b200_track_params_t& prm) {
+    const auto* cam = curr_frm.camera_;
+    fill_camera_intrinsics(cam, prm.cam, prm.img_bounds);
     prm.focal_x_baseline = cam->focal_x_baseline_;
     prm.monocular = cam->setup_type_ == camera::setup_type_t::Monocular ? 1 : 0;
-    prm.img_bounds[0] = cam->img_bounds_.min_x_; prm.img_bounds[1] = cam->img_bounds_.max_x_;
-    prm.img_bounds[2] = cam->img_bounds_.min_y_; prm.img_bounds[3] = cam->img_bounds_.max_y_;
     prm.grid_cols = static_cast<int32_t>(curr_frm.frm_obs_.num_grid_cols_);
     prm.grid_rows = static_cast<int32_t>(curr_frm.frm_obs_.num_grid_rows_);
     const auto* op = curr_frm.orb_params_;
