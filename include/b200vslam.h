@@ -670,6 +670,54 @@ int b200_robust_match_based_track(b200_orb_t orb, b200_matcher_t matcher, b200_l
 int b200_robust_track_stage_ms(b200_matcher_t matcher, int stage, float* ms);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * BoW-match tracking on the device: module::frame_tracker::bow_match_based_track (module/frame_tracker.cc:61-95) with
+ * match::bow_tree(0.7, true)::match_frame_and_keyframe (match/bow_tree.cc:169-256) for `n_frames` independent frames in ONE launch
+ * sequence, reading the extractor's results in HBM:
+ *   undistortion of the frame's keypoints (the four camera models of b200_keypoints_undistort) and their angles
+ *   match_frame_and_keyframe: the reference keyframe is side 1 (its keypoints whose landmark exists and is not will_be_erased, kf_valid),
+ *     the frame side 2; a keyframe keypoint only sees frame keypoints of its own BoW node, a frame keypoint that already received a
+ *     landmark is skipped, the 30-degree orientation gate, best <= HAMMING_DIST_THR_LOW and lowe_ratio * second >= best (float).  The
+ *     same candidate pass and resolve as b200_match_pairs variant B200_PAIRS_BOW, bit for bit.
+ *   applied = n_matches >= num_matches_thr (:69-72)
+ *   when applied: set_landmarks (a matched frame keypoint takes the keyframe keypoint's landmark, every other keypoint none), the pose
+ *     last_pose_cw, pose_optimizer::optimize (the < 5 observations early return included), then discard_outliers (:133-150): an outlier
+ *     keypoint loses its landmark; tracked = n_valid >= num_matches_thr.
+ * The BoW vectors stay on the host (curr_frm_.compute_bow, tracking_module.cc:343-345); the chain takes one node id per keypoint on both
+ * sides: the key of bow_feat_vec_ that lists the keypoint, or -1 when no node lists it (such a keypoint takes no part).
+ * prm: b200_track_params_t with lowe_ratio = 0.7 (bow_tree(0.7, true)), the camera, levels, the optimiser's trials and max_candidates
+ * (the gated candidates one keyframe keypoint keeps, 0 = 64 as in b200_match_pairs); margin, hamming_thr, grid, ray_cos_thr and
+ * log_scale_factor are not used.
+ * When applied is 0 the reference returns before it touches the frame: kp_landmark_out and pose_cw_out are not written, n_valid and
+ * tracked are 0.  B200_ERR_INVALID, with nothing written, for bad parameters, a null required pointer, an n_keypoints_in that
+ * disagrees with the extractor's count or a kp_cap below it; B200_ERR_CAPACITY, with nothing written, when a keyframe keypoint has more
+ * gated candidates than max_candidates.  One upload, one download and one stream synchronise per call. */
+typedef struct b200_bow_track_frame {
+    int32_t frame;                      /* index into the extractor's last batch */
+    const double* last_pose_cw;         /* 16, row-major: last_frm.get_pose_cw(), the optimisation's initial pose (:78) */
+    int32_t n_keypoints_in;             /* entries of kp_node and kp_x_right; must equal the frame's keypoint count */
+    const int32_t* kp_node;             /* BoW node of every frame keypoint (the key of bow_feat_vec_ that lists it), -1 = none */
+    const float* kp_x_right;            /* stereo_x_right_ of the current frame, NULL = monocular */
+    int32_t n_kf_keypoints;             /* reference keyframe, in its keypoint order: */
+    const uint8_t* kf_desc;             /* 32 per keypoint: frm_obs_.descriptors_ */
+    const float* kf_angle;              /* undist_keypts_[i].angle */
+    const int32_t* kf_node;             /* BoW node of every keyframe keypoint, -1 = none */
+    const uint8_t* kf_valid;            /* 1 = the keypoint has a landmark that is not will_be_erased */
+    const double* kf_pos_w;             /* 3 per keypoint: its landmark's position (read for valid keypoints only) */
+    int32_t kp_cap;                     /* capacity of kp_landmark_out (>= the frame's keypoint count) */
+    int32_t* kp_landmark_out;           /* out when applied, per keypoint: the keyframe keypoint whose landmark it carries, -1 none */
+    double pose_cw_out[16];             /* out when applied */
+    int32_t n_keypoints, n_matches;     /* out; n_matches = match_frame_and_keyframe's return value */
+    int32_t applied;                    /* out: n_matches >= num_matches_thr */
+    uint32_t n_valid;                   /* out: discard_outliers' count */
+    int32_t tracked;                    /* out: bow_match_based_track's return value */
+} b200_bow_track_frame_t;
+int b200_bow_match_based_track(b200_orb_t orb, b200_matcher_t matcher, b200_lba_t opt, const b200_track_params_t* prm, uint32_t num_matches_thr,
+                               int n_frames, b200_bow_track_frame_t* frames);
+/* Device time of the last b200_bow_match_based_track, per stage: 0 undistort + angles, 1 candidate lists, 2 resolve, 3 gate + landmark
+ * table, 4 edge build, 5 pose optimisation + discard, 6 whole chain (CUDA events on the stream). */
+int b200_bow_track_stage_ms(b200_matcher_t matcher, int stage, float* ms);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * New landmarks of the mapping module: module::two_view_triangulator (src/stella_vslam/module/two_view_triangulator.{h,cc}, with
  * solve::triangulator::triangulate, solve/triangulator.h:77-90, and data::triangulate_stereo, data/common.cc:192-260) and the
  * numeric chain of mapping_module::create_new_landmarks after the baseline test (mapping_module.cc, triangulate_with_two_keyframes).

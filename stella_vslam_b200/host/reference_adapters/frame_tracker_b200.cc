@@ -23,6 +23,7 @@
 #include <stdexcept>
 
 #include "b200vslam.h"
+#include "pairs_gather_b200.h"
 #include "track_params_b200.h"
 
 namespace stella_vslam {
@@ -181,6 +182,84 @@ bool robust_match_based_track_b200(data::frame& curr_frm, const data::frame& las
     if (!f.applied) return false;  // :105-108: the frame is not touched
 
     // ---- write-back: set_landmarks (:111) with the landmarks that survived discard_outliers, then the optimised pose
+    std::vector<std::shared_ptr<data::landmark>> lms(num_keypts, nullptr);
+    for (unsigned int idx = 0; idx < num_keypts; ++idx)
+        if (kp_landmark_out[idx] >= 0) lms[idx] = keyfrm_lms.at(kp_landmark_out[idx]);
+    curr_frm.set_landmarks(lms);
+    Mat44_t out;
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) out(r, c) = f.pose_cw_out[4 * r + c];
+    curr_frm.set_pose_cw(out);
+    return f.tracked != 0;
+}
+
+// module::frame_tracker::bow_match_based_track (module/frame_tracker.cc:61-95) as one device call: bow_tree(0.7, true)::
+// match_frame_and_keyframe against the reference keyframe, the gate, set_landmarks, the pose optimisation from the last pose and
+// discard_outliers (b200_bow_match_based_track).  The BoW vectors stay on the host: only one node id per keypoint on each side, and the
+// keyframe's descriptors, angles and landmark positions go up; the frame's keypoints and descriptors are read where the GPU extractor
+// left them.
+// Call site (tracking_module::track_current_frame, tracking_module.cc:333-355, USE_B200), in place of the first fallback, after
+// curr_frm_.compute_bow(bow_vocab_) (:343-345):
+//     succeeded = frame_tracker_.bow_match_based_track(curr_frm_, last_frm_, curr_frm_.ref_keyfrm_);
+//         -> succeeded = bow_match_based_track_b200(curr_frm_, last_frm_, curr_frm_.ref_keyfrm_, extractor_left_, num_matches_thr);
+// Precondition as motion_based_track_b200, and both bow_feat_vec_ computed.  Returns what frame_tracker::bow_match_based_track returns;
+// curr_frm is left exactly as it was when the frame is not applied (fewer matches than num_matches_thr, :69-72).
+bool bow_match_based_track_b200(data::frame& curr_frm, const data::frame& last_frm, const std::shared_ptr<data::keyframe>& ref_keyfrm,
+                                const feature::orb_extractor* extractor, unsigned int num_matches_thr) {
+    const b200_orb_t orb = feature::b200_handle_of(extractor);
+    if (!orb) throw std::runtime_error("bow_match_based_track_b200: the extractor has not extracted a frame yet");
+    static thread_local b200_matcher_t matcher = nullptr;
+    static thread_local b200_lba_t opt = nullptr;
+    if (!matcher && b200_matcher_create(0, &matcher) != B200_OK) throw std::runtime_error(b200_last_error());
+    if (!opt && b200_lba_create(0, &opt) != B200_OK) throw std::runtime_error(b200_last_error());
+
+    // ---- the keyframe side, in keyframe keypoint order; the same landmark vector serves the write-back (bow_tree.cc:174, 247)
+    const auto keyfrm_lms = ref_keyfrm->get_landmarks();
+    const auto& kf_kps = ref_keyfrm->frm_obs_.undist_keypts_;
+    const unsigned int n_kf = kf_kps.size();
+    std::vector<float> kf_angle(n_kf);
+    std::vector<uint8_t> kf_valid(n_kf, 0);
+    std::vector<double> kf_pos(3 * (size_t)n_kf, 0.0);
+    for (unsigned int i = 0; i < n_kf; ++i) {
+        kf_angle[i] = kf_kps[i].angle;
+        const auto& lm = keyfrm_lms.at(i);
+        if (!lm || lm->will_be_erased()) continue;  // bow_tree.cc:192-199
+        kf_valid[i] = 1;
+        const Vec3_t p = lm->get_pos_in_world();
+        kf_pos[3 * i] = p(0); kf_pos[3 * i + 1] = p(1); kf_pos[3 * i + 2] = p(2);
+    }
+    const unsigned int num_keypts = curr_frm.frm_obs_.undist_keypts_.size();
+    const auto kf_node = b200_gather::node_of(ref_keyfrm->bow_feat_vec_, n_kf);
+    const auto kp_node = b200_gather::node_of(curr_frm.bow_feat_vec_, num_keypts);
+
+    b200_track_params_t prm{};
+    fill_track_params(curr_frm, prm);
+    prm.lowe_ratio = 0.7f;  // match::bow_tree bow_matcher(0.7, true) (:62)
+
+    const Mat44_t last_pose_cw = last_frm.get_pose_cw();  // :78
+    double last_pose[16];
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) last_pose[4 * r + c] = last_pose_cw(r, c);
+    std::vector<int32_t> kp_landmark_out(num_keypts + 1, -1);
+    b200_bow_track_frame_t f{};
+    f.frame = 0;
+    f.last_pose_cw = last_pose;
+    f.n_keypoints_in = static_cast<int32_t>(num_keypts);
+    f.kp_node = kp_node.data();
+    const bool stereo = !curr_frm.frm_obs_.stereo_x_right_.empty();
+    f.kp_x_right = stereo ? curr_frm.frm_obs_.stereo_x_right_.data() : nullptr;
+    f.n_kf_keypoints = static_cast<int32_t>(n_kf);
+    f.kf_desc = ref_keyfrm->frm_obs_.descriptors_.ptr<uint8_t>();
+    f.kf_angle = kf_angle.data();
+    f.kf_node = kf_node.data();
+    f.kf_valid = kf_valid.data();
+    f.kf_pos_w = kf_pos.data();
+    f.kp_cap = static_cast<int32_t>(num_keypts);
+    f.kp_landmark_out = kp_landmark_out.data();
+    if (b200_bow_match_based_track(orb, matcher, opt, &prm, num_matches_thr, 1, &f) != B200_OK) throw std::runtime_error(b200_last_error());
+    if (!f.applied) return false;  // :69-72: the frame is not touched
+
+    // ---- write-back: set_landmarks (:75) with the landmarks that survived discard_outliers, then the optimised pose
     std::vector<std::shared_ptr<data::landmark>> lms(num_keypts, nullptr);
     for (unsigned int idx = 0; idx < num_keypts; ++idx)
         if (kp_landmark_out[idx] >= 0) lms[idx] = keyfrm_lms.at(kp_landmark_out[idx]);

@@ -1,0 +1,72 @@
+"""The C++ mirror of BoW-match tracking (include/b200vslam.hpp: tracking::frame_tracker::bow_match_based_track) drives the same frames
+as the Python mirror (stella_vslam_b200.tracking.frame_tracker) and gets the same results, bit for bit."""
+import os
+import subprocess
+
+import numpy as np
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+KITTI = dict(model="perspective", fx=718.856, fy=718.856, cx=607.1928, cy=185.2157, fxb=386.1448, cols=1241.0, rows=376.0, setup="stereo")
+
+
+@pytest.fixture(scope="module")
+def exe(tmp_path_factory):
+    from stella_vslam_b200 import build as builder
+    lib = builder.build()
+    out = str(tmp_path_factory.mktemp("bow_track_api") / "bow_track_api_test")
+    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-I", os.path.join(ROOT, "include"),
+                           os.path.join(ROOT, "tests", "cpp", "bow_track_api_test.cc"), "-o", out, lib, "-Wl,-rpath," + os.path.dirname(lib), "-ldl",
+                           "-lpthread", "-lrt"])
+    return out
+
+
+def test_cpp_mirror_builds_and_reports_usage(exe):
+    assert subprocess.run([exe], capture_output=True).returncode == 2
+
+
+def _hex(a):
+    a = np.ascontiguousarray(a)
+    return " ".join(b.tobytes().hex() for b in np.frombuffer(a.tobytes(), np.uint8).reshape(-1, a.dtype.itemsize))
+
+
+@pytest.mark.gpu
+def test_cpp_bow_track_matches_python(exe, tmp_path):
+    from stella_vslam_b200 import feature, tracking
+    from workloads import synth
+    n, w, h = 3, 1241, 376
+    gray = np.stack([synth.make_frame(w, h, seed=50 + i) for i in range(n)])
+    ex = feature.orb_extractor(feature.orb_params(), 800, max_batch=n)
+    kps, descs = ex.extract_batch(gray)
+    short = synth.make_bow_frame(kps[1], descs[1], KITTI, seed=72, stereo=True)
+    short = dict(short, keyframe={k: np.asarray(v)[:6] for k, v in short["keyframe"].items()})
+    frames = [dict(synth.make_bow_frame(kps[0], descs[0], KITTI, seed=70, stereo=True), frame=0),
+              dict(synth.make_bow_frame(kps[2], descs[2], KITTI, seed=71), frame=2, kp_x_right=None),
+              dict(short, frame=1)]
+    tr = tracking.frame_tracker(ex, KITTI)
+    want = tr.bow_match_based_track(frames)
+    path = tmp_path / "bow.bin"
+    with open(path, "wb") as f:
+        f.write(np.array([n, w, h], np.int32).tobytes() + gray.tobytes())
+        f.write(np.array([0, 0], np.int32).tobytes())
+        f.write(np.array([KITTI[k] for k in ("fx", "fy", "cx", "cy", "fxb", "cols", "rows")], np.float64).tobytes())
+        f.write(np.array([tr.num_matches_thr], np.uint32).tobytes())
+        for fr in frames:
+            kf = fr["keyframe"]
+            stereo = fr.get("kp_x_right") is not None
+            f.write(np.array([fr["frame"], len(fr["kp_node"]), int(stereo), len(kf["desc"])], np.int32).tobytes())
+            f.write(np.ascontiguousarray(fr["last_pose_cw"], np.float64).tobytes() + np.ascontiguousarray(fr["kp_node"], np.int32).tobytes())
+            if stereo:
+                f.write(np.ascontiguousarray(fr["kp_x_right"], np.float32).tobytes())
+            f.write(np.ascontiguousarray(kf["desc"], np.uint8).tobytes() + np.ascontiguousarray(kf["angle"], np.float32).tobytes())
+            f.write(np.ascontiguousarray(kf["node"], np.int32).tobytes() + np.ascontiguousarray(kf["valid"], np.uint8).tobytes())
+            f.write(np.ascontiguousarray(kf["pos_w"], np.float64).tobytes())
+    lines = subprocess.check_output([exe, "track", str(path)], text=True).splitlines()
+    for i, g in enumerate(want):
+        head, kp, pose = lines[3 * i:3 * i + 3]
+        assert head == f"frame {g['n_keypoints']} {g['n_matches']} {int(g['applied'])} {g['n_valid']} {int(g['tracked'])}"
+        if g["applied"]:
+            assert kp == ("kp " + _hex(g["kp_landmark"])).rstrip()
+            assert pose == "pose " + _hex(g["pose_cw"].reshape(16))
+    assert lines[3 * n] == "chain_ms_positive 1"
+    assert want[0]["tracked"] and want[1]["tracked"] and not want[2]["applied"]

@@ -717,6 +717,59 @@ def make_robust_frame(kps, desc, camera, seed=0, stereo=False, landmark_frac=0.6
                 keyframe=dict(desc=desc_all[perm], angle=ang_all[perm], bearings=bear_all[perm], valid=valid[perm], pos_w=pos_all))
 
 
+def _hamming_rows(a, b, chunk=256):
+    """Hamming distances (len(a), len(b)) between two sets of 32-byte descriptors."""
+    out = np.empty((len(a), len(b)), np.int32)
+    for s in range(0, len(a), chunk):
+        out[s:s + chunk] = np.bitwise_count(a[s:s + chunk, None, :] ^ b[None, :, :]).sum(-1)
+    return out
+
+
+def make_bow_frame(kps, desc, camera, seed=0, stereo=False, n_nodes=64, split_frac=0.1, lookalike_frac=0.1, unnoded_frac=0.05, kf_unnoded_frac=0.02,
+                   **robust_kw):
+    """The reference keyframe of frame_tracker::bow_match_based_track: make_robust_frame(kps, desc, camera, seed, stereo, **robust_kw) plus
+    the BoW node of every keypoint on both sides (kp_node, keyframe["node"]; -1 = no node lists the keypoint), drawn from a stream of
+    its own.  A keyframe keypoint built from a frame keypoint (its descriptor within max_flips bits) shares that keypoint's node, except
+    a `split_frac` share that lands in another node.  A `lookalike_frac` share of them gets a look-alike: the frame keypoint nearest to
+    its source moves into the same node and the keyframe descriptor moves towards it until the best distance is <= 50 but fails the
+    0.7 ratio test.  `unnoded_frac` of the frame's keypoints and `kf_unnoded_frac` of the keyframe's are in no node.  n_nodes = 1 puts
+    every listed keypoint into one node (all pairs meet)."""
+    fr = make_robust_frame(kps, desc, camera, seed=seed, stereo=stereo, **robust_kw)
+    rng = np.random.default_rng([int(seed), 0xB0])
+    desc = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32)
+    kf = fr["keyframe"]
+    kdesc = np.array(kf["desc"], np.uint8)
+    n_kp, n_kf = len(desc), len(kdesc)
+    d = _hamming_rows(kdesc, desc) if n_kp else np.zeros((n_kf, 0), np.int32)
+    src = d.argmin(1) if n_kp else np.full(n_kf, -1)
+    true = (d.min(1) <= robust_kw.get("max_flips", 20)) if n_kp else np.zeros(n_kf, bool)
+    kp_node = rng.integers(0, n_nodes, n_kp).astype(np.int32)
+    share = true & (rng.random(n_kf) >= split_frac)
+    look = share & (rng.random(n_kf) < lookalike_frac)
+    for j in np.nonzero(look)[0]:
+        a = src[j]
+        da = np.bitwise_count(desc ^ desc[a]).sum(-1)
+        da[a] = 1 << 20
+        b = int(da.argmin())
+        D = int(da[b])
+        k = int(np.floor(0.7 * D / 1.7)) + 1                     # 0.7 * (D - k) < k: the ratio test rejects; k <= 50 passes the threshold
+        if k > 50 or k > D:
+            continue
+        bits = np.nonzero(np.unpackbits(desc[a] ^ desc[b], bitorder="little"))[0]
+        x = np.unpackbits(desc[a], bitorder="little")
+        x[rng.choice(bits, k, replace=False)] ^= 1
+        kdesc[j] = np.packbits(x, bitorder="little")
+        kp_node[b] = kp_node[a]
+    knode = rng.integers(0, n_nodes, n_kf).astype(np.int32)
+    knode[share] = kp_node[src[share]]
+    split = true & ~share
+    if n_nodes > 1:
+        knode[split] = (kp_node[src[split]] + rng.integers(1, n_nodes, split.sum())) % n_nodes
+    kp_node[rng.random(n_kp) < unnoded_frac] = -1
+    knode[rng.random(n_kf) < kf_unnoded_frac] = -1
+    return dict(fr, kp_node=kp_node, keyframe=dict(kf, desc=kdesc, node=knode))
+
+
 def make_mapping_problem(seed, n_neighbours=10, n_keypoints=2000, model="perspective", stereo=False, num_levels=8, scale_factor=1.2):
     """A current keyframe and `n_neighbours` ordered covisibilities for the mapping module's landmark creation
     (mapping_module::create_new_landmarks, two_view_triangulator).  Returns (cur, neighbours): keyframe dicts in the shape of
