@@ -512,7 +512,9 @@ int b200_global_ba_solve(b200_lba_t h, const b200_lba_problem_t* problem, int nu
  * defaults num_trials_robust = 2, num_trials = 2, num_each_iter = 10, pose_optimizer_factory.h:18-47): motion-only bundle adjustment
  * of `n_problems` frames in one launch.  Each problem uses the b200_lba_problem_t layout with exactly ONE pose (free), the landmarks
  * the frame observes (all fixed) and one edge per observation (e_pose = 0; e_obs = undistorted x, y, x_right (< 0: monocular edge);
- * e_inv_sigma_sq = inv_level_sigma_sq_[octave]; e_delta = sqrt(chi-square), :84-88); one camera per problem.
+ * e_inv_sigma_sq = inv_level_sigma_sq_[octave]; e_delta = sqrt(chi-square), :84-88); one camera per problem: every edge must name
+ * the same camera (e_cam uniform, any index below n_cams; NULL = camera 0), as the reference optimises one frame of one camera
+ * (:38-43).  A problem whose edges name different cameras is refused with B200_ERR_INVALID and nothing is written.
  * Out: pose_cw_out [n_problems][16] row-major (the input pose when a frame has fewer than 5 observations, :116-118),
  * outlier_flags = the problems' edges concatenated (outlier_flags.at(idx), :141-160), n_valid[p] = num_init_obs - num_bad_obs. */
 int b200_pose_optimize(b200_lba_t h, int n_problems, const b200_lba_problem_t* problems, int num_trials_robust, int num_trials,

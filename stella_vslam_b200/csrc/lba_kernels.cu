@@ -2728,11 +2728,18 @@ int b200_pose_optimize(b200_lba_t h, int n_problems, const b200_lba_problem_t* p
             b200::set_error("b200_pose_optimize: problem %d must hold exactly one pose, its observed landmarks and one edge per observation", p);
             return B200_ERR_INVALID;
         }
-        for (int e = 0; e < P.n_edges; ++e)
+        for (int e = 0; e < P.n_edges; ++e) {
             if (P.e_point[e] < 0 || P.e_point[e] >= P.n_points || (P.e_cam && P.e_cam[e] >= P.n_cams)) {
                 b200::set_error("b200_pose_optimize: edge %d of problem %d references an invalid landmark/camera", e, p);
                 return B200_ERR_INVALID;
             }
+            // one frame, one camera (pose_optimizer_g2o.cc:38-43): the kernel projects every edge with the camera of edge 0
+            if (P.e_cam && P.e_cam[e] != P.e_cam[0]) {
+                b200::set_error("b200_pose_optimize: problem %d names camera %d on edge 0 and camera %d on edge %d; a frame has one camera", p,
+                                (int)P.e_cam[0], (int)P.e_cam[e], e);
+                return B200_ERR_INVALID;
+            }
+        }
         total_edges += (size_t)P.n_edges;
     }
     if (total_edges > 0 && !outlier_flags) return B200_ERR_INVALID;
