@@ -246,9 +246,9 @@ static void edge_error(const sim3_t* m, const sim3_t* v1, const sim3_t* v2, doub
     const sim3_t r = s_mul(&c1, &iv2);
     s_log(&r, e);
 }
-/* BaseFixedSizedEdge::linearizeOplus for one vertex side: J (7x7 row-major, rows = error components) */
-static void edge_jacobian(const sim3_t* m, const sim3_t* v1, const sim3_t* v2, int side, int fix_scale, double* J) {
-    const double delta = 1e-9, scalar = 1 / (2 * delta);
+/* BaseFixedSizedEdge::linearizeOplus for one vertex side (g2o's delta is 1e-9): J (7x7 row-major, rows = error components) */
+static void edge_jacobian_at(const sim3_t* m, const sim3_t* v1, const sim3_t* v2, int side, int fix_scale, double delta, double* J) {
+    const double scalar = 1 / (2 * delta);
     for (int d = 0; d < 7; ++d) {
         double add[7] = {0, 0, 0, 0, 0, 0, 0}, ep[7], em[7];
         add[d] = delta;
@@ -259,6 +259,9 @@ static void edge_jacobian(const sim3_t* m, const sim3_t* v1, const sim3_t* v2, i
         if (side == 0) edge_error(m, &p, v2, em); else edge_error(m, v1, &p, em);
         for (int k = 0; k < 7; ++k) J[7 * k + d] = scalar * (ep[k] - em[k]);
     }
+}
+static void edge_jacobian(const sim3_t* m, const sim3_t* v1, const sim3_t* v2, int side, int fix_scale, double* J) {
+    edge_jacobian_at(m, v1, v2, side, fix_scale, 1e-9, J);
 }
 
 /* ---------------- exported Sim3 algebra (sim3_t = 8 doubles: q xyzw, t, s) ---------------- */
@@ -280,6 +283,38 @@ void orc_edge_error(const double* m, const double* v1, const double* v2, double*
 }
 void orc_edge_jacobian(const double* m, const double* v1, const double* v2, int side, int fix_scale, double* J) {
     edge_jacobian((const sim3_t*)m, (const sim3_t*)v1, (const sim3_t*)v2, side, fix_scale, J);
+}
+
+/* Every edge's error and both vertex Jacobians by a central difference at `delta` of order 2 (g2o's stencil: at delta 1e-9 bit-identical
+ * to edge_jacobian) or 4 ((8 (f(h) - f(-h)) - (f(2h) - f(-2h))) / 12h).  err: ne x 7; J: ne x 2 x 7 x 7 (rows = error components), the
+ * side of a fixed vertex left untouched. */
+void orc_graph_linearize(int ne, int fix_scale, const double* est, const uint8_t* fixed, const int32_t* e1, const int32_t* e2,
+                         const double* meas, double delta, int order, double* err, double* J) {
+    const sim3_t* E = (const sim3_t*)est;
+    for (int k = 0; k < ne; ++k) {
+        const sim3_t* m = (const sim3_t*)meas + k;
+        const sim3_t* v[2] = {&E[e1[k]], &E[e2[k]]};
+        edge_error(m, v[0], v[1], err + 7 * (size_t)k);
+        for (int s = 0; s < 2; ++s) {
+            if (fixed[s == 0 ? e1[k] : e2[k]]) continue;
+            double* Jo = J + (size_t)(2 * k + s) * 49;
+            if (order == 2) {
+                edge_jacobian_at(m, v[0], v[1], s, fix_scale, delta, Jo);
+                continue;
+            }
+            for (int d = 0; d < 7; ++d) {
+                double f[4][7];
+                const double st[4] = {delta, -delta, 2 * delta, -2 * delta};
+                for (int q = 0; q < 4; ++q) {
+                    double add[7] = {0, 0, 0, 0, 0, 0, 0};
+                    add[d] = st[q];
+                    const sim3_t p = s_oplus(v[s], add, fix_scale);
+                    if (s == 0) edge_error(m, &p, v[1], f[q]); else edge_error(m, v[0], &p, f[q]);
+                }
+                for (int r = 0; r < 7; ++r) Jo[7 * r + d] = (8 * (f[0][r] - f[1][r]) - (f[2][r] - f[3][r])) / (12 * delta);
+            }
+        }
+    }
 }
 
 /* ---------------- ordering and envelope ---------------- */

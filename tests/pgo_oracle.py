@@ -35,8 +35,9 @@ def lib():
         L.orc_edge_jacobian.argtypes = [vp, vp, vp, i32, i32, vp]
         L.orc_rcm.argtypes = [i32, vp, i32, vp, vp, vp, vp, C.POINTER(C.c_int64)]
         L.orc_graph_optimize.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, i32, vp, vp, i32, C.c_double, vp, vp, vp, vp]
+        L.orc_graph_linearize.argtypes = [i32, i32, vp, vp, vp, vp, vp, C.c_double, i32, vp, vp]
         for name in ("orc_sim3_exp", "orc_sim3_log", "orc_sim3_inverse", "orc_sim3_mul", "orc_sim3_map", "orc_sim3_from_rts", "orc_edge_error",
-                     "orc_edge_jacobian"):
+                     "orc_edge_jacobian", "orc_graph_linearize"):
             getattr(L, name).restype = None
         _lib = L
     return _lib
@@ -95,6 +96,19 @@ def edge_jacobian(meas, v1, v2, side, fix_scale=False):
     lib().orc_edge_jacobian(_d(meas, 8).ctypes.data, _d(v1, 8).ctypes.data, _d(v2, 8).ctypes.data, int(side), int(bool(fix_scale)),
                             out.ctypes.data)
     return out
+
+
+def graph_linearize(graph, delta=1e-9, order=2):
+    """Every edge's error (m,7) and both vertex Jacobians (m,2,7,7) by a central difference of `order` 2 (g2o's, bit-identical to
+    edge_jacobian at delta 1e-9) or 4 at step `delta`; the Jacobian of a fixed vertex is zero."""
+    est = _d(graph["estimate"], (-1, 8))
+    fixed = np.ascontiguousarray(graph["fixed"], np.uint8)
+    e1, e2 = np.ascontiguousarray(graph["e_v1"], np.int32), np.ascontiguousarray(graph["e_v2"], np.int32)
+    meas = _d(graph["e_meas"], (-1, 8))
+    err, J = np.zeros((len(e1), 7)), np.zeros((len(e1), 2, 7, 7))
+    lib().orc_graph_linearize(len(e1), int(bool(graph.get("fix_scale", False))), est.ctypes.data, fixed.ctypes.data, e1.ctypes.data,
+                              e2.ctypes.data, meas.ctypes.data, float(delta), int(order), err.ctypes.data, J.ctypes.data)
+    return err, J
 
 
 def rcm(graph):

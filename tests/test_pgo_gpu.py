@@ -52,8 +52,11 @@ def _identity_envelope(g):
     return int(((np.arange(nt) - ft + 1) * 1024).sum())
 
 
-# On the larger drifted graphs the device and the oracle do not agree to the global-BA tolerances, not even after one LM iteration
-# (DESIGN.md section 8 lists this as open), so these cases check the structure and that the solve converges.
+# On the larger drifted graphs the device and the oracle do not agree to the global-BA tolerances, not even after one LM iteration:
+# g2o's delta-1e-9 Jacobian carries rounding noise of up to 2e-4 of a block at these graphs' units (|t| of hundreds of metres), CUDA
+# libm and glibc round it differently, and kappa(H + lambda I) ~ 1e5 amplifies the difference.  Neither run is the answer; both are
+# judged against a high-precision reference system in tests/test_pgo_precision_gpu.py (backward error of the step, device within 10x
+# of the oracle).  Here the cases check the structure and that the solve converges.
 @pytest.mark.gpu
 @pytest.mark.parametrize("n,fix_scale,seed", [(500, False, 3), (2000, False, 5), (4000, True, 6), (4000, False, 7)])
 def test_large_graphs_converge(n, fix_scale, seed):
