@@ -7,18 +7,14 @@ first use into a temporary directory (the tree is never written).  Perspective a
   track_local_map(camera, ...)         the per-frame chain of pyoracle.track_local_map for all four models
 """
 import ctypes as C
-import hashlib
 import math
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 from oracle import pyoracle as O
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "camera_models_oracle.c")
+import cbuild
+
 MODELS = {"perspective": 0, "equirectangular": 1, "fisheye": 2, "radial_division": 3}
 SENTINEL = np.float32(-1000000.0)
 # example/tum_vi/TUM_VI_mono.yaml and example/aist/fisheye.yaml of the reference
@@ -32,15 +28,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        with open(SRC, "rb") as f:
-            digest = hashlib.sha1(f.read()).hexdigest()[:12]
-        so = os.path.join(tempfile.gettempdir(), f"b200_camera_models_oracle_{os.getuid()}_{digest}.so")
-        if not os.path.exists(so):
-            tmp = so + f".{os.getpid()}.tmp"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=gnu11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                                   "-o", tmp, SRC, "-lm"])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = cbuild.load("camera_models_oracle.c")
         vp, f32, f64, i32 = C.c_void_p, C.c_float, C.c_double, C.c_int
         L.cmo_fisheye_undistort.argtypes = [vp, i32, f32, f32, f32, f32, vp, vp]
         L.cmo_fisheye_undistort.restype = None

@@ -1,16 +1,11 @@
 """CPU restatement of solve::essential_solver (test infrastructure): loads tests/essential_oracle.c, compiled on first use into a temporary
 directory (the tree is never written)."""
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "essential_oracle.c")
-DEPS = [SRC, os.path.join(HERE, "pnp_oracle.c"), os.path.join(HERE, "..", "stella_vslam_b200", "csrc", "essential_core.h")]
+import cbuild
+
 _lib = None
 
 STATUS_SCHUR, STATUS_SVD, STATUS_WIDE_KER = 1, 2, 4
@@ -19,17 +14,7 @@ STATUS_SCHUR, STATUS_SVD, STATUS_WIDE_KER = 1, 2, 4
 def lib():
     global _lib
     if _lib is None:
-        h = hashlib.sha1()
-        for p in DEPS:
-            with open(p, "rb") as f:
-                h.update(f.read())
-        so = os.path.join(tempfile.gettempdir(), f"b200_essential_oracle_{os.getuid()}_{h.hexdigest()[:12]}.so")
-        if not os.path.exists(so):
-            tmp = so + f".{os.getpid()}.tmp"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=gnu11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                                   "-o", tmp, SRC, "-lm"])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = cbuild.load("essential_oracle.c")
         vp, i32 = C.c_void_p, C.c_int
         L.orc_nullspace5.argtypes = [vp, vp, vp, C.POINTER(i32)]
         L.orc_lu_kernel.argtypes = [i32, vp, vp]

@@ -7,21 +7,14 @@ composes it with the two-view and essential RANSAC oracles.
 Problems are the dicts of stella_vslam_b200.initialize.initialize_batch; results carry the same keys.
 """
 import ctypes as C
-import hashlib
 import math
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
+import cbuild
 import essential_oracle as EO
 import twoview_oracle as TO
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "initialize_oracle.c")
-CSRC = os.path.join(HERE, "..", "stella_vslam_b200", "csrc")
-DEPS = TO.DEPS + [SRC, os.path.join(HERE, "motion_track_oracle.c"), os.path.join(CSRC, "initialize_core.h")]
 _lib = None
 
 MODEL_NONE, MODEL_H, MODEL_F, MODEL_E = 0, 1, 2, 3
@@ -34,17 +27,7 @@ _MODEL_CODES = {"perspective": 0, "equirectangular": 1, "fisheye": 2, "radial_di
 def lib():
     global _lib
     if _lib is None:
-        h = hashlib.sha1()
-        for p in DEPS:
-            with open(p, "rb") as f:
-                h.update(f.read())
-        so = os.path.join(tempfile.gettempdir(), f"b200_initialize_oracle_{os.getuid()}_{h.hexdigest()[:12]}.so")
-        if not os.path.exists(so):
-            tmp = so + f".{os.getpid()}.tmp"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=gnu11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                                   "-o", tmp, SRC, os.path.join(HERE, "motion_track_oracle.c"), "-lm"])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = cbuild.load("initialize_oracle.c", "motion_track_oracle.c")
         vp, i32, u32 = C.c_void_p, C.c_int, C.c_uint32
         L.ino_choose_H.argtypes = [C.c_float, C.c_float, i32]
         L.ino_svd33.argtypes = [vp, vp, vp, vp]

@@ -2,12 +2,10 @@
 into a temporary directory (the tree is never written), and composes the chain of create_new_landmarks from oracle.pyoracle's
 match_for_triangulation restatement and the triangulation, with the row claims between neighbour ranks."""
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
+
+import cbuild
 
 
 class TriKeyframe(C.Structure):
@@ -64,23 +62,13 @@ def epipolar_geometry(cur, ngh):
     return E, e / np.linalg.norm(e), bool(valid)
 
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "mapping_oracle.c")
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        with open(SRC, "rb") as f:
-            tag = hashlib.sha1(f.read()).hexdigest()[:12]
-        so = os.path.join(tempfile.gettempdir(), f"b200_mapping_oracle_{os.getuid()}_{tag}.so")
-        if not os.path.exists(so):
-            tmp = so + f".{os.getpid()}.tmp"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O3", "-fPIC", "-std=c11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                                   "-o", tmp, SRC, "-lm"])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = cbuild.load("mapping_oracle.c")
         P = C.POINTER(TriKeyframe)
         L.orc_triangulate_pairs.argtypes = [P, P, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.orc_jacobi_svd4_null.argtypes = [C.c_void_p, C.c_void_p]

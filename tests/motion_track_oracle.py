@@ -7,34 +7,21 @@ use into a temporary directory (the tree is never written), and composes it with
                                               pose_optimize -> discard_outliers, stage by stage
 """
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 from oracle import pyoracle as O
 
 import camera_models_oracle as CMO
+import cbuild
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "motion_track_oracle.c")
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        with open(SRC, "rb") as f:
-            digest = hashlib.sha1(f.read()).hexdigest()[:12]
-        so = os.path.join(tempfile.gettempdir(), f"b200_motion_track_oracle_{os.getuid()}_{digest}.so")
-        if not os.path.exists(so):
-            tmp = so + f".{os.getpid()}.tmp"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=gnu11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                                   "-o", tmp, SRC, "-lm"])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = cbuild.load("motion_track_oracle.c")
         L.mto_reproject.argtypes = [C.c_int] + [C.c_double] * 7 + [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.mto_reproject.restype = None
         _lib = L

@@ -1,30 +1,18 @@
 """CPU restatement of solve::pnp_solver (test infrastructure): loads tests/pnp_oracle.c, compiled on first use into a temporary
 directory (the tree is never written)."""
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "pnp_oracle.c")
+import cbuild
+
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        with open(SRC, "rb") as f:
-            tag = hashlib.sha1(f.read()).hexdigest()[:12]
-        so = os.path.join(tempfile.gettempdir(), f"b200_pnp_oracle_{os.getuid()}_{tag}.so")
-        if not os.path.exists(so):
-            tmp = so + f".{os.getpid()}.tmp"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=gnu11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                                   "-o", tmp, SRC, "-lm"])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = cbuild.load("pnp_oracle.c")
         vp, i32, u32 = C.c_void_p, C.c_int, C.c_uint
         L.orc_svd_square.argtypes = [i32, vp, vp, vp, vp, vp]
         L.orc_svd_solve_6xk.argtypes = [i32, vp, vp, vp, vp]

@@ -2,30 +2,18 @@
 directory (the tree is never written).  Maps as cv::initUndistortRectifyMap / cv::fisheye::initUndistortRectifyMap build them (CV_32F),
 their fixed-point form and cv::remap INTER_LINEAR / BORDER_CONSTANT 0."""
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "rectify_oracle.c")
+import cbuild
+
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        with open(SRC, "rb") as f:
-            tag = hashlib.sha1(f.read()).hexdigest()[:12]
-        so = os.path.join(tempfile.gettempdir(), f"b200_rectify_oracle_{os.getuid()}_{tag}.so")
-        if not os.path.exists(so):
-            tmp = so + f".{os.getpid()}.tmp"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                                   "-o", tmp, SRC, "-lm"])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = cbuild.load("rectify_oracle.c")
         vp, sz, i32 = C.c_void_p, C.c_size_t, C.c_int
         L.orc_rect_map.argtypes = [i32, i32, i32, vp, vp, i32, vp, vp, vp, vp]
         L.orc_rect_fixed.argtypes = [sz, vp, vp, vp, vp]

@@ -6,17 +6,12 @@ first use into a temporary directory (the tree is never written).
   depth_landmarks(problem)                           keyframe_inserter (mode 0) / create_map_for_stereo (mode 1) with triangulate_stereo
 """
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 import camera_models_oracle as CM
+import cbuild
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "rgbd_oracle.c")
 DEPTH_TYPES = {np.dtype(np.uint16): 2, np.dtype(np.float32): 5}  # cv::Mat::type() codes
 # TUM RGB-D (fr1 / freiburg1 calibration of the reference's example/tum_rgbd configs), 640x480
 TUM_RGBD = dict(model="perspective", fx=517.306408, fy=516.469215, cx=318.643040, cy=255.313989, k1=0.262383, k2=-0.953104, p1=-0.005358,
@@ -29,15 +24,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        with open(SRC, "rb") as f:
-            digest = hashlib.sha1(f.read()).hexdigest()[:12]
-        so = os.path.join(tempfile.gettempdir(), f"b200_rgbd_oracle_{os.getuid()}_{digest}.so")
-        if not os.path.exists(so):
-            tmp = so + f".{os.getpid()}.tmp"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=gnu11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                                   "-o", tmp, SRC, "-lm"])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = cbuild.load("rgbd_oracle.c")
         vp, f32, f64, i32 = C.c_void_p, C.c_float, C.c_double, C.c_int
         L.rgo_depths.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, C.c_size_t, f64, f64, vp, vp]
         L.rgo_depths.restype = None

@@ -1,25 +1,17 @@
 """The C++ mirror of solve::essential_solver (include/b200vslam.hpp, b200::solve) drives the same problems as the Python mirror
 (stella_vslam_b200.solve) and gets the same minimal sets and the same RANSAC results, bit for bit."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import cbuild
 from workloads import synth
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
-    from stella_vslam_b200 import build as builder
-    lib = builder.build()
-    out = str(tmp_path_factory.mktemp("essential_api") / "essential_api_test")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-I", os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "essential_api_test.cc"), "-o", out, lib,
-                           "-Wl,-rpath," + os.path.dirname(lib), "-ldl", "-lpthread", "-lrt"])
-    return out
+    return cbuild.cpp_mirror("essential_api_test", tmp_path_factory.mktemp("essential_api"))
 
 
 @pytest.mark.parametrize("set_size", [5, 8])

@@ -1,24 +1,14 @@
 """The C++ mirror (include/b200vslam.hpp) compiles against the C ABI alone and honours the no-fallback contract."""
-import os
 import subprocess
 import sys
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _build(tmp_path):
-    from stella_vslam_b200 import build as builder
-    lib = builder.build()
-    exe = str(tmp_path / "host_api_test")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "host_api_test.cc"),
-                           "-o", exe, lib, "-Wl,-rpath," + os.path.dirname(lib), "-ldl", "-lpthread", "-lrt"])
-    return exe
+import cbuild
 
 
 def test_cpp_mirror_compiles_and_fails_loudly_without_gpu(tmp_path):
-    exe = _build(tmp_path)
+    exe = cbuild.cpp_mirror("host_api_test", tmp_path)
     r = subprocess.run([exe], capture_output=True, text=True)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "sm_90a" in r.stdout
@@ -26,7 +16,7 @@ def test_cpp_mirror_compiles_and_fails_loudly_without_gpu(tmp_path):
 
 @pytest.mark.gpu
 def test_cpp_mirror_runs_on_gpu(tmp_path):
-    exe = _build(tmp_path)
+    exe = cbuild.cpp_mirror("host_api_test", tmp_path)
     r = subprocess.run([exe], capture_output=True, text=True)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "keypoints" in r.stdout and "self matches" in r.stdout and "projection matches" in r.stdout and "stereo matches" in r.stdout and "tracking matches" in r.stdout

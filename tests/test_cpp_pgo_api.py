@@ -6,19 +6,13 @@ import subprocess
 import numpy as np
 import pytest
 
+import cbuild
 from workloads import synth
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
-    from stella_vslam_b200 import build as builder
-    lib = builder.build()
-    out = str(tmp_path_factory.mktemp("pgo_api") / "pgo_api_test")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "pgo_api_test.cc"),
-                           "-o", out, lib, "-Wl,-rpath," + os.path.dirname(lib), "-ldl", "-lpthread", "-lrt"])
-    return out
+    return cbuild.cpp_mirror("pgo_api_test", tmp_path_factory.mktemp("pgo_api"))
 
 
 def test_cpp_mirror_compiles(exe):

@@ -1,24 +1,19 @@
 """The C++ mirror of the RGB-D frame step and the depth-seeded landmarks (include/b200vslam.hpp: feature::orb_extractor::rgbd_depths,
 module::depth_landmarks) drives the same problems as the Python mirror and gets the same results, bit for bit."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import cbuild
+
 TUM_RGBD = dict(model=0, fx=517.306408, fy=516.469215, cx=318.643040, cy=255.313989, k1=0.262383, k2=-0.953104, p1=-0.005358, p2=0.002628,
                 k3=1.163314, cols=640.0, rows=480.0, k4=0.0, distortion=0.0)
 
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
-    from stella_vslam_b200 import build as builder
-    lib = builder.build()
-    out = str(tmp_path_factory.mktemp("rgbd_api") / "rgbd_api_test")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "rgbd_api_test.cc"),
-                           "-o", out, lib, "-Wl,-rpath," + os.path.dirname(lib), "-ldl", "-lpthread", "-lrt"])
-    return out
+    return cbuild.cpp_mirror("rgbd_api_test", tmp_path_factory.mktemp("rgbd_api"))
 
 
 def test_cpp_mirror_builds_and_reports_usage(exe):

@@ -1,24 +1,18 @@
 """The C++ mirror of robust-match tracking (include/b200vslam.hpp: tracking::frame_tracker::robust_match_based_track) drives the same frames
 as the Python mirror (stella_vslam_b200.tracking.frame_tracker) and gets the same results, bit for bit."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import cbuild
+
 KITTI = dict(model="perspective", fx=718.856, fy=718.856, cx=607.1928, cy=185.2157, fxb=386.1448, cols=1241.0, rows=376.0, setup="stereo")
 
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
-    from stella_vslam_b200 import build as builder
-    lib = builder.build()
-    out = str(tmp_path_factory.mktemp("robust_track_api") / "robust_track_api_test")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-I", os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "robust_track_api_test.cc"), "-o", out, lib, "-Wl,-rpath," + os.path.dirname(lib), "-ldl",
-                           "-lpthread", "-lrt"])
-    return out
+    return cbuild.cpp_mirror("robust_track_api_test", tmp_path_factory.mktemp("robust_track_api"))
 
 
 def test_cpp_mirror_builds_and_reports_usage(exe):

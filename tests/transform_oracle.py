@@ -2,33 +2,18 @@
 tests/pgo_oracle.c for the g2o::Sim3 algebra), compiled on first use into a temporary directory (the tree is never written).  Sim3s are
 8-vectors (q x y z w, t, s), as b200_sim3_t; a camera is a dict(model, fx, fy, cx, cy, cols, rows) as b200_camera_t."""
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "transform_oracle.c")
-DEPS = (SRC, os.path.join(HERE, "pgo_oracle.c"))
+import cbuild
+
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        h = hashlib.sha1()
-        for p in DEPS:
-            with open(p, "rb") as f:
-                h.update(f.read())
-        so = os.path.join(tempfile.gettempdir(), f"b200_transform_oracle_{os.getuid()}_{h.hexdigest()[:12]}.so")
-        if not os.path.exists(so):
-            tmp = so + f".{os.getpid()}.tmp"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=gnu11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                                   "-o", tmp, SRC, "-lm"])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = cbuild.load("transform_oracle.c")
         vp, i32 = C.c_void_p, C.c_int
         L.orc_transform_edge.argtypes = [vp, i32, vp, vp, vp, C.c_float, vp]
         L.orc_transform_edge.restype = C.c_double

@@ -1,17 +1,11 @@
 """CPU restatement of solve::homography_solver / fundamental_solver (test infrastructure): loads tests/twoview_oracle.c, compiled on
 first use into a temporary directory (the tree is never written)."""
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "twoview_oracle.c")
-CSRC = os.path.join(HERE, "..", "stella_vslam_b200", "csrc")
-DEPS = [SRC, os.path.join(HERE, "pnp_oracle.c"), os.path.join(CSRC, "essential_core.h"), os.path.join(CSRC, "twoview_core.h")]
+import cbuild
+
 _lib = None
 
 MODEL_H, MODEL_F = 0, 1
@@ -21,17 +15,7 @@ STATUS_SVD = 2
 def lib():
     global _lib
     if _lib is None:
-        h = hashlib.sha1()
-        for p in DEPS:
-            with open(p, "rb") as f:
-                h.update(f.read())
-        so = os.path.join(tempfile.gettempdir(), f"b200_twoview_oracle_{os.getuid()}_{h.hexdigest()[:12]}.so")
-        if not os.path.exists(so):
-            tmp = so + f".{os.getpid()}.tmp"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=gnu11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                                   "-o", tmp, SRC, "-lm"])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = cbuild.load("twoview_oracle.c")
         vp, i32 = C.c_void_p, C.c_int
         L.orc_normalize.argtypes = [i32, vp, vp, vp, vp, vp]
         L.orc_normalize.restype = None
