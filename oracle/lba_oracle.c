@@ -593,6 +593,44 @@ int orc_lba_solve(const orc_lba_problem_t* P, int iters1, int iters2, volatile u
     return 0;
 }
 
+/* What build_system uses for every edge at one state: the residual, the robust weight inv_sigma_sq * rho'(chi2) and both Jacobians,
+ * for the edges with level[e] == 0 (the others are left zero).  Test infrastructure: lets the tests check an independent restatement
+ * of the three edge models edge by edge.  pose_cw / points: the state (NULL: the problem's own); level: NULL = every edge active;
+ * robust: per-edge Huber switch (NULL: the problem's e_robust).  Returns the number of active edges. */
+int orc_lba_linearize(const orc_lba_problem_t* P, const double* pose_cw, const double* points, const uint8_t* level, const uint8_t* robust,
+                      double* err_out, double* weight_out, double* Ji_out, double* Jj_out) {
+    orc_lba_problem_t Q = *P;
+    if (pose_cw) Q.pose_cw = pose_cw;
+    if (points) Q.points = points;
+    lba_t S;
+    state_init(&S, &Q);
+    const int E = P->n_edges;
+    int n = 0;
+    for (int e = 0; e < E; ++e) {
+        if (level) S.level[e] = level[e];
+        if (robust) S.robust[e] = robust[e];
+    }
+    memset(err_out, 0, sizeof(double) * 3 * (size_t)E);
+    memset(weight_out, 0, sizeof(double) * (size_t)E);
+    memset(Ji_out, 0, sizeof(double) * 9 * (size_t)E);
+    memset(Jj_out, 0, sizeof(double) * 18 * (size_t)E);
+    compute_active_errors(&S);
+    for (int e = 0; e < E; ++e) {
+        if (S.level[e]) continue;
+        ++n;
+        edge_jacobians(&S, e, Ji_out + 9 * e, Jj_out + 18 * e);
+        double rho1 = 1.0; /* as build_system */
+        if (S.robust[e]) {
+            const double e2 = edge_chi2(&S, e), delta = (double)P->e_delta[e];
+            if (e2 > delta * delta) rho1 = delta / sqrt(e2);
+        }
+        weight_out[e] = (double)P->e_inv_sigma_sq[e] * rho1;
+        memcpy(err_out + 3 * e, S.err + 3 * e, sizeof(double) * 3);
+    }
+    state_free(&S);
+    return n;
+}
+
 /* optimize::global_bundle_adjuster (src/stella_vslam/optimize/global_bundle_adjuster.cc:26-192 optimize_impl, :258-420 optimize,
  * :201-256 optimize_for_initialization) on a flattened problem: the same vertices and reprojection edges as the local bundle adjuster
  * (every keyframe free except the spanning root, Huber on landmark edges when use_huber_kernel), ONE optimize(num_iter) with the

@@ -189,6 +189,12 @@ int orc_lba_solve(const orc_lba_problem_t* P, int iters1, int iters2, volatile u
                   double* points_out, uint8_t* outlier_out, orc_lba_stats_t* stats);
 int orc_global_ba_solve(const orc_lba_problem_t* P, int num_iter, double gain_threshold, volatile uint8_t* force_stop, double* pose_cw_out,
                         double* points_out, orc_lba_stats_t* stats);
+/* Test infrastructure: what build_system uses for every active edge at the state (pose_cw K x 16, points L x 3; NULL = the problem's):
+ * residual (E x 3), robust weight inv_sigma_sq * rho' (E), landmark Jacobian (E x 3x3) and pose Jacobian (E x 3x6, rotation first),
+ * rows past the edge's dimension and inactive edges (level[e] != 0) zero.  robust: per-edge Huber switch (NULL = P->e_robust).
+ * Returns the number of active edges. */
+int orc_lba_linearize(const orc_lba_problem_t* P, const double* pose_cw, const double* points, const uint8_t* level, const uint8_t* robust,
+                      double* err_out, double* weight_out, double* Ji_out, double* Jj_out);
 
 /* optimize::pose_optimizer_g2o::optimize (pose_optimizer_g2o.cc:38-175): motion-only BA of one frame.  P: one free pose, fixed
  * points, one edge per observation.  Returns the number of inlier observations; outlier_flags[e] per edge. */

@@ -399,6 +399,22 @@ def global_ba_solve(prob, num_iter=10, gain_threshold=1e-3, force_stop=None):
                 lambda_final=st.lambda_final[0])
 
 
+def lba_linearize(prob, pose_cw=None, points=None, level=None, robust=None):
+    """orc_lba_linearize: per edge the residual (E,3), robust weight (E,), landmark Jacobian (E,3,3) and pose Jacobian (E,3,6) that
+    the oracle's build_system uses at the state (pose_cw, points) -- default: the problem's -- with the edges of level != 0 left out
+    (all zero).  robust: per-edge Huber switch (default: the problem's e_robust).  Test infrastructure only."""
+    L_ = lib()
+    L_.orc_lba_linearize.argtypes = [C.POINTER(LbaProblem)] + [C.c_void_p] * 8
+    L_.orc_lba_linearize.restype = C.c_int
+    P, keep = pack_lba_problem(prob)
+    E = P.n_edges
+    args = [None if a is None else np.ascontiguousarray(a, dt) for a, dt in
+            ((pose_cw, np.float64), (points, np.float64), (level, np.uint8), (robust, np.uint8))]
+    err, w, Ji, Jj = np.zeros((E, 3)), np.zeros(E), np.zeros((E, 3, 3)), np.zeros((E, 3, 6))
+    n = L_.orc_lba_linearize(C.byref(P), *[_p(a) for a in args], _p(err), _p(w), _p(Ji), _p(Jj))
+    return dict(n_active=n, err=err, weight=w, Ji=Ji, Jj=Jj)
+
+
 def pose_optimize(prob, num_trials_robust=2, num_trials=2, num_each_iter=10):
     """orc_pose_optimize on a flattened frame (synth.make_pose_problem).  Returns (num_valid_obs, pose (4,4), outlier_flags bool)."""
     P, keep = pack_lba_problem(prob)

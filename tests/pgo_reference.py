@@ -13,6 +13,7 @@ import scipy.sparse as sp
 import scipy.sparse.linalg as spl
 
 import pgo_oracle as O
+from sparse_lm import backward_error, damped, exact_step, factor, kappa_bound, rel  # noqa: F401
 
 DELTA, STENCIL = 1e-4, 4
 
@@ -125,36 +126,6 @@ def step(graph, est_out, order, near=None):
     return x
 
 
-def damped(H, lam):
-    return (H + lam * sp.identity(H.shape[0], format="csc")).tocsc()
-
-
-def backward_error(A, x, b):
-    """Normwise backward error ||A x - b||_inf / (||A||_inf ||x||_inf + ||b||_inf)."""
-    r = A @ x - b
-    a_inf = abs(A).sum(axis=1).max()
-    return float(np.abs(r).max() / (a_inf * np.abs(x).max() + np.abs(b).max()))
-
-
-def factor(A):
-    """Sparse LU of A (minimum degree on A^T + A, the pattern being symmetric)."""
-    return spl.splu(A.tocsc(), permc_spec="MMD_AT_PLUS_A")
-
-
-def exact_step(A, b, lu=None):
-    """A^-1 b by a sparse LU and one step of iterative refinement."""
-    lu = lu or factor(A)
-    x = lu.solve(b)
-    return x + lu.solve(b - A @ x)
-
-
-def kappa_bound(A, lam):
-    """Upper bound on the 2-norm condition number of A = H + lam I, H positive semi-definite: ||A||_inf (>= its largest eigenvalue)
-    over lam (<= its smallest).  Lanczos takes minutes on these clustered spectra; on the 500-keyframe graph the bound is within a
-    factor 1.3 of eigsh's condition number (tests/test_pgo_precision_cpu.py)."""
-    return float(abs(A).sum(axis=1).max() / lam)
-
-
 def kappa(A):
     """2-norm condition number of the SPD matrix A by eigsh (largest, and smallest by shift-invert at 0): for small graphs."""
     hi = spl.eigsh(A, k=1, which="LA", return_eigenvectors=False, tol=1e-6)[0]
@@ -176,10 +147,6 @@ def gauss_newton(graph, est=None, tol=1e-10, max_iter=12):
         if np.abs(x).max() <= tol * max(1.0, np.abs(est[:, 4:7]).max()):
             break
     return est, system(dict(graph, estimate=est))["chi2"]
-
-
-def rel(x, y):
-    return float(np.linalg.norm(x - y) / np.linalg.norm(y))
 
 
 # The graphs the precision tests solve: the drifted loops of tests/test_pgo_gpu.py's large-graph cases (500 to 4 000 keyframes, free
