@@ -1,6 +1,8 @@
 """optimize::pose_optimizer oracle (oracle/lba_oracle.c: orc_pose_optimize, pose_optimizer_g2o.cc:38-175).  No reference test or
-golden exists (parity unpinned); the restatement shares the LM / edge code that tests/test_lba_cpu.py checks against an
-independent dense solver, so here: protocol properties and agreement with ground truth on synthetic frames."""
+golden exists; each LM step is pinned instead against the independent high-precision reference of tests/pose_reference.py (its
+lambda_init, the lambda of later steps, the classification between rounds and the re-posed later rounds:
+tests/test_pose_precision_cpu.py, and on the device tests/test_pose_precision_gpu.py).  Here: protocol properties and agreement
+with ground truth on synthetic frames."""
 import numpy as np
 import pytest
 
