@@ -1537,6 +1537,8 @@ struct ChainTimer {
             if (e) cudaEventDestroy(e);
     }
 };
+// The index of each chain's timer in Matcher::chain_timers
+enum ChainId { kLocalMapChain, kMotionChain, kRobustChain, kBowChain, kChains };
 
 struct Matcher {
     int device = 0;
@@ -1548,8 +1550,7 @@ struct Matcher {
     bool async_resolve = false, resolve_pending = false;
     bool timing = false;
     cudaEvent_t ev_t[3] = {nullptr, nullptr, nullptr};
-    ChainTimer track_timer, motion_timer, robust_timer;  // b200_track_local_map, b200_motion_based_track, b200_robust_match_based_track
-    ChainTimer bow_timer;                                // b200_bow_match_based_track
+    ChainTimer chain_timers[kChains];  // indexed by ChainId
     int join() {  // the main stream waits for the side stream's resolve
         if (resolve_pending) {
             B200_CUDA(cudaStreamWaitEvent(stream, ev_resolved, 0));
@@ -1647,20 +1648,15 @@ static int guided_resolve_smem(const char* who, int n, size_t* bytes) {
 }  // namespace match
 }  // namespace b200
 
+struct b200_matcher_s {
+    b200::match::Matcher m;
+};
+
 // The host scaffold of the tracking chains (b200_track_local_map, b200_motion_based_track, b200_robust_match_based_track,
 // b200_bow_match_based_track)
 namespace b200 {
 namespace chain {
 using match::GuidedDev;
-
-// The checks of b200_track_params_t that every chain makes; `extra` is the entry point's own
-static int check_params(const char* who, const b200_track_params_t& p, bool extra) {
-    if (p.scale_factors && p.inv_level_sigma_sq && p.num_levels != 0 && p.num_levels <= 32 && camera_valid(p.cam) && p.num_trials_robust >= 0
-        && p.num_trials >= 0 && p.num_each_iter >= 0 && extra)
-        return B200_OK;
-    set_error("%s: invalid parameters", who);
-    return B200_ERR_INVALID;
-}
 
 // The keypoint grid, image bounds and window bound of the chains that run the guided search
 static bool search_params_valid(const b200_track_params_t& p) {
@@ -1677,18 +1673,6 @@ struct Extracted {
     cudaStream_t st = nullptr;
 };
 
-static int open_extracted(const char* who, b200_orb_t orb, int device, Extracted* x) {
-    int orb_device = 0;
-    int rc = orb_results(orb, &x->kps, &x->descs, &x->counts, &x->stride, &x->batch, &x->st, &orb_device);
-    if (rc) return rc;
-    if (orb_device != device) {
-        set_error("%s: extractor and matcher live on different devices", who);
-        return B200_ERR_INVALID;
-    }
-    B200_CUDA(cudaSetDevice(device));
-    return B200_OK;
-}
-
 // Row-major 4x4 pose -> rot_cw row-major, then trans_cw
 static void rt_of(const double* P, double* Rt) {
     for (int r = 0; r < 3; ++r) {
@@ -1697,10 +1681,11 @@ static void rt_of(const double* P, double* Rt) {
     }
 }
 
-// The per-frame blocks every chain has: its kp_landmark_out and status outputs (taken by the chain among its outputs), stage A's
-// products (kout among the outputs when the chain downloads kp_outlier) and, in the chains that run the guided search, its
-// queries and scratch.
+// The per-frame blocks every chain has: its x_right and landmark-position inputs (taken by the chain among its inputs), its
+// kp_landmark_out and status outputs (taken by Call::begin_outputs), stage A's products (kout among the outputs when the chain
+// downloads kp_outlier) and, in the chains that run the guided search, its queries and scratch.
 struct FrameBlocks {
+    size_t xr = 0, pos = 0;  // taken by the chain among its inputs, staged by Call::frame_dev
     size_t klo, status, und, tx, ty, toct, occ, kout;
     bool guided = false;
     size_t qx, qy, qm, qxr, qlo, qhi, qval, cstart, citems, ccur, lists, llen, own;
@@ -1731,38 +1716,178 @@ struct FrameBlocks {
     }
 };
 
-// The fields of TrackFrameDev that every chain fills the same way.  x_right and pos_w are device pointers (x_right may be null).
-static TrackFrameDev frame_dev(const Extracted& x, int frame, int n_kp_in, int n_lm, const float* x_right, const double* pos_w,
-                               const double* pose_cw, const FrameBlocks& B, unsigned char* db) {
-    TrackFrameDev t{};
-    t.kps = x.kps + (size_t)frame * x.stride;
-    t.n_kp = x.counts + frame;
-    t.kp_cap = x.stride;
-    t.n_kp_in = n_kp_in;
-    t.n_lm = n_lm;
-    t.kp_x_right = x_right;
-    t.pos_w = pos_w;
-    rt_of(pose_cw, t.Rt);
-    for (int r = 0; r < 3; ++r) t.twc[r] = -(t.Rt[r] * t.Rt[9] + t.Rt[3 + r] * t.Rt[10] + t.Rt[6 + r] * t.Rt[11]);
-    t.undist = (b200_keypoint_t*)(db + B.und);
-    t.t_x = (float*)(db + B.tx);
-    t.t_y = (float*)(db + B.ty);
-    t.t_octave = db + B.toct;
-    t.occupied = db + B.occ;
-    t.kp_landmark_out = (int*)(db + B.klo);
-    t.kp_outlier = db + B.kout;
-    t.status = (int*)(db + B.status);
-    if (B.guided) {
-        t.q_x = (float*)(db + B.qx);
-        t.q_y = (float*)(db + B.qy);
-        t.q_margin = (float*)(db + B.qm);
-        t.q_xr = (float*)(db + B.qxr);
-        t.q_lo = (signed char*)(db + B.qlo);
-        t.q_hi = (signed char*)(db + B.qhi);
-        t.q_valid = db + B.qval;
+// One call of a tracking chain.  It owns what every chain does alike: the argument checks and the extractor's batch (open), the
+// TrackFrameDev table at offset 0 of the arena, stage C's outputs (begin_outputs), the arena and the stage timer (reserve), the common
+// fields of every frame's TrackFrameDev and its initial pose (frame_dev), the upload of the inputs and the zeroing of the outputs
+// (start), then stage C, motion_discard_kernel in a gated chain, the download and the synchronise (finish).  The entry point adds its
+// own blocks, staging, launches (with mark(1) .. mark(4) between them) and results, in that order.
+struct Call {
+    const char* who;
+    match::ChainId id;
+    match::Matcher* m = nullptr;
+    b200_lba_t opt = nullptr;
+    const b200_track_params_t* p = nullptr;
+    int n = 0;
+    Extracted x;
+    Layout a;
+    size_t out_begin = 0, out_end = 0;  // inputs [0, out_begin), outputs [out_begin, out_end), then scratch
+    size_t o_pose = 0, o_nvalid = 0;    // 16 doubles, one unsigned per frame
+    bool gated = false;                 // the frame_tracker chains: a gate per frame decides whether stage C applies
+    size_t o_stat = 0, o_gate = 0;      // kMotionStat words, one int per frame
+    unsigned char *hb = nullptr, *db = nullptr;
+    TrackFrameDev* hf = nullptr;        // the table in the pinned mirror
+    const TrackFrameDev* df = nullptr;  // and on the device
+    std::vector<const double*> poses;
+
+    Call(const char* who, match::ChainId id) : who(who), id(id) {}
+    match::ChainTimer& timer() const { return m->chain_timers[id]; }
+
+    // B200_OK with nothing opened when n_frames is 0.  extra() is the entry point's own check of its parameters.
+    template <class Extra>
+    int open(b200_orb_t orb, b200_matcher_t h, b200_lba_t lba, const b200_track_params_t* prm, int n_frames, Extra extra) {
+        if (!orb || !h || !lba || !prm || n_frames < 0) return B200_ERR_INVALID;
+        if (n_frames == 0) return B200_OK;
+        const b200_track_params_t& q = *prm;
+        if (!(q.scale_factors && q.inv_level_sigma_sq && q.num_levels != 0 && q.num_levels <= 32 && camera_valid(q.cam) && q.num_trials_robust >= 0
+              && q.num_trials >= 0 && q.num_each_iter >= 0 && extra())) {
+            set_error("%s: invalid parameters", who);
+            return B200_ERR_INVALID;
+        }
+        m = &h->m;
+        opt = lba;
+        p = prm;
+        n = n_frames;
+        int orb_device = 0;
+        int rc = orb_results(orb, &x.kps, &x.descs, &x.counts, &x.stride, &x.batch, &x.st, &orb_device);
+        if (rc) return rc;
+        if (orb_device != m->device) {
+            set_error("%s: extractor and matcher live on different devices", who);
+            return B200_ERR_INVALID;
+        }
+        B200_CUDA(cudaSetDevice(m->device));
+        a.take<TrackFrameDev>(n);  // at offset 0
+        poses.resize(n);
+        return B200_OK;
     }
-    return t;
-}
+    // Ends the inputs and takes the outputs every chain has, in this order: stage C's poses and inlier counts, in a gated chain the
+    // status words and gates, then each frame's kp_landmark_out and status
+    template <class Lay>
+    void begin_outputs(std::vector<Lay>& lay, bool gate) {
+        out_begin = a.end;
+        o_pose = a.take(8 * 16 * (size_t)n);
+        o_nvalid = a.take(4 * (size_t)n);
+        gated = gate;
+        if (gated) {
+            o_stat = a.take(4 * match::kMotionStat * (size_t)n);
+            o_gate = a.take(4 * (size_t)n);
+        }
+        for (FrameBlocks& B : lay) {
+            B.klo = a.take(4 * (size_t)std::max(x.stride, 1));
+            B.status = a.take(16);
+        }
+    }
+    void end_outputs() { out_end = a.end; }
+    int reserve() {
+        int rc = m->arena.reserve(a.end, out_end, x.st);
+        if (rc || (rc = timer().create())) return rc;
+        hb = m->arena.h;
+        db = m->arena.d;
+        hf = m->arena.host<TrackFrameDev>(0);
+        df = m->arena.dev<const TrackFrameDev>(0);
+        return B200_OK;
+    }
+    // Frame f's entry of the table with the fields that every chain fills the same way.  x_right (may be null) and pos_w are the
+    // caller's, staged into B.xr and B.pos; pose_cw is the initial pose of stage C.
+    TrackFrameDev& frame_dev(int f, int frame, int n_kp_in, int n_lm, const float* x_right, const double* pos_w, const double* pose_cw,
+                             const FrameBlocks& B) {
+        m->arena.put(B.xr, x_right, 4 * (size_t)n_kp_in);
+        m->arena.put(B.pos, pos_w, 24 * (size_t)n_lm);
+        poses[f] = pose_cw;
+        TrackFrameDev& t = hf[f];
+        t = TrackFrameDev{};
+        t.kps = x.kps + (size_t)frame * x.stride;
+        t.n_kp = x.counts + frame;
+        t.kp_cap = x.stride;
+        t.n_kp_in = n_kp_in;
+        t.n_lm = n_lm;
+        t.kp_x_right = x_right ? (const float*)(db + B.xr) : nullptr;
+        t.pos_w = (const double*)(db + B.pos);
+        rt_of(pose_cw, t.Rt);
+        for (int r = 0; r < 3; ++r) t.twc[r] = -(t.Rt[r] * t.Rt[9] + t.Rt[3 + r] * t.Rt[10] + t.Rt[6 + r] * t.Rt[11]);
+        t.undist = (b200_keypoint_t*)(db + B.und);
+        t.t_x = (float*)(db + B.tx);
+        t.t_y = (float*)(db + B.ty);
+        t.t_octave = db + B.toct;
+        t.occupied = db + B.occ;
+        t.kp_landmark_out = (int*)(db + B.klo);
+        t.kp_outlier = db + B.kout;
+        t.status = (int*)(db + B.status);
+        if (B.guided) {
+            t.q_x = (float*)(db + B.qx);
+            t.q_y = (float*)(db + B.qy);
+            t.q_margin = (float*)(db + B.qm);
+            t.q_xr = (float*)(db + B.qxr);
+            t.q_lo = (signed char*)(db + B.qlo);
+            t.q_hi = (signed char*)(db + B.qhi);
+            t.q_valid = db + B.qval;
+        }
+        return t;
+    }
+    // wait_matcher: the chain runs the brute-force matcher on the extractor's stream, and an earlier device-variant call on the
+    // matcher's stream may still read this handle's brute-force scratch
+    int start(bool wait_matcher = false) {
+        int rc = m->join();
+        if (rc) return rc;
+        if (wait_matcher && m->stream != x.st) {
+            B200_CUDA(cudaEventRecord(m->ev_topk, m->stream));
+            B200_CUDA(cudaStreamWaitEvent(x.st, m->ev_topk, 0));
+        }
+        B200_CUDA(cudaEventRecord(timer().ev[0], x.st));
+        B200_CUDA(m->arena.upload(out_begin, x.st));
+        B200_CUDA(cudaMemsetAsync(db + out_begin, 0, out_end - out_begin, x.st));
+        return B200_OK;
+    }
+    cudaError_t mark(int i) const { return cudaEventRecord(timer().ev[i], x.st); }
+    // num_matches_thr: the threshold of motion_discard_kernel in a gated chain
+    int finish(const TrackShared& sh, uint32_t num_matches_thr = 0) {
+        int* d_gate = gated ? (int*)(db + o_gate) : nullptr;
+        int rc = track_stage_c(opt, x.st, sh, df, hf, poses.data(), n, x.stride, p->num_trials_robust, p->num_trials, p->num_each_iter,
+                               (double*)(db + o_pose), (unsigned*)(db + o_nvalid), timer().ev[5], d_gate);
+        if (rc) return rc;
+        if (gated) {
+            match::motion_discard_kernel<<<n, 256, 0, x.st>>>(df, d_gate, num_matches_thr, (int*)(db + o_stat));
+            B200_CUDA(cudaGetLastError());
+        }
+        B200_CUDA(cudaEventRecord(timer().ev[6], x.st));
+        B200_CUDA(m->arena.download(out_begin, out_end, x.st));
+        B200_CUDA(cudaStreamSynchronize(x.st));
+        timer().timed = true;
+        return B200_OK;
+    }
+
+    // After finish: the overflow word of the guided search, a window returned more keypoints than cap
+    int overflow(size_t o_overflow, int cap) const {
+        const int k = *reinterpret_cast<const int*>(hb + o_overflow);
+        if (k <= 0) return B200_OK;
+        set_error("%s: a search window returned %d keypoints, max_candidates is %d", who, k, cap);
+        return B200_ERR_CAPACITY;
+    }
+    const int* status(const FrameBlocks& B) const { return reinterpret_cast<const int*>(hb + B.status); }
+    // status[0] is frame f's keypoint count, status[1] != 0 when n_keypoints_in disagrees with it (B200_ERR_INVALID); a count
+    // above kp_cap returns over_cap_rc
+    int check(int f, const FrameBlocks& B, int n_keypoints_in, int kp_cap, int over_cap_rc) const {
+        const int* s = status(B);
+        if (!s[1] && s[0] <= kp_cap) return B200_OK;
+        set_error("%s: frame %d has %d keypoints, n_keypoints_in is %d and kp_cap %d", who, f, s[0], n_keypoints_in, kp_cap);
+        return s[1] ? B200_ERR_INVALID : over_cap_rc;
+    }
+    const int* stat(int f) const { return reinterpret_cast<const int*>(hb + o_stat) + match::kMotionStat * (size_t)f; }
+    int gate(int f) const { return reinterpret_cast<const int*>(hb + o_gate)[f]; }
+    // fewer than 5 edges (pose_optimizer_g2o.cc:116-118): the initial pose stays
+    void pose(int f, const FrameBlocks& B, const double* pose_in, double* pose_out) const {
+        std::memcpy(pose_out, status(B)[2] < 5 ? (const void*)pose_in : hb + o_pose + sizeof(double) * 16 * (size_t)f, sizeof(double) * 16);
+    }
+};
 
 // A guided search of frame t's landmark table over the keypoints stage A wrote (n_train is set on the device from the extractor's
 // counter).  t_angle and q_angle are null when the search has no orientation gate.
@@ -1802,34 +1927,6 @@ static GuidedDev guided_of(const b200_track_params_t& p, int cap, const TrackFra
     return g;
 }
 
-// The end of every chain, once its outputs are downloaded and the stream synchronised
-struct Epilogue {
-    const char* who;
-    const unsigned char* hb;
-    size_t o_pose;  // 16 doubles per frame
-
-    // the overflow word of the guided search: a window returned more keypoints than cap
-    int overflow(size_t o_overflow, int cap) const {
-        const int n = *reinterpret_cast<const int*>(hb + o_overflow);
-        if (n <= 0) return B200_OK;
-        set_error("%s: a search window returned %d keypoints, max_candidates is %d", who, n, cap);
-        return B200_ERR_CAPACITY;
-    }
-    const int* status(const FrameBlocks& B) const { return reinterpret_cast<const int*>(hb + B.status); }
-    // status[0] is frame f's keypoint count, status[1] != 0 when n_keypoints_in disagrees with it (B200_ERR_INVALID); a count
-    // above kp_cap returns over_cap_rc
-    int check(int f, const FrameBlocks& B, int n_keypoints_in, int kp_cap, int over_cap_rc) const {
-        const int* s = status(B);
-        if (!s[1] && s[0] <= kp_cap) return B200_OK;
-        set_error("%s: frame %d has %d keypoints, n_keypoints_in is %d and kp_cap %d", who, f, s[0], n_keypoints_in, kp_cap);
-        return s[1] ? B200_ERR_INVALID : over_cap_rc;
-    }
-    // fewer than 5 edges (pose_optimizer_g2o.cc:116-118): the initial pose stays
-    void pose(int f, const FrameBlocks& B, const double* pose_in, double* pose_out) const {
-        std::memcpy(pose_out, status(B)[2] < 5 ? (const void*)pose_in : hb + o_pose + sizeof(double) * 16 * (size_t)f, sizeof(double) * 16);
-    }
-};
-
 // The by-value parameters of every chain; a kernel reads only the fields of its own chain
 static TrackShared shared_of(const b200_track_params_t& p, double true_baseline) {
     TrackShared sh{};
@@ -1855,10 +1952,6 @@ static TrackShared shared_of(const b200_track_params_t& p, double true_baseline)
 }
 }  // namespace chain
 }  // namespace b200
-
-struct b200_matcher_s {
-    b200::match::Matcher m;
-};
 
 using b200::match::Side;
 
@@ -1896,10 +1989,7 @@ int b200_matcher_destroy(b200_matcher_t h) {
     h->m.arena.release();
     for (int i = 0; i < 3; ++i)
         if (h->m.ev_t[i]) cudaEventDestroy(h->m.ev_t[i]);
-    h->m.track_timer.destroy();
-    h->m.motion_timer.destroy();
-    h->m.robust_timer.destroy();
-    h->m.bow_timer.destroy();
+    for (b200::match::ChainTimer& t : h->m.chain_timers) t.destroy();
     if (h->m.ev_topk) cudaEventDestroy(h->m.ev_topk);
     if (h->m.ev_resolved) cudaEventDestroy(h->m.ev_resolved);
     if (h->m.side_stream) cudaStreamDestroy(h->m.side_stream);
@@ -2230,36 +2320,38 @@ int b200_match_guided(b200_matcher_t h, int n_problems, b200_guided_problem_t* p
     return B200_OK;
 }
 
-int b200_track_stage_ms(b200_matcher_t h, int stage, float* ms) { return h ? h->m.track_timer.elapsed(stage, ms) : B200_ERR_INVALID; }
+static int chain_stage_ms(b200_matcher_t h, b200::match::ChainId id, int stage, float* ms) {
+    return h ? h->m.chain_timers[id].elapsed(stage, ms) : B200_ERR_INVALID;
+}
+int b200_track_stage_ms(b200_matcher_t h, int stage, float* ms) { return chain_stage_ms(h, b200::match::kLocalMapChain, stage, ms); }
+int b200_motion_track_stage_ms(b200_matcher_t h, int stage, float* ms) { return chain_stage_ms(h, b200::match::kMotionChain, stage, ms); }
+int b200_robust_track_stage_ms(b200_matcher_t h, int stage, float* ms) { return chain_stage_ms(h, b200::match::kRobustChain, stage, ms); }
+int b200_bow_track_stage_ms(b200_matcher_t h, int stage, float* ms) { return chain_stage_ms(h, b200::match::kBowChain, stage, ms); }
 
 // The device-resident tracking chain (see include/b200vslam.h).  Arena of the matcher handle:
-//   [TrackFrameDev x n][GuidedDev x n][caller inputs]  -- mirrored in pinned memory, one upload
-//   [outputs]                                          -- one download
+//   [TrackFrameDev x n][GuidedDev x n][caller inputs]                                         -- mirrored in pinned memory, one upload
+//   [poses, n_valid][per frame: kp_landmark_out, status]
+//   [per frame: observable, kp_outlier, match_out, n_matches][overflow]                       -- one download
 //   [stage-A products, guided scratch]
 int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const b200_track_params_t* prm, int n_frames, b200_track_frame_t* frames) {
     B200_RANGE("b200:track:local_map");
     namespace chain = b200::chain;
     using chain::TrackFrameDev;
     using b200::match::GuidedDev;
-    const char* who = "b200_track_local_map";
-    if (!orb || !h || !opt || !prm || n_frames < 0) return B200_ERR_INVALID;
-    if (n_frames == 0) return B200_OK;
-    int rc = chain::check_params(who, *prm, frames && chain::search_params_valid(*prm));
-    if (rc) return rc;
-    auto& m = h->m;
-    chain::Extracted x;
-    if ((rc = chain::open_extracted(who, orb, m.device, &x))) return rc;
+    chain::Call C("b200_track_local_map", b200::match::kLocalMapChain);
+    int rc = C.open(orb, h, opt, prm, n_frames, [&] { return frames && chain::search_params_valid(*prm); });
+    if (rc || n_frames == 0) return rc;
+    const chain::Extracted& x = C.x;
     const int stride = x.stride;
     cudaStream_t st = x.st;
     const int cap = prm->max_candidates ? prm->max_candidates : 256;
     struct Lay : chain::FrameBlocks {
-        size_t xr, kl, pos, nrm, lo, hi, desc, skip, hobs;  // inputs
-        size_t obs, mout, nm;                               // outputs (with klo, kout and status)
+        size_t kl, nrm, lo, hi, desc, skip, hobs;  // inputs (with xr and pos)
+        size_t obs, mout, nm;                      // outputs (with klo, kout and status)
     };
     std::vector<Lay> lay(n_frames);
     int max_lm = 0;
-    b200::Layout a;
-    a.take<TrackFrameDev>(n_frames);  // at offset 0
+    b200::Layout& a = C.a;
     const size_t o_gd = a.take<GuidedDev>(n_frames);
     for (int f = 0; f < n_frames; ++f) {
         const b200_track_frame_t& F = frames[f];
@@ -2282,54 +2374,42 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const
         L.hobs = a.take(nl);
         max_lm = std::max(max_lm, F.n_landmarks);
     }
-    const size_t in_bytes = a.end, out_begin = a.end;
+    C.begin_outputs(lay, false);
     const size_t kc = (size_t)std::max(stride, 1);
     for (int f = 0; f < n_frames; ++f) {
         Lay& L = lay[f];
         const size_t nl = (size_t)frames[f].n_landmarks;
         L.obs = a.take(nl);
-        L.klo = a.take(4 * kc);
         L.kout = a.take(kc);
-        L.status = a.take(16);
         L.mout = a.take(4 * nl);
         L.nm = a.take(4);
     }
-    const size_t o_pose = a.take(8 * 16 * (size_t)n_frames);
-    const size_t o_nvalid = a.take(4 * (size_t)n_frames);
     const size_t o_overflow = a.take(4);
-    const size_t out_end = a.end;
+    C.end_outputs();
     const size_t cells = (size_t)prm->grid_cols * prm->grid_rows;
     for (int f = 0; f < n_frames; ++f) {
         lay[f].take_stage_a(a, kc, false);
         lay[f].take_guided(a, kc, (size_t)frames[f].n_landmarks, cells, cap);
     }
     size_t rs_bytes = 0;
-    if ((rc = b200::match::guided_resolve_smem(who, stride, &rs_bytes))) return rc;
-    if ((rc = m.arena.reserve(a.end, out_end, st))) return rc;
-    b200::match::ChainTimer& T = m.track_timer;
-    if ((rc = T.create())) return rc;
-    b200::StagingArena& A = m.arena;
-    unsigned char *hb = A.h, *db = A.d;
-    TrackFrameDev* hf = A.host<TrackFrameDev>(0);
+    if ((rc = b200::match::guided_resolve_smem(C.who, stride, &rs_bytes))) return rc;
+    if ((rc = C.reserve())) return rc;
+    b200::StagingArena& A = C.m->arena;
+    unsigned char *hb = C.hb, *db = C.db;
     GuidedDev* hg = A.host<GuidedDev>(o_gd);
     const chain::TrackShared sh = chain::shared_of(*prm, 0.0);
-    std::vector<const double*> poses(n_frames);
     for (int f = 0; f < n_frames; ++f) {
         const b200_track_frame_t& F = frames[f];
         const Lay& L = lay[f];
         const size_t nk = (size_t)F.n_keypoints_in, nl = (size_t)F.n_landmarks;
-        A.put(L.xr, F.kp_x_right, 4 * nk);
         A.put(L.kl, F.kp_landmark, 4 * nk);
-        A.put(L.pos, F.lm_pos_w, 24 * nl);
         A.put(L.nrm, F.lm_mean_normal, 24 * nl);
         A.put(L.lo, F.lm_min_valid_dist, 4 * nl);
         A.put(L.hi, F.lm_max_valid_dist, 4 * nl);
         A.put(L.desc, F.lm_desc, 32 * nl);
         A.put(L.skip, F.lm_skip, nl);
         A.put(L.hobs, F.lm_has_observation, nl);
-        poses[f] = F.pose_cw;
-        TrackFrameDev t = chain::frame_dev(x, F.frame, F.n_keypoints_in, F.n_landmarks, F.kp_x_right ? (const float*)(db + L.xr) : nullptr,
-                                           (const double*)(db + L.pos), F.pose_cw, L, db);
+        TrackFrameDev& t = C.frame_dev(f, F.frame, F.n_keypoints_in, F.n_landmarks, F.kp_x_right, F.lm_pos_w, F.pose_cw, L);
         t.kp_landmark = F.kp_landmark ? (const int*)(db + L.kl) : nullptr;
         t.mean_normal = (const double*)(db + L.nrm);
         t.min_d = (const float*)(db + L.lo);
@@ -2338,57 +2418,45 @@ int b200_track_local_map(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const
         t.lm_has_obs = F.lm_has_observation ? db + L.hobs : nullptr;
         t.observable = db + L.obs;
         t.match_out = (const int*)(db + L.mout);
-        hf[f] = t;
         hg[f] = chain::guided_of(*prm, cap, t, L, db, F.n_landmarks, reinterpret_cast<const uint4*>(x.descs + (size_t)F.frame * stride * 32),
                                  (const uint4*)(db + L.desc), nullptr, nullptr, t.occupied, (int*)(db + L.mout), (int*)(db + L.nm));
     }
-    if ((rc = m.join())) return rc;
-    B200_CUDA(cudaEventRecord(T.ev[0], st));
-    B200_CUDA(A.upload(in_bytes, st));
-    B200_CUDA(cudaMemsetAsync(db + out_begin, 0, out_end - out_begin, st));
-    const TrackFrameDev* df = A.dev<const TrackFrameDev>(0);
+    if ((rc = C.start())) return rc;
+    const TrackFrameDev* df = C.df;
     GuidedDev* dg = A.dev<GuidedDev>(o_gd);
     if ((rc = chain::track_stage_a(st, sh, df, n_frames, stride, max_lm))) return rc;
     b200::match::track_set_counts_kernel<<<b200::ceil_div(n_frames, 128), 128, 0, st>>>(dg, df, n_frames);
-    B200_CUDA(cudaEventRecord(T.ev[1], st));
+    B200_CUDA(C.mark(1));
     b200::match::guided_grid_kernel<<<n_frames, 1024, 0, st>>>(dg);
-    B200_CUDA(cudaEventRecord(T.ev[2], st));
+    B200_CUDA(C.mark(2));
     b200::match::guided_candidates_kernel<<<dim3(std::max(1, b200::ceil_div(max_lm, 128)), n_frames), 128, 0, st>>>(dg, B200_GUIDED_LANDMARKS, 0,
                                                                                                                      (int*)(db + o_overflow));
-    B200_CUDA(cudaEventRecord(T.ev[3], st));
+    B200_CUDA(C.mark(3));
     b200::match::guided_resolve_kernel<GuidedDev><<<n_frames, 32, rs_bytes, st>>>(dg, B200_GUIDED_LANDMARKS, prm->hamming_thr, prm->lowe_ratio);
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaEventRecord(T.ev[4], st));
-    if ((rc = chain::track_stage_c(opt, st, sh, df, hf, poses.data(), n_frames, stride, prm->num_trials_robust, prm->num_trials, prm->num_each_iter,
-                                   (double*)(db + o_pose), (unsigned*)(db + o_nvalid), T.ev[5])))
-        return rc;
-    B200_CUDA(cudaEventRecord(T.ev[6], st));
-    B200_CUDA(A.download(out_begin, out_end, st));
-    B200_CUDA(cudaStreamSynchronize(st));
-    T.timed = true;
-    const chain::Epilogue E{who, hb, o_pose};
-    if ((rc = E.overflow(o_overflow, cap))) return rc;
+    B200_CUDA(C.mark(4));
+    if ((rc = C.finish(sh))) return rc;
+    if ((rc = C.overflow(o_overflow, cap))) return rc;
     for (int f = 0; f < n_frames; ++f) {
         b200_track_frame_t& F = frames[f];
         const Lay& L = lay[f];
-        if ((rc = E.check(f, L, F.n_keypoints_in, F.kp_cap, B200_ERR_CAPACITY))) return rc;
-        const int nk = E.status(L)[0];
+        if ((rc = C.check(f, L, F.n_keypoints_in, F.kp_cap, B200_ERR_CAPACITY))) return rc;
+        const int nk = C.status(L)[0];
         F.n_keypoints = nk;
         if (F.n_landmarks > 0) std::memcpy(F.lm_observable, hb + L.obs, (size_t)F.n_landmarks);
         std::memcpy(F.kp_landmark_out, hb + L.klo, 4 * (size_t)nk);
         std::memcpy(F.kp_outlier, hb + L.kout, (size_t)nk);
         F.n_matches = *reinterpret_cast<const int*>(hb + L.nm);
-        F.n_valid = reinterpret_cast<const unsigned*>(hb + o_nvalid)[f];
-        E.pose(f, L, F.pose_cw, F.pose_cw_out);
+        F.n_valid = reinterpret_cast<const unsigned*>(hb + C.o_nvalid)[f];
+        C.pose(f, L, F.pose_cw, F.pose_cw_out);
     }
     return B200_OK;
 }
 
-int b200_motion_track_stage_ms(b200_matcher_t h, int stage, float* ms) { return h ? h->m.motion_timer.elapsed(stage, ms) : B200_ERR_INVALID; }
-
 // Motion-model tracking on the device (see include/b200vslam.h).  Arena of the matcher handle, as for b200_track_local_map:
 //   [TrackFrameDev x n][GuidedDev x n][GuidedDev x n (second search)][caller inputs]  -- mirrored in pinned memory, one upload
-//   [outputs]                                                                        -- one download
+//   [poses, n_valid, status words, gates][per frame: kp_landmark_out, status]
+//   [per frame: match_out, n_matches][overflow]                                       -- one download
 //   [stage-A products, guided scratch, second-search buffers]
 int b200_motion_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const b200_track_params_t* prm, double true_baseline,
                             uint32_t num_matches_thr, int n_frames, b200_motion_track_frame_t* frames) {
@@ -2396,28 +2464,22 @@ int b200_motion_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, co
     namespace chain = b200::chain;
     using chain::TrackFrameDev;
     using b200::match::GuidedDev;
-    using b200::match::kMotionStat;
-    const char* who = "b200_motion_based_track";
-    if (!orb || !h || !opt || !prm || n_frames < 0) return B200_ERR_INVALID;
-    if (n_frames == 0) return B200_OK;
-    int rc = chain::check_params(who, *prm, frames && chain::search_params_valid(*prm) && !std::isnan(true_baseline));
-    if (rc) return rc;
-    auto& m = h->m;
-    chain::Extracted x;
-    if ((rc = chain::open_extracted(who, orb, m.device, &x))) return rc;
+    chain::Call C("b200_motion_based_track", b200::match::kMotionChain);
+    int rc = C.open(orb, h, opt, prm, n_frames, [&] { return frames && chain::search_params_valid(*prm) && !std::isnan(true_baseline); });
+    if (rc || n_frames == 0) return rc;
+    const chain::Extracted& x = C.x;
     const int stride = x.stride;
     cudaStream_t st = x.st;
     const int cap = prm->max_candidates ? prm->max_candidates : 256;
     struct Lay : chain::FrameBlocks {
-        size_t xr, pos, desc, oct, ang, hobs;  // inputs
-        size_t mout, nm;                       // outputs (with klo and status)
-        size_t tang;                           // stage A: keypoint angles
-        size_t occ2, mout2, nm2;               // second search
+        size_t desc, oct, ang, hobs;  // inputs (with xr and pos)
+        size_t mout, nm;              // outputs (with klo and status)
+        size_t tang;                  // stage A: keypoint angles
+        size_t occ2, mout2, nm2;      // second search
     };
     std::vector<Lay> lay(n_frames);
     int max_lm = 0;
-    b200::Layout a;
-    a.take<TrackFrameDev>(n_frames);  // at offset 0
+    b200::Layout& a = C.a;
     const size_t o_gd = a.take<GuidedDev>(n_frames), o_gd2 = a.take<GuidedDev>(n_frames);
     for (int f = 0; f < n_frames; ++f) {
         const b200_motion_track_frame_t& F = frames[f];
@@ -2442,22 +2504,16 @@ int b200_motion_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, co
         L.hobs = a.take(nl);
         max_lm = std::max(max_lm, F.n_landmarks);
     }
-    const size_t in_bytes = a.end, out_begin = a.end;
+    C.begin_outputs(lay, true);
     const size_t kc = (size_t)std::max(stride, 1);
     for (int f = 0; f < n_frames; ++f) {
         Lay& L = lay[f];
         const size_t nl = (size_t)frames[f].n_landmarks;
-        L.klo = a.take(4 * kc);
-        L.status = a.take(16);
         L.mout = a.take(4 * nl);
         L.nm = a.take(4);
     }
-    const size_t o_pose = a.take(8 * 16 * (size_t)n_frames);
-    const size_t o_nvalid = a.take(4 * (size_t)n_frames);
-    const size_t o_stat = a.take(4 * kMotionStat * (size_t)n_frames);
-    const size_t o_gate = a.take(4 * (size_t)n_frames);
     const size_t o_overflow = a.take(4);
-    const size_t out_end = a.end;
+    C.end_outputs();
     const size_t cells = (size_t)prm->grid_cols * prm->grid_rows;
     for (int f = 0; f < n_frames; ++f) {
         Lay& L = lay[f];
@@ -2470,37 +2526,28 @@ int b200_motion_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, co
         L.nm2 = a.take(4);
     }
     size_t rs_bytes = 0;
-    if ((rc = b200::match::guided_resolve_smem(who, stride, &rs_bytes))) return rc;
-    if ((rc = m.arena.reserve(a.end, out_end, st))) return rc;
-    b200::match::ChainTimer& T = m.motion_timer;
-    if ((rc = T.create())) return rc;
-    b200::StagingArena& A = m.arena;
-    unsigned char *hb = A.h, *db = A.d;
-    TrackFrameDev* hf = A.host<TrackFrameDev>(0);
+    if ((rc = b200::match::guided_resolve_smem(C.who, stride, &rs_bytes))) return rc;
+    if ((rc = C.reserve())) return rc;
+    b200::StagingArena& A = C.m->arena;
+    unsigned char* db = C.db;
     GuidedDev* hg = A.host<GuidedDev>(o_gd);
     GuidedDev* hg2 = A.host<GuidedDev>(o_gd2);
     const chain::TrackShared sh = chain::shared_of(*prm, true_baseline);
-    std::vector<const double*> poses(n_frames);
     for (int f = 0; f < n_frames; ++f) {
         const b200_motion_track_frame_t& F = frames[f];
         const Lay& L = lay[f];
-        const size_t nk = (size_t)F.n_keypoints_in, nl = (size_t)F.n_landmarks;
-        A.put(L.xr, F.kp_x_right, 4 * nk);
-        A.put(L.pos, F.lm_pos_w, 24 * nl);
+        const size_t nl = (size_t)F.n_landmarks;
         A.put(L.desc, F.lm_desc, 32 * nl);
         A.put(L.oct, F.lm_octave, nl);
         A.put(L.ang, F.lm_angle, 4 * nl);
         A.put(L.hobs, F.lm_has_observation, nl);
-        poses[f] = F.pose_cw;
         // kp_landmark stays null: the frame starts without landmarks (frame_tracker.cc:27)
-        TrackFrameDev t = chain::frame_dev(x, F.frame, F.n_keypoints_in, F.n_landmarks, F.kp_x_right ? (const float*)(db + L.xr) : nullptr,
-                                           (const double*)(db + L.pos), F.pose_cw, L, db);
+        TrackFrameDev& t = C.frame_dev(f, F.frame, F.n_keypoints_in, F.n_landmarks, F.kp_x_right, F.lm_pos_w, F.pose_cw, L);
         t.lm_has_obs = F.lm_has_observation ? db + L.hobs : nullptr;
         t.lm_octave = db + L.oct;
         if (F.last_pose_cw) chain::rt_of(F.last_pose_cw, t.last_Rt);
         t.t_angle = (float*)(db + L.tang);
         t.match_out = (const int*)(db + L.mout);
-        hf[f] = t;
         const uint4* t_desc = reinterpret_cast<const uint4*>(x.descs + (size_t)F.frame * stride * 32);
         const uint4* q_desc = (const uint4*)(db + L.desc);
         const float* q_angle = (const float*)(db + L.ang);
@@ -2509,84 +2556,64 @@ int b200_motion_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, co
         // both counts of the second search are set by motion_retry_kernel
         hg2[f] = chain::guided_of(*prm, cap, t, L, db, 0, t_desc, q_desc, t.t_angle, q_angle, db + L.occ2, (int*)(db + L.mout2), (int*)(db + L.nm2));
     }
-    if ((rc = m.join())) return rc;
-    B200_CUDA(cudaEventRecord(T.ev[0], st));
-    B200_CUDA(A.upload(in_bytes, st));
-    B200_CUDA(cudaMemsetAsync(db + out_begin, 0, out_end - out_begin, st));
-    const TrackFrameDev* df = A.dev<const TrackFrameDev>(0);
+    if ((rc = C.start())) return rc;
+    const TrackFrameDev* df = C.df;
     GuidedDev* dg = A.dev<GuidedDev>(o_gd);
     GuidedDev* dg2 = A.dev<GuidedDev>(o_gd2);
-    int* d_stat = (int*)(db + o_stat);
-    int* d_gate = (int*)(db + o_gate);
+    int* d_stat = (int*)(db + C.o_stat);
     const unsigned thr = num_matches_thr;
     const dim3 q_grid(std::max(1, b200::ceil_div(max_lm, 128)), n_frames);
     const float lowe = 0.9f;  // projection(0.9, true): mode 1 has no ratio test
     if ((rc = chain::motion_stage_a(st, sh, df, n_frames, stride, max_lm))) return rc;
     b200::match::track_set_counts_kernel<<<b200::ceil_div(n_frames, 128), 128, 0, st>>>(dg, df, n_frames);
-    B200_CUDA(cudaEventRecord(T.ev[1], st));
+    B200_CUDA(C.mark(1));
     b200::match::guided_grid_kernel<<<n_frames, 1024, 0, st>>>(dg);
-    B200_CUDA(cudaEventRecord(T.ev[2], st));
+    B200_CUDA(C.mark(2));
     b200::match::guided_candidates_kernel<<<q_grid, 128, 0, st>>>(dg, B200_GUIDED_LAST_FRAME, 1, (int*)(db + o_overflow));
     b200::match::guided_resolve_kernel<GuidedDev><<<n_frames, 32, rs_bytes, st>>>(dg, B200_GUIDED_LAST_FRAME, prm->hamming_thr, lowe);
-    B200_CUDA(cudaEventRecord(T.ev[3], st));
+    B200_CUDA(C.mark(3));
     b200::match::motion_retry_kernel<<<n_frames, 128, 0, st>>>(dg, dg2, df, thr, d_stat);
     b200::match::guided_candidates_kernel<<<q_grid, 128, 0, st>>>(dg2, B200_GUIDED_LAST_FRAME, 1, (int*)(db + o_overflow));
     b200::match::guided_resolve_kernel<GuidedDev><<<n_frames, 32, rs_bytes, st>>>(dg2, B200_GUIDED_LAST_FRAME, prm->hamming_thr, lowe);
-    b200::match::motion_select_kernel<<<q_grid, 128, 0, st>>>(dg, dg2, thr, d_stat, d_gate);
+    b200::match::motion_select_kernel<<<q_grid, 128, 0, st>>>(dg, dg2, thr, d_stat, (int*)(db + C.o_gate));
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaEventRecord(T.ev[4], st));
-    if ((rc = chain::track_stage_c(opt, st, sh, df, hf, poses.data(), n_frames, stride, prm->num_trials_robust, prm->num_trials, prm->num_each_iter,
-                                   (double*)(db + o_pose), (unsigned*)(db + o_nvalid), T.ev[5], d_gate)))
-        return rc;
-    b200::match::motion_discard_kernel<<<n_frames, 256, 0, st>>>(df, d_gate, thr, d_stat);
-    B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaEventRecord(T.ev[6], st));
-    B200_CUDA(A.download(out_begin, out_end, st));
-    B200_CUDA(cudaStreamSynchronize(st));
-    T.timed = true;
-    const chain::Epilogue E{who, hb, o_pose};
-    if ((rc = E.overflow(o_overflow, cap))) return rc;
+    B200_CUDA(C.mark(4));
+    if ((rc = C.finish(sh, thr))) return rc;
+    if ((rc = C.overflow(o_overflow, cap))) return rc;
     for (int f = 0; f < n_frames; ++f) {
         b200_motion_track_frame_t& F = frames[f];
         const Lay& L = lay[f];
-        if ((rc = E.check(f, L, F.n_keypoints_in, F.kp_cap, B200_ERR_CAPACITY))) return rc;
-        const int nk = E.status(L)[0];
-        const int* ms = reinterpret_cast<const int*>(hb + o_stat) + kMotionStat * (size_t)f;
+        if ((rc = C.check(f, L, F.n_keypoints_in, F.kp_cap, B200_ERR_CAPACITY))) return rc;
+        const int nk = C.status(L)[0];
+        const int* ms = C.stat(f);
         F.n_keypoints = nk;
-        std::memcpy(F.kp_landmark_out, hb + L.klo, 4 * (size_t)nk);
+        std::memcpy(F.kp_landmark_out, C.hb + L.klo, 4 * (size_t)nk);
         F.n_matches_first = ms[0];
         F.retried = ms[1];
         F.n_matches = ms[2];
         F.n_valid = (uint32_t)ms[3];
         F.tracked = ms[4];
-        E.pose(f, L, F.pose_cw, F.pose_cw_out);  // a failed frame builds no edge: the predicted pose stays
+        C.pose(f, L, F.pose_cw, F.pose_cw_out);  // a failed frame builds no edge: the predicted pose stays
     }
     return B200_OK;
 }
 
-int b200_robust_track_stage_ms(b200_matcher_t h, int stage, float* ms) { return h ? h->m.robust_timer.elapsed(stage, ms) : B200_ERR_INVALID; }
-
 // Robust-match tracking on the device (see include/b200vslam.h).  Arena of the matcher handle:
 //   [TrackFrameDev x n][engines][off1 | off2 | cnt2][keyframe descriptors | angles | valid | bearings, concatenated][per frame: x_right,
 //   landmark positions]                                                                  -- mirrored in pinned memory, one upload
-//   [per frame: kp_landmark_out, status][poses, n_valid, status words, gates]             -- one download
+//   [poses, n_valid, status words, gates][per frame: kp_landmark_out, status]             -- one download
 //   [stage-A products, pairs, essential problems and scratch]
 int b200_robust_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const b200_track_params_t* prm, uint32_t num_matches_thr,
                                   int n_frames, b200_robust_track_frame_t* frames) {
     B200_RANGE("b200:track:robust");
     namespace chain = b200::chain;
     using chain::TrackFrameDev;
-    using b200::match::kMotionStat;
     using b200::match::kRobustIter;
     namespace ess = b200::ess;
-    const char* who = "b200_robust_match_based_track";
-    if (!orb || !h || !opt || !prm || n_frames < 0) return B200_ERR_INVALID;
-    if (n_frames == 0) return B200_OK;
-    int rc = chain::check_params(who, *prm, frames && std::isfinite(prm->lowe_ratio));
-    if (rc) return rc;
-    auto& m = h->m;
-    chain::Extracted x;
-    if ((rc = chain::open_extracted(who, orb, m.device, &x))) return rc;
+    chain::Call C("b200_robust_match_based_track", b200::match::kRobustChain);
+    int rc = C.open(orb, h, opt, prm, n_frames, [&] { return frames && std::isfinite(prm->lowe_ratio); });
+    if (rc || n_frames == 0) return rc;
+    const chain::Extracted& x = C.x;
     const int stride = x.stride;
     cudaStream_t st = x.st;
     long long total_kf = 0;
@@ -2609,12 +2636,10 @@ int b200_robust_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t o
     const size_t kc = (size_t)std::max(stride, 1), nf = (size_t)n_frames, T2 = (size_t)std::max(total_kf, 1LL);
     const size_t NH = nf * kRobustIter, rows = nf * kc;
     struct Lay : chain::FrameBlocks {
-        size_t xr, pos;    // inputs
-        size_t bear, mout; // stage A: bearings; landmark-table matches
+        size_t bear, mout;  // stage A: bearings; landmark-table matches
     };
     std::vector<Lay> lay(n_frames);
-    b200::Layout a;
-    a.take<TrackFrameDev>(n_frames);  // at offset 0
+    b200::Layout& a = C.a;
     const size_t o_eng = a.take<b200_mt19937_t>(n_frames);
     const size_t o_meta = a.take<int>(3 * nf);  // off1 | off2 | cnt2
     const size_t o_kdesc = a.take(32 * T2), o_kang = a.take(4 * T2), o_kval = a.take(T2), o_kbear = a.take(24 * T2);
@@ -2622,13 +2647,8 @@ int b200_robust_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t o
         lay[f].xr = a.take(4 * (size_t)frames[f].n_keypoints_in);
         lay[f].pos = a.take(24 * (size_t)frames[f].n_kf_keypoints);
     }
-    const size_t in_bytes = a.end, out_begin = a.end;
-    for (int f = 0; f < n_frames; ++f) {
-        lay[f].klo = a.take(4 * kc);
-        lay[f].status = a.take(16);
-    }
-    const size_t o_pose = a.take(8 * 16 * nf), o_nvalid = a.take(4 * nf), o_stat = a.take(4 * kMotionStat * nf), o_gate = a.take(4 * nf);
-    const size_t out_end = a.end;
+    C.begin_outputs(lay, true);
+    C.end_outputs();
     for (int f = 0; f < n_frames; ++f) {
         Lay& L = lay[f];
         L.take_stage_a(a, kc, true);
@@ -2640,20 +2660,16 @@ int b200_robust_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t o
     const size_t o_b1 = a.take<double>(3 * rows), o_b2 = a.take<double>(3 * rows);
     const size_t o_cand = a.take<double>(9 * ess::kMaxCand * NH), o_hyp = a.take<ess::HypDev>(NH), o_sc = a.take<ess::ScoreDev>(ess::kMaxCand * NH);
     const size_t o_idx = a.take<int32_t>(rows), o_mat = a.take<double>(9 * rows), o_fl = a.take(rows), o_res = a.take<ess::ResultDev>(nf);
-    if ((rc = m.arena.reserve(a.end, out_end, st))) return rc;
-    b200::match::ChainTimer& T = m.robust_timer;
-    if ((rc = T.create())) return rc;
-    b200::StagingArena& A = m.arena;
-    unsigned char *hb = A.h, *db = A.d;
-    TrackFrameDev* hf = A.host<TrackFrameDev>(0);
+    if ((rc = C.reserve())) return rc;
+    b200::StagingArena& A = C.m->arena;
+    unsigned char* db = C.db;
     const chain::TrackShared sh = chain::shared_of(*prm, 0.0);
     int* meta = A.host<int>(o_meta);
-    std::vector<const double*> poses(n_frames);
     size_t koff = 0;
     for (int f = 0; f < n_frames; ++f) {
         const b200_robust_track_frame_t& F = frames[f];
         const Lay& L = lay[f];
-        const size_t nk = (size_t)F.n_keypoints_in, nkf = (size_t)F.n_kf_keypoints;
+        const size_t nkf = (size_t)F.n_kf_keypoints;
         if (F.engine) A.put(o_eng + sizeof(b200_mt19937_t) * f, F.engine, sizeof(b200_mt19937_t));
         else b200_mt19937_seed(A.host<b200_mt19937_t>(o_eng) + f, nullptr, 0);
         meta[f] = F.frame * stride;
@@ -2663,44 +2679,29 @@ int b200_robust_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t o
         A.put(o_kang + 4 * koff, F.kf_angle, 4 * nkf);
         A.put(o_kval + koff, F.kf_valid, nkf);
         A.put(o_kbear + 24 * koff, F.kf_bearings, 24 * nkf);
-        A.put(L.xr, F.kp_x_right, 4 * nk);
-        A.put(L.pos, F.kf_pos_w, 24 * nkf);
         koff += nkf;
-        poses[f] = F.last_pose_cw;
         // the landmark table is the keyframe's keypoints; kp_landmark stays null: set_landmarks replaces every slot (frame_tracker.cc:111)
-        TrackFrameDev t = chain::frame_dev(x, F.frame, F.n_keypoints_in, F.n_kf_keypoints, F.kp_x_right ? (const float*)(db + L.xr) : nullptr,
-                                           (const double*)(db + L.pos), F.last_pose_cw, L, db);
+        TrackFrameDev& t = C.frame_dev(f, F.frame, F.n_keypoints_in, F.n_kf_keypoints, F.kp_x_right, F.kf_pos_w, F.last_pose_cw, L);
         t.match_out = (const int*)(db + L.mout);
         t.bearings = (double*)(db + L.bear);
         t.count_out = (int*)(db + o_cnt1) + f;
-        hf[f] = t;
     }
-    // the brute-force scratch of this handle may still be read by an earlier device-variant call on the matcher's stream
-    if ((rc = m.join())) return rc;
-    if (m.stream != st) {
-        B200_CUDA(cudaEventRecord(m.ev_topk, m.stream));
-        B200_CUDA(cudaStreamWaitEvent(st, m.ev_topk, 0));
-    }
-    B200_CUDA(cudaEventRecord(T.ev[0], st));
-    B200_CUDA(A.upload(in_bytes, st));
-    B200_CUDA(cudaMemsetAsync(db + out_begin, 0, out_end - out_begin, st));
-    const TrackFrameDev* df = A.dev<const TrackFrameDev>(0);
-    int* d_stat = (int*)(db + o_stat);
-    int* d_gate = (int*)(db + o_gate);
+    if ((rc = C.start(true))) return rc;
+    const TrackFrameDev* df = C.df;
     const int* d_meta = A.dev<const int>(o_meta);
     int* d_pairs = (int*)(db + o_pairs);
     int* d_npairs = (int*)(db + o_npairs);
     if ((rc = chain::robust_stage_a(st, sh, df, n_frames, stride))) return rc;
-    B200_CUDA(cudaEventRecord(T.ev[1], st));
+    B200_CUDA(C.mark(1));
     using b200::match::Side;
     const Side S1{reinterpret_cast<const uint4*>(x.descs), reinterpret_cast<const unsigned char*>(x.kps) + offsetof(b200_keypoint_t, angle),
                   (long long)sizeof(b200_keypoint_t), d_meta, (const int*)(db + o_cnt1)};
     const Side S2{(const uint4*)(db + o_kdesc), db + o_kang, (long long)sizeof(float), d_meta + n_frames, d_meta + 2 * n_frames};
-    if ((rc = m.run(st, n_frames, S1, S2, db + o_kval, stride, max_kf, prm->lowe_ratio, 1, d_pairs, (int)kc, d_npairs))) return rc;
-    B200_CUDA(cudaEventRecord(T.ev[2], st));
+    if ((rc = C.m->run(st, n_frames, S1, S2, db + o_kval, stride, max_kf, prm->lowe_ratio, 1, d_pairs, (int)kc, d_npairs))) return rc;
+    B200_CUDA(C.mark(2));
     int32_t* d_ms = (int32_t*)(db + o_ms);
     if ((rc = chain::draw_min_sets(st, n_frames, A.dev<const b200_mt19937_t>(o_eng), d_npairs, ess::kMinSet, kRobustIter, d_ms))) return rc;
-    B200_CUDA(cudaEventRecord(T.ev[3], st));
+    B200_CUDA(C.mark(3));
     double* d_b1 = (double*)(db + o_b1);
     double* d_b2 = (double*)(db + o_b2);
     b200::match::robust_gather_kernel<<<n_frames, 256, 0, st>>>(d_pairs, d_npairs, (int)kc, df, (const double*)(db + o_kbear), d_meta + n_frames, d_b1,
@@ -2710,63 +2711,48 @@ int b200_robust_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t o
                             (ess::HypDev*)(db + o_hyp), (ess::ScoreDev*)(db + o_sc), (int32_t*)(db + o_idx), (double*)(db + o_mat), db + o_fl,
                             (ess::ResultDev*)(db + o_res)};
     if ((rc = ess::enqueue_ransac(st, n_frames, (int)NH, rd))) return rc;
-    B200_CUDA(cudaEventRecord(T.ev[4], st));
+    B200_CUDA(C.mark(4));
     b200::match::robust_apply_kernel<<<n_frames, 256, 0, st>>>(d_pairs, d_npairs, (int)kc, db + o_fl, (const ess::ResultDev*)(db + o_res), df,
-                                                               num_matches_thr, d_stat, d_gate);
+                                                               num_matches_thr, (int*)(db + C.o_stat), (int*)(db + C.o_gate));
     B200_CUDA(cudaGetLastError());
-    if ((rc = chain::track_stage_c(opt, st, sh, df, hf, poses.data(), n_frames, stride, prm->num_trials_robust, prm->num_trials, prm->num_each_iter,
-                                   (double*)(db + o_pose), (unsigned*)(db + o_nvalid), T.ev[5], d_gate)))
-        return rc;
-    b200::match::motion_discard_kernel<<<n_frames, 256, 0, st>>>(df, d_gate, num_matches_thr, d_stat);
-    B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaEventRecord(T.ev[6], st));
-    B200_CUDA(A.download(out_begin, out_end, st));
-    B200_CUDA(cudaStreamSynchronize(st));
-    T.timed = true;
-    const chain::Epilogue E{who, hb, o_pose};
+    if ((rc = C.finish(sh, num_matches_thr))) return rc;
     for (int f = 0; f < n_frames; ++f)  // every check before the first write: an error writes nothing
-        if ((rc = E.check(f, lay[f], frames[f].n_keypoints_in, frames[f].kp_cap, B200_ERR_INVALID))) return rc;
+        if ((rc = C.check(f, lay[f], frames[f].n_keypoints_in, frames[f].kp_cap, B200_ERR_INVALID))) return rc;
     for (int f = 0; f < n_frames; ++f) {
         b200_robust_track_frame_t& F = frames[f];
-        const int nk = E.status(lay[f])[0];
-        const int* rs = reinterpret_cast<const int*>(hb + o_stat) + kMotionStat * (size_t)f;
+        const int nk = C.status(lay[f])[0];
+        const int* rs = C.stat(f);
         F.n_keypoints = nk;
         F.n_matches = rs[0];
         F.essential_valid = rs[1];
         F.status = rs[5] ? B200_ERR_INVALID : B200_OK;
         F.n_inliers = rs[2];
-        F.applied = reinterpret_cast<const int*>(hb + o_gate)[f];
+        F.applied = C.gate(f);
         F.n_valid = F.applied ? (uint32_t)rs[3] : 0u;
         F.tracked = F.applied ? rs[4] : 0;
         if (!F.applied) continue;  // frame_tracker.cc:105-108: the frame is not touched
-        std::memcpy(F.kp_landmark_out, hb + lay[f].klo, 4 * (size_t)nk);
-        E.pose(f, lay[f], F.last_pose_cw, F.pose_cw_out);
+        std::memcpy(F.kp_landmark_out, C.hb + lay[f].klo, 4 * (size_t)nk);
+        C.pose(f, lay[f], F.last_pose_cw, F.pose_cw_out);
     }
     return B200_OK;
 }
 
-int b200_bow_track_stage_ms(b200_matcher_t h, int stage, float* ms) { return h ? h->m.bow_timer.elapsed(stage, ms) : B200_ERR_INVALID; }
-
 // BoW-match tracking on the device (see include/b200vslam.h).  Arena of the matcher handle:
 //   [TrackFrameDev x n][PairsDev x n][per frame: x_right, frame nodes, keyframe descriptors | angles | nodes | rows | landmark positions]
 //                                                                                         -- mirrored in pinned memory, one upload
-//   [per frame: kp_landmark_out, status][poses, n_valid, status words, gates, overflow]   -- one download
+//   [poses, n_valid, status words, gates][per frame: kp_landmark_out, status][overflow]   -- one download
 //   [per frame: stage-A products, angles, match_out, n_matches, candidate lists]
 int b200_bow_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt, const b200_track_params_t* prm, uint32_t num_matches_thr,
                                int n_frames, b200_bow_track_frame_t* frames) {
     B200_RANGE("b200:track:bow");
     namespace chain = b200::chain;
     using chain::TrackFrameDev;
-    using b200::match::kMotionStat;
     using b200::match::PairsDev;
-    const char* who = "b200_bow_match_based_track";
-    if (!orb || !h || !opt || !prm || n_frames < 0) return B200_ERR_INVALID;
-    if (n_frames == 0) return B200_OK;
-    int rc = chain::check_params(who, *prm, frames && std::isfinite(prm->lowe_ratio) && prm->max_candidates >= 0);
-    if (rc) return rc;
-    auto& m = h->m;
-    chain::Extracted x;
-    if ((rc = chain::open_extracted(who, orb, m.device, &x))) return rc;
+    chain::Call C("b200_bow_match_based_track", b200::match::kBowChain);
+    const char* who = C.who;
+    int rc = C.open(orb, h, opt, prm, n_frames, [&] { return frames && std::isfinite(prm->lowe_ratio) && prm->max_candidates >= 0; });
+    if (rc || n_frames == 0) return rc;
+    const chain::Extracted& x = C.x;
     const int stride = x.stride;
     cudaStream_t st = x.st;
     const int cap = prm->max_candidates ? prm->max_candidates : 64;
@@ -2789,12 +2775,11 @@ int b200_bow_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt,
     }
     const size_t kc = (size_t)std::max(stride, 1), nf = (size_t)n_frames;
     struct Lay : chain::FrameBlocks {
-        size_t xr, node, kdesc, kang, knode, kval, pos;  // inputs
-        size_t tang, mout, nm, lists, llen;              // angles of stage A; the matcher's products
+        size_t node, kdesc, kang, knode, kval;  // inputs (with xr and pos)
+        size_t tang, mout, nm, lists, llen;     // angles of stage A; the matcher's products
     };
     std::vector<Lay> lay(n_frames);
-    b200::Layout a;
-    a.take<TrackFrameDev>(n_frames);  // at offset 0
+    b200::Layout& a = C.a;
     const size_t o_pd = a.take<PairsDev>(nf);
     for (int f = 0; f < n_frames; ++f) {
         Lay& L = lay[f];
@@ -2807,14 +2792,9 @@ int b200_bow_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt,
         L.kval = a.take(nkf);
         L.pos = a.take(24 * nkf);
     }
-    const size_t in_bytes = a.end, out_begin = a.end;
-    for (int f = 0; f < n_frames; ++f) {
-        lay[f].klo = a.take(4 * kc);
-        lay[f].status = a.take(16);
-    }
-    const size_t o_pose = a.take(8 * 16 * nf), o_nvalid = a.take(4 * nf), o_stat = a.take(4 * kMotionStat * nf), o_gate = a.take(4 * nf);
+    C.begin_outputs(lay, true);
     const size_t o_overflow = a.take(4);
-    const size_t out_end = a.end;
+    C.end_outputs();
     for (int f = 0; f < n_frames; ++f) {
         Lay& L = lay[f];
         const size_t nkf = (size_t)frames[f].n_kf_keypoints;
@@ -2827,36 +2807,27 @@ int b200_bow_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt,
     }
     size_t rs_bytes = 0;
     if ((rc = b200::match::guided_resolve_smem<PairsDev>(who, stride, &rs_bytes))) return rc;
-    if ((rc = m.arena.reserve(a.end, out_end, st))) return rc;
-    b200::match::ChainTimer& T = m.bow_timer;
-    if ((rc = T.create())) return rc;
-    b200::StagingArena& A = m.arena;
-    unsigned char *hb = A.h, *db = A.d;
-    TrackFrameDev* hf = A.host<TrackFrameDev>(0);
+    if ((rc = C.reserve())) return rc;
+    b200::StagingArena& A = C.m->arena;
+    unsigned char *hb = C.hb, *db = C.db;
     PairsDev* hp = A.host<PairsDev>(o_pd);
     const chain::TrackShared sh = chain::shared_of(*prm, 0.0);
-    std::vector<const double*> poses(n_frames);
     for (int f = 0; f < n_frames; ++f) {
         const b200_bow_track_frame_t& F = frames[f];
         const Lay& L = lay[f];
         const size_t nk = (size_t)F.n_keypoints_in, nkf = (size_t)F.n_kf_keypoints;
-        A.put(L.xr, F.kp_x_right, 4 * nk);
         A.put(L.node, F.kp_node, 4 * nk);
         A.put(L.kdesc, F.kf_desc, 32 * nkf);
         A.put(L.kang, F.kf_angle, 4 * nkf);
         A.put(L.knode, F.kf_node, 4 * nkf);
-        A.put(L.pos, F.kf_pos_w, 24 * nkf);
         // a keyframe keypoint takes part iff its landmark is live (bow_tree.cc:192-199) and a node lists it; a frame keypoint that no
         // node lists is then never a candidate, since only rows of its own node see it
         unsigned char* kval = hb + L.kval;
         for (size_t i = 0; i < nkf; ++i) kval[i] = (F.kf_valid[i] && F.kf_node[i] >= 0) ? 1 : 0;
-        poses[f] = F.last_pose_cw;
         // the landmark table is the keyframe's keypoints; kp_landmark stays null: set_landmarks replaces every slot (frame_tracker.cc:75)
-        TrackFrameDev t = chain::frame_dev(x, F.frame, F.n_keypoints_in, F.n_kf_keypoints, F.kp_x_right ? (const float*)(db + L.xr) : nullptr,
-                                           (const double*)(db + L.pos), F.last_pose_cw, L, db);
+        TrackFrameDev& t = C.frame_dev(f, F.frame, F.n_keypoints_in, F.n_kf_keypoints, F.kp_x_right, F.kf_pos_w, F.last_pose_cw, L);
         t.t_angle = (float*)(db + L.tang);
         t.match_out = (const int*)(db + L.mout);
-        hf[f] = t;
         PairsDev g{};
         g.n_queries = F.n_kf_keypoints;
         g.n_train = 0;  // set on the device by bow_set_counts_kernel
@@ -2874,38 +2845,25 @@ int b200_bow_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt,
         g.n_matches = (int*)(db + L.nm);
         hp[f] = g;
     }
-    if ((rc = m.join())) return rc;
-    B200_CUDA(cudaEventRecord(T.ev[0], st));
-    B200_CUDA(A.upload(in_bytes, st));
-    B200_CUDA(cudaMemsetAsync(db + out_begin, 0, out_end - out_begin, st));
-    const TrackFrameDev* df = A.dev<const TrackFrameDev>(0);
+    if ((rc = C.start())) return rc;
+    const TrackFrameDev* df = C.df;
     PairsDev* dp = A.dev<PairsDev>(o_pd);
-    int* d_stat = (int*)(db + o_stat);
-    int* d_gate = (int*)(db + o_gate);
     if ((rc = chain::track_stage_a(st, sh, df, n_frames, stride, 0))) return rc;
     b200::match::bow_set_counts_kernel<<<b200::ceil_div(n_frames, 128), 128, 0, st>>>(dp, df, n_frames);
-    B200_CUDA(cudaEventRecord(T.ev[1], st));
+    B200_CUDA(C.mark(1));
     b200::match::pairs_candidates_kernel<<<dim3(std::max(1, b200::ceil_div(max_kf, b200::match::kPairRows)), n_frames), b200::match::kPairRows, 0,
                                            st>>>(dp, B200_PAIRS_BOW, b200::match::pairs_list_thr(prm->lowe_ratio, false), 1, (int*)(db + o_overflow));
-    B200_CUDA(cudaEventRecord(T.ev[2], st));
+    B200_CUDA(C.mark(2));
     b200::match::guided_resolve_kernel<PairsDev><<<n_frames, 32, rs_bytes, st>>>(dp, 5, (unsigned)b200::match::kThrLow, prm->lowe_ratio);
-    B200_CUDA(cudaEventRecord(T.ev[3], st));
-    b200::match::bow_gate_kernel<<<b200::ceil_div(n_frames, 128), 128, 0, st>>>(dp, df, n_frames, num_matches_thr, d_stat, d_gate);
+    B200_CUDA(C.mark(3));
+    b200::match::bow_gate_kernel<<<b200::ceil_div(n_frames, 128), 128, 0, st>>>(dp, df, n_frames, num_matches_thr, (int*)(db + C.o_stat),
+                                                                                 (int*)(db + C.o_gate));
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaEventRecord(T.ev[4], st));
-    if ((rc = chain::track_stage_c(opt, st, sh, df, hf, poses.data(), n_frames, stride, prm->num_trials_robust, prm->num_trials, prm->num_each_iter,
-                                   (double*)(db + o_pose), (unsigned*)(db + o_nvalid), T.ev[5], d_gate)))
-        return rc;
-    b200::match::motion_discard_kernel<<<n_frames, 256, 0, st>>>(df, d_gate, num_matches_thr, d_stat);
-    B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaEventRecord(T.ev[6], st));
-    B200_CUDA(A.download(out_begin, out_end, st));
-    B200_CUDA(cudaStreamSynchronize(st));
-    T.timed = true;
-    const chain::Epilogue E{who, hb, o_pose};
+    B200_CUDA(C.mark(4));
+    if ((rc = C.finish(sh, num_matches_thr))) return rc;
     // every check before the first write: an error writes nothing
     for (int f = 0; f < n_frames; ++f)
-        if ((rc = E.check(f, lay[f], frames[f].n_keypoints_in, frames[f].kp_cap, B200_ERR_INVALID))) return rc;
+        if ((rc = C.check(f, lay[f], frames[f].n_keypoints_in, frames[f].kp_cap, B200_ERR_INVALID))) return rc;
     if (*reinterpret_cast<const int*>(hb + o_overflow) > 0) {
         b200::set_error("%s: a keyframe keypoint kept %d gated candidates, max_candidates is %d", who, *reinterpret_cast<const int*>(hb + o_overflow),
                         cap);
@@ -2913,16 +2871,16 @@ int b200_bow_match_based_track(b200_orb_t orb, b200_matcher_t h, b200_lba_t opt,
     }
     for (int f = 0; f < n_frames; ++f) {
         b200_bow_track_frame_t& F = frames[f];
-        const int nk = E.status(lay[f])[0];
-        const int* bs = reinterpret_cast<const int*>(hb + o_stat) + kMotionStat * (size_t)f;
+        const int nk = C.status(lay[f])[0];
+        const int* bs = C.stat(f);
         F.n_keypoints = nk;
         F.n_matches = bs[0];
-        F.applied = reinterpret_cast<const int*>(hb + o_gate)[f];
+        F.applied = C.gate(f);
         F.n_valid = F.applied ? (uint32_t)bs[3] : 0u;
         F.tracked = F.applied ? bs[4] : 0;
         if (!F.applied) continue;  // frame_tracker.cc:69-72: the frame is not touched
         std::memcpy(F.kp_landmark_out, hb + lay[f].klo, 4 * (size_t)nk);
-        E.pose(f, lay[f], F.last_pose_cw, F.pose_cw_out);
+        C.pose(f, lay[f], F.last_pose_cw, F.pose_cw_out);
     }
     return B200_OK;
 }
