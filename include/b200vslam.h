@@ -853,6 +853,61 @@ typedef struct b200_depth_landmarks_problem {
 } b200_depth_landmarks_problem_t;
 int b200_depth_landmarks(b200_matcher_t h, int n_problems, b200_depth_landmarks_problem_t* problems);
 
+/* Keyframe culling: module::local_map_cleaner::remove_redundant_keyframes (module/local_map_cleaner.cc:68-193) with the observation
+ * erasure of keyframe::prepare_for_erasing and landmark::erase_observation (data/keyframe.cc:613-660, data/landmark.cc:124-160), for
+ * many maps in one upload, one launch (one CTA per problem), one download and one synchronisation on the matcher's stream.
+ * The caller gathers under map_database::mtx_database_:
+ *   - the covisibilities, graph_node_->get_top_n_covisibilities(top_n) in that order (a covisibility's position is its rank);
+ *   - a landmark table holding every landmark that a covisibility's keypoint lists, once, in CSR form: per landmark its observations
+ *     as get_observations() walks them, each with the observer's rank (-1 for any keyframe that is not a listed covisibility, the
+ *     current keyframe included), the octave undist_keypts_.at(obs.second).octave and the weight (2 when the observer's
+ *     stereo_x_right_ is not empty and stereo_x_right_.at(obs.second) >= 0, else 1: landmark::add_observation, landmark.cc:116-121).
+ *     The starting num_observations() of a landmark is the sum of its weights.
+ * Ranks run in order.  A rank is skipped (skipped = 1) for the spanning root and (skipped = 2) for the recent window
+ * id <= cur_id && cur_id <= id + 2 in uint32_t arithmetic.  Otherwise every keypoint whose landmark is live and whose depth passes
+ * (depth == NULL, or !(depth < 0 || depth_thr < depth) in double) counts in n_valid; one whose landmark has num_observations() > 3 and
+ * at least 3 live observations by other keyframes at an octave <= its own + 1 counts in n_redundant.  The keypoint's own octave is
+ * that of its landmark's observation by this rank.  The rank is removed when
+ * redundant_obs_ratio_thr <= (double)((float)n_redundant / (float)n_valid) (so 9/10 against 0.9 is kept and 0/0 is kept), and its
+ * observations are then erased before the next rank counts: each live landmark it lists loses that observation and its weight, and a
+ * landmark left with no observation is discarded (will_be_erased), so no later rank counts it.
+ * The caller makes the reference's early return (redundant_obs_ratio_thr < 0 or top_n <= 0: no call) and applies each removed rank's
+ * prepare_for_erasing in rank order.  A keyframe that set_not_to_be_erased() pinned is not erased by prepare_for_erasing although the
+ * reference counts it as removed; the device's later ranks assumed it was.  The caller therefore checks will_be_erased() after each
+ * prepare_for_erasing, and when a removed keyframe was not erased it gathers again and calls again for the ranks after it: the
+ * reference's count is then the removed ranks of the first call up to that keyframe plus the second call's n_removed.
+ * B200_ERR_INVALID, with nothing written, for: a negative count; a null required pointer; obs_offsets not starting at 0 or descending;
+ * an obs_rank outside [-1, n_covisibilities), an obs_weight other than 1 or 2, or a kp_landmark outside [-1, n_landmarks); and a
+ * landmark that a covisibility's keypoints list a number of times other than the number of its observations by that rank, unless
+ * both are 0 -- each listed landmark must name the rank exactly once and each observation by a rank must be listed by exactly one
+ * keypoint of it. */
+typedef struct b200_cull_keyframe {
+    uint32_t id;                    /* keyframe::id_ */
+    int32_t is_root;                /* graph_node_->is_spanning_root() */
+    int32_t n_keypoints;            /* frm_obs_.undist_keypts_.size() */
+    const int32_t* kp_landmark;     /* get_landmarks()[idx] as a landmark-table row; -1 when null or will_be_erased() */
+    const float* depth;             /* frm_obs_.depths_ when depth_is_available(), else NULL */
+    double depth_thr;               /* camera_->depth_thr_ */
+    /* out */
+    int32_t n_valid, n_redundant;   /* count_redundant_observations; 0 for a skipped rank */
+    int32_t skipped;                /* 0, 1 (spanning root) or 2 (recent window) */
+    int32_t removed;                /* 1 when the rank is removed */
+} b200_cull_keyframe_t;
+typedef struct b200_cull_problem {
+    uint32_t cur_id;                /* cur_keyfrm->id_ */
+    double redundant_obs_ratio_thr; /* local_map_cleaner::redundant_obs_ratio_thr_ (default 0.9) */
+    int32_t n_covisibilities;
+    b200_cull_keyframe_t* covisibilities; /* in rank order */
+    int32_t n_landmarks;
+    const int32_t* obs_offsets;     /* n_landmarks + 1 (may be NULL when n_landmarks is 0) */
+    const int32_t* obs_rank;        /* obs_offsets[n_landmarks] entries each */
+    const int32_t* obs_octave;
+    const uint8_t* obs_weight;
+    int32_t n_removed;              /* out: the reference's return value */
+    int32_t status;                 /* out: B200_OK once the problem has run */
+} b200_cull_problem_t;
+int b200_remove_redundant_keyframes(b200_matcher_t h, int n_problems, b200_cull_problem_t* problems);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Relocalisation's PnP: solve::pnp_solver (src/stella_vslam/solve/pnp_solver.{h,cc}) -- EPnP (Lepetit et al., IJCV 2009) inside
  * RANSAC -- for many problems (lost frame x candidate keyframe) in one launch sequence on the b200_lba_t handle's stream, so the pose

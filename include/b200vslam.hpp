@@ -15,6 +15,7 @@
 //   b200::solve::essential_solver         <-> stella_vslam::solve::essential_solver         (solve/essential_solver.h)
 //   b200::initialize::perspective / bearing_vector <-> stella_vslam::initialize::perspective / bearing_vector (initialize/*.h)
 //   b200::module::depth_landmarks         <-> the depth branches of module::keyframe_inserter and module::initializer
+//   b200::module::local_map_cleaner       <-> stella_vslam::module::local_map_cleaner::remove_redundant_keyframes (module/local_map_cleaner.h)
 #pragma once
 
 #include <cmath>
@@ -385,6 +386,31 @@ public:
     }
 
 private:
+    match::device_matcher m_;
+};
+
+// module::local_map_cleaner's keyframe culling (module/local_map_cleaner.cc:68-193) on gathered tables (b200_remove_redundant_keyframes),
+// for many maps in one call.  The caller gathers each problem from get_top_n_covisibilities(top_n_covisibilities_to_search()), applies
+// prepare_for_erasing to the removed ranks in rank order, and calls again for the ranks after a removed keyframe it could not erase.
+class local_map_cleaner {
+public:
+    explicit local_map_cleaner(double redundant_obs_ratio_thr = 0.9, unsigned int top_n_covisibilities_to_search = 30, int device = 0)
+        : redundant_obs_ratio_thr_(redundant_obs_ratio_thr), top_n_covisibilities_to_search_(top_n_covisibilities_to_search), m_(device) {}
+    unsigned int top_n_covisibilities_to_search() const { return top_n_covisibilities_to_search_; }
+    // Sets each problem's threshold, runs them and returns each n_removed; the per-rank results are in the problems' covisibilities.
+    // The reference's early return (a negative threshold or top_n of 0) returns zeros without a call.
+    std::vector<unsigned int> remove_redundant_keyframes(std::vector<b200_cull_problem_t>& problems) const {
+        std::vector<unsigned int> n_removed(problems.size(), 0);
+        if (redundant_obs_ratio_thr_ < 0.0 || top_n_covisibilities_to_search_ == 0 || problems.empty()) return n_removed;
+        for (auto& p : problems) p.redundant_obs_ratio_thr = redundant_obs_ratio_thr_;
+        check(b200_remove_redundant_keyframes(m_.get(), (int)problems.size(), problems.data()), "b200_remove_redundant_keyframes");
+        for (size_t k = 0; k < problems.size(); ++k) n_removed[k] = (unsigned int)problems[k].n_removed;
+        return n_removed;
+    }
+
+private:
+    double redundant_obs_ratio_thr_;
+    unsigned int top_n_covisibilities_to_search_;
     match::device_matcher m_;
 };
 

@@ -158,7 +158,7 @@ SYMBOLS = [
     "b200_match_bruteforce_device", "b200_match_guided", "b200_match_cross_check", "b200_match_pairs", "b200_stereo_compute", "b200_landmark_descriptors", "b200_landmark_geometry", "b200_matcher_set_stream", "b200_matcher_sync", "b200_matcher_set_async_resolve", "b200_matcher_join", "b200_matcher_enable_timing", "b200_matcher_stage_ms",
     "b200_lba_create", "b200_lba_destroy", "b200_lba_solve", "b200_lba_solve_batch", "b200_pose_optimize", "b200_lba_last_profile", "b200_lba_enable_profile", "b200_lba_kernel_ms",
     "b200_global_ba_solve", "b200_track_local_map", "b200_track_stage_ms", "b200_motion_based_track", "b200_motion_track_stage_ms", "b200_bow_match_based_track", "b200_bow_track_stage_ms", "b200_orb_export_keyframe_blobs", "b200_keyframe_blob_to_keypoints",
-    "b200_triangulate_pairs", "b200_create_new_landmarks", "b200_rgbd_depths", "b200_depth_landmarks",
+    "b200_triangulate_pairs", "b200_create_new_landmarks", "b200_rgbd_depths", "b200_depth_landmarks", "b200_remove_redundant_keyframes",
     "b200_rectifier_create", "b200_rectifier_destroy", "b200_rectifier_set_stream", "b200_rectifier_maps", "b200_stereo_rectify",
     "b200_stereo_rectify_device",
     "b200_pnp_ransac", "b200_epnp_compute_pose", "b200_mt19937_seed", "b200_mt19937_next", "b200_pnp_draw_min_sets",

@@ -1517,6 +1517,121 @@ __global__ void __launch_bounds__(kDepthLmThreads) depth_landmarks_kernel(const 
     if (tid == 0) *P.n_created = base_out;
 }
 
+// b200_remove_redundant_keyframes: one CTA per problem walks the ranks in order.  The live landmark state (weighted observation
+// count, observation count, per-observation erased flag) sits in device scratch owned by that CTA; a rank's erasure pass writes it
+// and __syncthreads publishes it to the next rank's counting pass.  It is read with __ldcg so that no thread sees an L1 copy older
+// than another thread's atomic.  Each landmark is listed at most once per rank (checked on the host), so the erasure pass touches
+// every landmark from one thread only.
+struct CullKfDev {
+    unsigned id;
+    int is_root, n;
+    const int* kp_lm;
+    const float* depth;  // may be null
+    double depth_thr;
+    int* out;  // n_valid, n_redundant, skipped, removed
+};
+struct CullDev {
+    unsigned cur_id;
+    int n_cov, n_lm;
+    double thr;
+    const CullKfDev* kf;
+    const int *off, *rank, *octave;
+    const unsigned char* weight;
+    int *live_weight, *live_count;  // scratch, n_lm each
+    unsigned char* erased;          // scratch, one per observation
+    int* n_removed;
+};
+constexpr int kCullThreads = 512;
+
+// the observation of landmark [b, e) by rank r that is still live (the host checked that there is exactly one)
+__device__ __forceinline__ int cull_own_obs(const CullDev& P, int b, int e, int r) {
+    for (int j = b; j < e; ++j)
+        if (P.rank[j] == r && !__ldcg(P.erased + j)) return j;
+    return -1;
+}
+
+__global__ void __launch_bounds__(kCullThreads) cull_keyframes_kernel(const CullDev* __restrict__ probs) {
+    __shared__ int s_warp[2][kCullThreads / 32];
+    __shared__ int s_removed;
+    const CullDev& P = probs[blockIdx.x];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    for (int l = tid; l < P.n_lm; l += kCullThreads) {
+        int w = 0;
+        for (int j = P.off[l]; j < P.off[l + 1]; ++j) w += P.weight[j];
+        P.live_weight[l] = w;
+        P.live_count[l] = P.off[l + 1] - P.off[l];
+    }
+    for (int j = tid; j < P.off[P.n_lm]; j += kCullThreads) P.erased[j] = 0;
+    int n_removed = 0;
+    __syncthreads();
+    for (int r = 0; r < P.n_cov; ++r) {
+        const CullKfDev& K = P.kf[r];
+        // local_map_cleaner.cc:83-90, unsigned as the reference
+        const int skipped = K.is_root ? 1 : (K.id <= P.cur_id && P.cur_id <= K.id + 2u) ? 2 : 0;
+        if (skipped) {
+            if (tid == 0) K.out[2] = skipped;
+            continue;
+        }
+        // count_redundant_observations (local_map_cleaner.cc:123-193)
+        int nv = 0, nr = 0;
+        for (int i = tid; i < K.n; i += kCullThreads) {
+            const int l = K.kp_lm[i];
+            if (l < 0 || __ldcg(P.live_count + l) == 0) continue;
+            if (K.depth) {
+                const float d = K.depth[i];
+                if (d < 0.0 || K.depth_thr < d) continue;
+            }
+            ++nv;
+            if (__ldcg(P.live_weight + l) <= 3) continue;
+            const int b = P.off[l], e = P.off[l + 1];
+            const long long octave = P.octave[cull_own_obs(P, b, e, r)];
+            int better = 0;
+            for (int j = b; j < e; ++j) {
+                if (P.rank[j] == r || __ldcg(P.erased + j)) continue;
+                if (P.octave[j] <= octave + 1 && ++better >= 3) break;
+            }
+            nr += better >= 3;
+        }
+#pragma unroll
+        for (int d = 16; d > 0; d >>= 1) {
+            nv += __shfl_xor_sync(0xffffffffu, nv, d);
+            nr += __shfl_xor_sync(0xffffffffu, nr, d);
+        }
+        if (lane == 0) {
+            s_warp[0][warp] = nv;
+            s_warp[1][warp] = nr;
+        }
+        __syncthreads();
+        if (tid == 0) {
+            int v = 0, red = 0;
+            for (int w = 0; w < kCullThreads / 32; ++w) {
+                v += s_warp[0][w];
+                red += s_warp[1][w];
+            }
+            // local_map_cleaner.cc:99: float / float, compared as double
+            const int rm = P.thr <= (double)__fdiv_rn((float)(unsigned)red, (float)(unsigned)v);
+            K.out[0] = v;
+            K.out[1] = red;
+            K.out[3] = rm;
+            s_removed = rm;
+        }
+        __syncthreads();
+        if (!s_removed) continue;  // uniform: no thread writes s_removed before the next rank's __syncthreads
+        ++n_removed;
+        // keyframe::prepare_for_erasing -> landmark::erase_observation for every live landmark of the rank
+        for (int i = tid; i < K.n; i += kCullThreads) {
+            const int l = K.kp_lm[i];
+            if (l < 0 || __ldcg(P.live_count + l) == 0) continue;
+            const int j = cull_own_obs(P, P.off[l], P.off[l + 1], r);
+            P.erased[j] = 1;
+            atomicSub(P.live_weight + l, (int)P.weight[j]);
+            atomicSub(P.live_count + l, 1);  // 0 = discarded
+        }
+        __syncthreads();
+    }
+    if (tid == 0) *P.n_removed = n_removed;
+}
+
 // The stage boundaries of one tracking chain's last call: ev[0] before the upload, ev[6] after the last kernel
 struct ChainTimer {
     cudaEvent_t ev[7] = {};
@@ -3339,6 +3454,167 @@ int b200_depth_landmarks(b200_matcher_t h, int n_problems, b200_depth_landmarks_
         std::memcpy(P.max_valid_dist, A.host(L.hi), 4 * K);
     }
     return first_bad;
+}
+
+namespace {
+
+// b200_remove_redundant_keyframes' input check: ranges, then per rank that the landmarks its keypoints list and the landmarks with an
+// observation by it are the same set, each listed and observed exactly once.  Returns B200_OK or B200_ERR_INVALID with the error set.
+int check_cull_problem(int p, const b200_cull_problem_t& P) {
+    auto bad = [p](const char* what) {
+        b200::set_error("b200_remove_redundant_keyframes: problem %d: %s", p, what);
+        return B200_ERR_INVALID;
+    };
+    if (P.n_covisibilities < 0 || P.n_landmarks < 0) return bad("negative count");
+    if ((P.n_covisibilities > 0 && !P.covisibilities) || (P.n_landmarks > 0 && !P.obs_offsets)) return bad("null covisibilities or obs_offsets");
+    const int L = P.n_landmarks;
+    if (L > 0 && P.obs_offsets[0] != 0) return bad("obs_offsets[0] is not 0");
+    for (int l = 0; l < L; ++l)
+        if (P.obs_offsets[l + 1] < P.obs_offsets[l]) return bad("obs_offsets descend");
+    const int total = L > 0 ? P.obs_offsets[L] : 0;
+    if (total > 0 && (!P.obs_rank || !P.obs_octave || !P.obs_weight)) return bad("null observation table");
+    std::vector<int> rank_start((size_t)P.n_covisibilities + 1, 0);
+    for (int j = 0; j < total; ++j) {
+        if (P.obs_rank[j] < -1 || P.obs_rank[j] >= P.n_covisibilities) return bad("obs_rank out of range");
+        if (P.obs_weight[j] != 1 && P.obs_weight[j] != 2) return bad("obs_weight is not 1 or 2");
+        if (P.obs_rank[j] >= 0) ++rank_start[P.obs_rank[j] + 1];
+    }
+    for (int r = 0; r < P.n_covisibilities; ++r) rank_start[r + 1] += rank_start[r];
+    std::vector<int> by_rank((size_t)rank_start[P.n_covisibilities]), fill(rank_start.begin(), rank_start.end() - 1);
+    for (int l = 0; l < L; ++l)
+        for (int j = P.obs_offsets[l]; j < P.obs_offsets[l + 1]; ++j)
+            if (P.obs_rank[j] >= 0) by_rank[fill[P.obs_rank[j]]++] = l;
+    std::vector<int> mark((size_t)L, -1);
+    for (int r = 0; r < P.n_covisibilities; ++r) {
+        const b200_cull_keyframe_t& K = P.covisibilities[r];
+        if (K.n_keypoints < 0 || (K.n_keypoints > 0 && !K.kp_landmark)) return bad("bad keypoint count or null kp_landmark");
+        int listed = 0;
+        for (int i = 0; i < K.n_keypoints; ++i) {
+            const int l = K.kp_landmark[i];
+            if (l < -1 || l >= L) return bad("kp_landmark out of range");
+            if (l < 0) continue;
+            if (mark[l] == r) return bad("a landmark is listed by two keypoints of one covisibility");
+            mark[l] = r;
+            ++listed;
+        }
+        if (listed != rank_start[r + 1] - rank_start[r]) return bad("a covisibility's keypoints and its observations disagree");
+        for (int k = rank_start[r]; k < rank_start[r + 1]; ++k) {
+            if (mark[by_rank[k]] != r) return bad("a covisibility's keypoints and its observations disagree");
+            mark[by_rank[k]] = -1;  // a second observation by r of the same landmark fails here
+        }
+    }
+    return B200_OK;
+}
+
+}  // namespace
+
+int b200_remove_redundant_keyframes(b200_matcher_t h, int n_problems, b200_cull_problem_t* problems) {
+    B200_RANGE("b200:match:remove_redundant_keyframes");
+    if (!h || n_problems < 0 || (n_problems > 0 && !problems)) return B200_ERR_INVALID;
+    for (int p = 0; p < n_problems; ++p)
+        if (int rc = check_cull_problem(p, problems[p])) return rc;
+    if (n_problems == 0) return B200_OK;
+    using b200::match::CullDev;
+    using b200::match::CullKfDev;
+    // one staging block: the problem table, then per problem its covisibility table, observation table and keypoint arrays; the
+    // outputs (n_removed, then n_valid / n_redundant / skipped / removed per rank); the device-only live landmark state
+    struct Lay { size_t kf, off, rank, octave, weight, out, live_w, live_c, erased; std::vector<size_t> kp_lm, depth; };
+    std::vector<Lay> lay(n_problems);
+    b200::Layout a;
+    a.take<CullDev>(n_problems);  // at offset 0
+    for (int p = 0; p < n_problems; ++p) {
+        const b200_cull_problem_t& P = problems[p];
+        const size_t L = (size_t)P.n_landmarks, total = L ? (size_t)P.obs_offsets[L] : 0;
+        Lay& Y = lay[p];
+        Y.kf = a.take<CullKfDev>(P.n_covisibilities);
+        Y.off = a.take<int>(L + 1);
+        Y.rank = a.take<int>(total);
+        Y.octave = a.take<int>(total);
+        Y.weight = a.take(total);
+        for (int r = 0; r < P.n_covisibilities; ++r) {
+            const b200_cull_keyframe_t& K = P.covisibilities[r];
+            Y.kp_lm.push_back(a.take<int>(K.n_keypoints));
+            Y.depth.push_back(K.depth ? a.take<float>(K.n_keypoints) : 0);
+        }
+    }
+    const size_t in_bytes = a.end;
+    for (int p = 0; p < n_problems; ++p) lay[p].out = a.take<int>(1 + 4 * (size_t)problems[p].n_covisibilities);
+    const size_t out_end = a.end;
+    for (int p = 0; p < n_problems; ++p) {
+        const size_t L = (size_t)problems[p].n_landmarks;
+        lay[p].live_w = a.take<int>(L);
+        lay[p].live_c = a.take<int>(L);
+        lay[p].erased = a.take(L ? (size_t)problems[p].obs_offsets[L] : 0);
+    }
+    auto& m = h->m;
+    B200_CUDA(cudaSetDevice(m.device));
+    cudaStream_t st = m.stream;
+    int rc;
+    if ((rc = m.arena.reserve(a.end, out_end, st))) return rc;
+    b200::StagingArena& A = m.arena;
+    CullDev* dev = A.host<CullDev>(0);
+    for (int p = 0; p < n_problems; ++p) {
+        const b200_cull_problem_t& P = problems[p];
+        const Lay& Y = lay[p];
+        const size_t L = (size_t)P.n_landmarks, total = L ? (size_t)P.obs_offsets[L] : 0;
+        CullDev& D = dev[p];
+        std::memset(&D, 0, sizeof(D));
+        D.cur_id = P.cur_id;
+        D.n_cov = P.n_covisibilities;
+        D.n_lm = P.n_landmarks;
+        D.thr = P.redundant_obs_ratio_thr;
+        D.kf = A.dev<const CullKfDev>(Y.kf);
+        if (L) A.put(Y.off, P.obs_offsets, 4 * (L + 1));
+        else *A.host<int>(Y.off) = 0;
+        A.put(Y.rank, P.obs_rank, 4 * total);
+        A.put(Y.octave, P.obs_octave, 4 * total);
+        A.put(Y.weight, P.obs_weight, total);
+        D.off = A.dev<const int>(Y.off);
+        D.rank = A.dev<const int>(Y.rank);
+        D.octave = A.dev<const int>(Y.octave);
+        D.weight = A.dev<const unsigned char>(Y.weight);
+        D.live_weight = A.dev<int>(Y.live_w);
+        D.live_count = A.dev<int>(Y.live_c);
+        D.erased = A.dev<unsigned char>(Y.erased);
+        D.n_removed = A.dev<int>(Y.out);
+        CullKfDev* kf = A.host<CullKfDev>(Y.kf);
+        for (int r = 0; r < P.n_covisibilities; ++r) {
+            const b200_cull_keyframe_t& K = P.covisibilities[r];
+            CullKfDev& E = kf[r];
+            std::memset(&E, 0, sizeof(E));
+            E.id = K.id;
+            E.is_root = K.is_root != 0;
+            E.n = K.n_keypoints;
+            E.depth_thr = K.depth_thr;
+            A.put(Y.kp_lm[r], K.kp_landmark, 4 * (size_t)K.n_keypoints);
+            E.kp_lm = A.dev<const int>(Y.kp_lm[r]);
+            if (K.depth) {
+                A.put(Y.depth[r], K.depth, 4 * (size_t)K.n_keypoints);
+                E.depth = A.dev<const float>(Y.depth[r]);
+            }
+            E.out = A.dev<int>(Y.out) + 1 + 4 * r;
+        }
+    }
+    B200_CUDA(A.upload(in_bytes, st));
+    B200_CUDA(cudaMemsetAsync(A.dev(in_bytes), 0, out_end - in_bytes, st));
+    b200::match::cull_keyframes_kernel<<<n_problems, b200::match::kCullThreads, 0, st>>>(A.dev<const CullDev>(0));
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(A.download(in_bytes, out_end, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    for (int p = 0; p < n_problems; ++p) {
+        b200_cull_problem_t& P = problems[p];
+        const int* o = A.host<const int>(lay[p].out);
+        P.n_removed = o[0];
+        for (int r = 0; r < P.n_covisibilities; ++r) {
+            b200_cull_keyframe_t& K = P.covisibilities[r];
+            K.n_valid = o[1 + 4 * r];
+            K.n_redundant = o[2 + 4 * r];
+            K.skipped = o[3 + 4 * r];
+            K.removed = o[4 + 4 * r];
+        }
+        P.status = B200_OK;
+    }
+    return B200_OK;
 }
 
 int b200_match_cross_check(const int32_t* idx2_in_1, int n1, const int32_t* idx1_in_2, int n2, int32_t* mutual_out, int32_t* n_mutual) {

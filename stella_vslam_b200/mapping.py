@@ -1,6 +1,7 @@
 """Host-side mirror of the mapping module's landmark creation: module::two_view_triangulator
 (src/stella_vslam/module/two_view_triangulator.{h,cc}) and the numeric chain of mapping_module::create_new_landmarks
-(match_for_triangulation per covisibility, then triangulation; src/stella_vslam/mapping_module.cc).
+(match_for_triangulation per covisibility, then triangulation; src/stella_vslam/mapping_module.cc), the depth-seeded landmarks, and
+the keyframe culling of module::local_map_cleaner::remove_redundant_keyframes on gathered tables.
 
 Keyframes are dicts in the shape of workloads.synth.make_keyframe_pair, extended with the triangulator's fields:
     pose_cw, pose_wc (4x4), model (0 perspective family / 1 equirectangular), fx, fy, cx, cy, fx_inv, fy_inv, focal_x_baseline,
@@ -252,6 +253,72 @@ def depth_landmarks(problems, device=0, raise_on_error=True):
     return [dict({f: v[:arr[k].n_created].copy() for f, v in o.items()}, status=int(arr[k].status)) for k, o in enumerate(outs)]
 
 
+class CullKeyframe(C.Structure):
+    """b200_cull_keyframe_t."""
+    _fields_ = [("id", C.c_uint32), ("is_root", C.c_int32), ("n_keypoints", C.c_int32), ("kp_landmark", C.c_void_p), ("depth", C.c_void_p),
+                ("depth_thr", C.c_double), ("n_valid", C.c_int32), ("n_redundant", C.c_int32), ("skipped", C.c_int32), ("removed", C.c_int32)]
+
+
+class CullProblem(C.Structure):
+    """b200_cull_problem_t."""
+    _fields_ = [("cur_id", C.c_uint32), ("redundant_obs_ratio_thr", C.c_double), ("n_covisibilities", C.c_int32),
+                ("covisibilities", C.POINTER(CullKeyframe)), ("n_landmarks", C.c_int32), ("obs_offsets", C.c_void_p), ("obs_rank", C.c_void_p),
+                ("obs_octave", C.c_void_p), ("obs_weight", C.c_void_p), ("n_removed", C.c_int32), ("status", C.c_int32)]
+
+
+CULL_SKIPPED_ROOT, CULL_SKIPPED_RECENT = 1, 2
+
+
+def pack_cull_problems(problems):
+    """Flat culling tables -> (CullProblem array, keep-alive list).  Each problem is a dict: cur_id, redundant_obs_ratio_thr,
+    covisibilities (rank order; each a dict of id, is_root, kp_landmark, depth (None when the keyframe has no depths), depth_thr),
+    obs_offsets, obs_rank, obs_octave, obs_weight (the landmark table in CSR form, b200_cull_problem_t)."""
+    keep, arr = [], (CullProblem * max(len(problems), 1))()
+    for k, pr in enumerate(problems):
+        P = arr[k]
+        P.cur_id = int(pr["cur_id"])
+        P.redundant_obs_ratio_thr = float(pr["redundant_obs_ratio_thr"])
+        covs = pr["covisibilities"]
+        kfs = (CullKeyframe * max(len(covs), 1))()
+        keep.append(kfs)
+        for r, cv in enumerate(covs):
+            K = kfs[r]
+            K.id, K.is_root = int(cv["id"]), int(bool(cv.get("is_root", False)))
+            K.n_keypoints = len(cv["kp_landmark"])
+            K.kp_landmark = _arr(keep, cv["kp_landmark"], np.int32)
+            K.depth = _arr(keep, cv.get("depth"), np.float32)
+            K.depth_thr = float(cv.get("depth_thr", 0.0))
+        P.n_covisibilities, P.covisibilities = len(covs), kfs
+        off = np.asarray(pr["obs_offsets"], np.int32)
+        P.n_landmarks = len(off) - 1
+        P.obs_offsets = _arr(keep, off, np.int32)
+        P.obs_rank, P.obs_octave = _arr(keep, pr["obs_rank"], np.int32), _arr(keep, pr["obs_octave"], np.int32)
+        P.obs_weight = _arr(keep, pr["obs_weight"], np.uint8)
+    return arr, keep
+
+
+def cull_results(arr, problems):
+    """Per problem dict(n_removed, status, skipped, n_valid, n_redundant, removed) (per-rank int arrays) read from a CullProblem array."""
+    out = []
+    for k, pr in enumerate(problems):
+        P, n = arr[k], len(pr["covisibilities"])
+        d = dict(n_removed=int(P.n_removed), status=int(P.status))
+        for f in ("skipped", "n_valid", "n_redundant", "removed"):
+            d[f] = np.array([getattr(P.covisibilities[r], f) for r in range(n)], np.int64)
+        out.append(d)
+    return out
+
+
+def remove_redundant_keyframes(problems, device=0):
+    """b200_remove_redundant_keyframes: local_map_cleaner::remove_redundant_keyframes' decisions for many maps in one launch, on flat
+    tables as pack_cull_problems takes them (workloads.synth.gather_cull_problem builds them from an object-graph map).  The caller
+    makes the reference's early return (redundant_obs_ratio_thr < 0 or no covisibility to search).  Returns cull_results."""
+    arr, _keep = pack_cull_problems(problems)
+    _setup()
+    check(lib().b200_remove_redundant_keyframes(_matcher(device), len(problems), arr))
+    return cull_results(arr, problems)
+
+
 _argtypes_set = False
 
 
@@ -263,4 +330,5 @@ def _setup():
     L.b200_triangulate_pairs.argtypes = [C.c_void_p, C.c_int, C.POINTER(TriangulateProblem)]
     L.b200_create_new_landmarks.argtypes = [C.c_void_p, C.c_int, C.POINTER(NewLandmarksProblem), C.c_float, C.c_float, C.c_float, C.c_int]
     L.b200_depth_landmarks.argtypes = [C.c_void_p, C.c_int, C.POINTER(DepthLandmarksProblem)]
+    L.b200_remove_redundant_keyframes.argtypes = [C.c_void_p, C.c_int, C.POINTER(CullProblem)]
     _argtypes_set = True

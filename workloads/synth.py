@@ -1308,3 +1308,84 @@ def make_rgbd_frames(w=640, h=480, seed=0, depthmap_factor=5000.0, n_planes=4, h
     d32[special & (kinds == 1)] = -rng.uniform(0.1, 5.0, int((special & (kinds == 1)).sum())).astype(np.float32)
     d32[special & (kinds == 2)] = np.inf
     return gray, d16, d32
+
+
+def make_cull_map(rng, n_covisibilities=30, n_keypoints=2000, observers=8, landmark_frac=0.8, redundant_frac=0.5, stereo_frac=0.3,
+                  erased_frac=0.02, n_others=6, cur_id=1000, depth_thr=5.0):
+    """A covisibility neighbourhood of a new keyframe as local_map_cleaner::remove_redundant_keyframes sees it, as an object graph:
+    dict(cur_id, keyframes {id: keyframe}, landmarks [landmark], covisibilities [ids in rank order]).
+      keyframe: id, is_root, octave (undist_keypts_ octaves), x_right / depth (None without stereo), depth_thr, landmarks (landmark
+                index per keypoint, -1 for none), will_be_erased, cannot_be_erased;
+      landmark: observations {keyframe id: keypoint index} in insertion order, num_observations (stereo observations count 2),
+                will_be_erased.
+    The covisibilities' ids are spread below cur_id with a few in the recent window and above it; the oldest is the spanning root with
+    probability 1/2.  Besides them, cur_id and `n_others` keyframes observe landmarks (rank -1).  A landmark has about `observers`
+    observers.  A share `redundant_frac` of the keyframes sees its keypoints at a raised floor octave, which makes them redundant
+    against the other observers; with the observation counts falling as keyframes are erased, some ranks are removed and some later
+    ones are kept only because of an earlier removal.  Stereo keyframes carry x_right (about 70 % matched, weight 2) and depths in
+    [-1, 1.5 depth_thr) with some exactly at depth_thr."""
+    pool = rng.choice(np.arange(max(cur_id - 4 * n_covisibilities - n_others, 0), min(cur_id + 4, 1 << 32)), n_covisibilities + n_others + 1, replace=False)
+    pool = [int(k) for k in pool if k != cur_id][:n_covisibilities + n_others]
+    covs = pool[:n_covisibilities]
+    ids = covs + pool[n_covisibilities:] + [cur_id]
+    root = min(covs) if covs and rng.random() < 0.5 else None
+    keyframes = {}
+    for kid in ids:
+        floor = int(rng.integers(0, 7)) if rng.random() < redundant_frac else 0
+        kf = dict(id=kid, is_root=kid == root, octave=rng.integers(floor, 8, n_keypoints).astype(np.int32), x_right=None, depth=None,
+                  depth_thr=float(depth_thr), landmarks=np.full(n_keypoints, -1, np.int64), will_be_erased=False, cannot_be_erased=False)
+        if rng.random() < stereo_frac:
+            kf["x_right"] = np.where(rng.random(n_keypoints) < 0.7, rng.uniform(0.0, 640.0, n_keypoints), -1.0).astype(np.float32)
+            d = rng.uniform(-1.0, 1.5 * depth_thr, n_keypoints)
+            d[rng.random(n_keypoints) < 0.05] = depth_thr
+            kf["depth"] = d.astype(np.float32)
+        keyframes[kid] = kf
+    free = {kid: list(rng.permutation(n_keypoints)) for kid in ids}
+    landmarks = []
+    for _ in range(int(len(ids) * n_keypoints * landmark_frac / observers)):
+        k = int(min(len(ids), 1 + rng.poisson(observers - 1)))
+        obs = {}
+        for o in rng.choice(len(ids), k, replace=False):
+            kid = ids[int(o)]
+            if free[kid]:
+                obs[kid] = int(free[kid].pop())
+        if not obs:
+            continue
+        li = len(landmarks)
+        num = 0
+        for kid, idx in obs.items():
+            keyframes[kid]["landmarks"][idx] = li
+            xr = keyframes[kid]["x_right"]
+            num += 2 if xr is not None and 0 <= xr[idx] else 1
+        landmarks.append(dict(observations=obs, num_observations=num, will_be_erased=bool(rng.random() < erased_frac)))
+    return dict(cur_id=cur_id, keyframes=keyframes, landmarks=landmarks, covisibilities=covs)
+
+
+def gather_cull_problem(cull_map, covisibilities=None, redundant_obs_ratio_thr=0.9):
+    """The flat tables of b200_remove_redundant_keyframes (mapping.pack_cull_problems' dict) for an object-graph map of make_cull_map,
+    as the reference-side adapter gathers them: the covisibilities (default: the map's list) in rank order, and every live landmark
+    their keypoints list once, with its observations by any keyframe (rank -1 outside the list)."""
+    keyframes, landmarks = cull_map["keyframes"], cull_map["landmarks"]
+    covs = cull_map["covisibilities"] if covisibilities is None else list(covisibilities)
+    rank = {kid: r for r, kid in enumerate(covs)}
+    rows = {}
+    out_covs = []
+    for kid in covs:
+        kf = keyframes[kid]
+        kl = np.full(len(kf["landmarks"]), -1, np.int32)
+        for idx in np.flatnonzero(kf["landmarks"] >= 0):
+            li = int(kf["landmarks"][idx])
+            if not landmarks[li]["will_be_erased"]:
+                kl[idx] = rows.setdefault(li, len(rows))
+        out_covs.append(dict(id=kid, is_root=kf["is_root"], kp_landmark=kl, depth=kf["depth"], depth_thr=kf["depth_thr"]))
+    off, o_rank, o_oct, o_w = [0], [], [], []
+    for li in rows:
+        for kid, idx in landmarks[li]["observations"].items():
+            kf = keyframes[kid]
+            o_rank.append(rank.get(kid, -1))
+            o_oct.append(int(kf["octave"][idx]))
+            o_w.append(2 if kf["x_right"] is not None and 0 <= kf["x_right"][idx] else 1)
+        off.append(len(o_rank))
+    return dict(cur_id=cull_map["cur_id"], redundant_obs_ratio_thr=redundant_obs_ratio_thr, covisibilities=out_covs,
+                obs_offsets=np.array(off, np.int32), obs_rank=np.array(o_rank, np.int32), obs_octave=np.array(o_oct, np.int32),
+                obs_weight=np.array(o_w, np.uint8))
