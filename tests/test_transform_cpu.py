@@ -9,44 +9,12 @@ import scipy.linalg as sl
 import scipy.optimize as so
 
 import transform_oracle as O
+import transform_reference as TR
 import test_abi_layout as ABI
 from workloads import synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MODELS = [("perspective", "perspective"), ("equirect", "equirect"), ("perspective", "equirect")]
-
-
-def _hat(u):
-    w, v, s = u[:3], u[3:6], u[6]
-    M = np.zeros((4, 4))
-    M[:3, :3] = np.array([[0, -w[2], w[1]], [w[2], 0, -w[0]], [-w[1], w[0], 0]]) + s * np.eye(3)
-    M[:3, 3] = v
-    return M
-
-
-def _mat(g):
-    """4x4 similarity [s R | t] of a Sim3 8-vector."""
-    x, y, z, w = g[:4]
-    R = np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
-                  [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
-                  [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
-    M = np.eye(4)
-    M[:3, :3] = g[7] * R
-    M[:3, 3] = g[4:7]
-    return M
-
-
-def _project(cam, p):
-    if cam["model"] == 1:
-        th, ph = np.arctan2(p[0], p[2]), -np.arcsin(p[1] / np.linalg.norm(p))
-        return np.array([cam["cols"] * (0.5 + th / (2 * np.pi)), cam["rows"] * (0.5 - ph / np.pi)])
-    return np.array([cam["fx"] * p[0] / p[2] + cam["cx"], cam["fy"] * p[1] / p[2] + cam["cy"]])
-
-
-def _np_error(M12, side, pc, cam, obs):
-    """numpy restatement of forward_reproj_edge / backward_reproj_edge::computeError with the Sim3 as a 4x4 matrix."""
-    M = M12 if side == 0 else np.linalg.inv(M12)
-    return np.asarray(obs, np.float64) - _project(cam, (M @ np.append(pc, 1.0))[:3])
 
 
 def _edges(pr):
@@ -61,11 +29,11 @@ def _edges(pr):
 @pytest.mark.parametrize("models", MODELS)
 def test_edge_errors_match_numpy(models):
     pr = synth.make_sim3_pair(3, 40, models=models, outlier_frac=0.2)
-    M = _mat(pr["sim3_12"])
+    M = TR.mat(pr["sim3_12"])
     for side, pc, cam, obs, w in _edges(pr):
         e, chi = O.transform_edge(pr["sim3_12"], side, pc, cam, obs, w)
-        want = _np_error(M, side, pc, cam, obs)
-        np.testing.assert_allclose(e, want, rtol=0, atol=1e-9 * max(1.0, np.abs(_project(cam, pc)).max()))
+        want = TR.np_error(M, side, pc, cam, obs)
+        np.testing.assert_allclose(e, want, rtol=0, atol=1e-9 * max(1.0, np.abs(TR.project(cam, pc)).max()))
         assert chi == pytest.approx(float(w) * (e @ e), rel=1e-14)
 
 
@@ -80,8 +48,8 @@ def test_numeric_jacobian_matches_independent_difference(models, fix_scale):
         for d in range(6 if fix_scale else 7):
             du = np.zeros(7)
             du[d] = 1e-6
-            fp = _np_error(sl.expm(_hat(du)) @ _mat(S), side, pc, cam, obs)
-            fm = _np_error(sl.expm(_hat(-du)) @ _mat(S), side, pc, cam, obs)
+            fp = TR.np_error(sl.expm(TR.hat(du)) @ TR.mat(S), side, pc, cam, obs)
+            fm = TR.np_error(sl.expm(TR.hat(-du)) @ TR.mat(S), side, pc, cam, obs)
             Jr[:, d] = (fp - fm) / 2e-6
         np.testing.assert_allclose(J, Jr, rtol=0, atol=2e-4 * max(1.0, np.abs(Jr).max()))
         if fix_scale:
@@ -94,24 +62,24 @@ def test_lm_optimum_matches_least_squares(models):
     pr = synth.make_sim3_pair(5, 60, models=models, outlier_frac=0.0, pixel_sigma=0.2)
     ref = O.transform_optimize(pr, 10.0, num_iter=50)
     assert ref["n_outliers_round1"] == 0 and ref["num_inliers"] == 60
-    S0 = _mat(pr["sim3_12"])
+    S0 = TR.mat(pr["sim3_12"])
     edges = _edges(pr)
 
     def resid(u):
-        M = sl.expm(_hat(u)) @ S0
-        return np.concatenate([np.sqrt(float(w)) * _np_error(M, side, pc, cam, obs) for side, pc, cam, obs, w in edges])
+        M = sl.expm(TR.hat(u)) @ S0
+        return np.concatenate([np.sqrt(float(w)) * TR.np_error(M, side, pc, cam, obs) for side, pc, cam, obs, w in edges])
 
     sol = so.least_squares(resid, np.zeros(7), xtol=1e-15, ftol=1e-15, gtol=1e-15, method="lm")
     assert 2 * sol.cost < 10.0 * len(edges) * 0.1          # well inside the Huber zone on average
     assert max(float(w) * (r @ r) for (_, _, _, _, w), r in zip(edges, resid(sol.x).reshape(-1, 2))) < 10.0
-    want = sl.expm(_hat(sol.x)) @ S0
-    np.testing.assert_allclose(_mat(ref["sim3_12"]), want, rtol=0, atol=1e-6 * max(1.0, np.abs(want).max()))
+    want = sl.expm(TR.hat(sol.x)) @ S0
+    np.testing.assert_allclose(TR.mat(ref["sim3_12"]), want, rtol=0, atol=1e-6 * max(1.0, np.abs(want).max()))
 
 
 def _noise_free(pr):
     """Points back-projected from the (float) observations through the true Sim3, so every edge's error at the truth is rounding."""
     pr = dict(pr)
-    gt = _mat(pr["gt_sim3_12"])
+    gt = TR.mat(pr["gt_sim3_12"])
     for side, obs_key, pos_key, cam_key, R_key, t_key, M in ((0, "obs_1", "pos_w_2", "cam_1", "rot_2w", "trans_2w", np.linalg.inv(gt)),
                                                              (1, "obs_2", "pos_w_1", "cam_2", "rot_1w", "trans_1w", gt)):
         cam = pr[cam_key]
